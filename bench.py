@@ -8,11 +8,13 @@ camera moves around a 64-view ring, one new view per step and rank).  `value` is
 all inputs resident in HBM; `e2e` goes through the public drop-in API (GaussianRasterizer + autograd) with the
 step's host inputs (camera + ground-truth image) copied from pinned memory and the loss read back every step.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C3]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C3] [--dump-outputs DIR]
 
---impl reference times the UNMODIFIED reference extension (oracle/_ref, built from /root/reference for sm_100a by
+--impl reference times the UNMODIFIED reference extension (oracle/_ref, built from the original project for sm_90a by
 oracle/build_ref.sh) on the same GPU through its own entry points; if that build is absent it times the CPU
 restatement of the reference (oracle/) on a bounded sample and says so in `cpu_baseline.kind`.
+--dump-outputs DIR writes what the last timed step computed as DIR/<name>.npy (see dump_outputs), so that two builds
+can be compared output for output on identical, seeded inputs.
 """
 import argparse
 import json
@@ -36,7 +38,7 @@ import gof_synth  # noqa: E402
 
 # --------------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md): one streaming
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region: one streaming
     `nvidia-smi -lms 50` process whose lines are collected by this thread."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -164,24 +166,36 @@ def bwd_args(fa, radii, geom, R, binning, img, grad):
             campos, geom, R, binning, img, dbg)
 
 
-NCU_SUMMARY = "profiles/r2_ncu_render_call7.txt"      # ncu --set full of the shipped kernels at C3 (sections "Kernel Name ...")
+DUMP_ROWS = 65536
+DUMP_LIMIT = 64 << 20
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of `kernel` ("render_fwd" / "render_bwd") at the C3 workload,
-    from the committed `ncu --set full` summary; None if the file or the kernel's section is missing."""
-    want = {"render_bwd": "k_render_backward", "render_fwd": "k_render_forward"}.get(kernel, kernel)
-    try:
-        tot, inside = 0.0, False
-        for ln in open(os.path.join(ROOT, NCU_SUMMARY)):
-            f = ln.split()
-            if ln.startswith("Kernel Name"):
-                inside = want in ln
-            elif inside and len(f) >= 3 and f[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                tot += float(f[1]) * {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[f[2]]
-        return tot or None
-    except Exception:
-        return None
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy, float32 (float64 stays float64).  An array with more than DUMP_ROWS rows is cut
+    to a fixed sample of its rows, seeded by the row count, so that arrays of the same length are sampled alike and two
+    builds run with the same arguments write comparable files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        t = t.detach().reshape(1) if t.dim() == 0 else t.detach()
+        n = t.shape[0]
+        if n > DUMP_ROWS:
+            idx = np.sort(np.random.default_rng(n).choice(n, DUMP_ROWS, replace=False))
+            t = t.index_select(0, torch.from_numpy(idx).to(t.device))
+        a = t.cpu().numpy()
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        total += a.nbytes
+        assert total <= DUMP_LIMIT, f"--dump-outputs: more than {DUMP_LIMIT >> 20} MB"
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+def image_rows(img):
+    """(C, H, W) -> (H*W, C): rows are pixels, so that dump_outputs samples pixels."""
+    return img.permute(1, 2, 0).reshape(-1, img.shape[0])
+
+
+GRAD_NAMES = ("dmeans2D", "dcolors", "dopacity", "dmeans3D", "dcov3D", "dsh", "dscales", "drot", "dview2gaussian")
 
 
 def algorithmic_bytes(P, V, R, N):
@@ -378,7 +392,7 @@ def run_ours(args, rank, world, dev):
         grads = _C.rasterize_gaussians_backward(*bwd_args(fa, radii, geom, R, binning, img, dL), _out=bucket.views)
         if world > 1:
             bucket.all_reduce()      # gradients (SUM) and this step's densification statistics (SUM | MAX tail) in ONE exchange
-        return color
+        return color, radii, grads
 
     # ---- kernel-path throughput: inputs resident in HBM, CUDA events, max over ranks --------------------------
     for s in range(args.warmup):
@@ -430,12 +444,18 @@ def run_ours(args, rank, world, dev):
     barrier_sync(world)
     e0.record()
     for s in range(args.steps):
-        step_device(args.warmup + s)
+        out = step_device(args.warmup + s)
+        last = out if args.dump_outputs and s == args.steps - 1 else None      # only the dumped step's outputs outlive it
+        del out
     e1.record()
     barrier_sync(world)
     clocks = sampler.stop()
     ms = max_over_ranks(e0.elapsed_time(e1), world, dev)
     launches = _C.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        color, radii, grads = last
+        dump_outputs(args.dump_outputs, {"color": image_rows(color), "radii": radii, **dict(zip(GRAD_NAMES, grads))})
+    del last
     # per-kernel durations: a separate short pass with the library's CUDA-event brackets around every launch
     # (kept out of the timed region above: the brackets add host work between launches)
     prof_steps = min(args.steps, 5)
@@ -486,7 +506,7 @@ def run_ours(args, rank, world, dev):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     dom = max(("render_bwd", "render_fwd"), key=lambda k: prof.get(k, (0, 0.0))[1])
     dom_cnt, dom_ms = prof.get(dom, (1, 0.0))
     dom_bytes = bwd_bytes if dom == "render_bwd" else fwd_bytes
@@ -499,16 +519,15 @@ def run_ours(args, rank, world, dev):
         "config": {"workload": WORKLOAD_FMT.format(cfg=args.config, P=wl.P, W=wl.W, H=wl.H, seed=wl.cfg["seed"]) + (APPEARANCE_NOTE if app else ""),
                    "visible": V, "num_rendered": R, "stats_view": stats_view, **tile_stats,
                    "parallelism": f"view-parallel dp{world}" if world > 1 else "single GPU",
-                   "l2": "no explicit flush: a step touches >400 MB (> 126 MB L2) and every step renders a new view"},
+                   "l2": "no explicit flush: a step touches >400 MB (> 50 MB L2) and every step renders a new view"},
         "e2e": {"value": world * args.steps / (e2e_ms * 1e-3), "unit": "views/s", "h2d_bytes_per_step": h2d,
                 "d2h_bytes_per_step": 4, "ms_per_step": e2e_ms / args.steps,
                 "api": E2E_API},
         "gpu_launches": int(launches),
         "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": (achieved / peak) if achieved else None, "traffic": ncu_traffic(dom),
-                     "traffic_source": f"{NCU_SUMMARY} (ncu --set full, C3 workload, per launch)",
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                     "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet, 3350 GB/s HBM3",
                      "algorithmic_bytes_per_launch": dom_bytes, "launch_ms": dom_ms / max(dom_cnt, 1),
                      "step_algorithmic_bytes": step_bytes,
                      "step_frac": step_bytes / ((ms / args.steps) * 1e-3) / 1e9 / peak},
@@ -654,6 +673,7 @@ def run_reference(args, rank, world, dev):
         if world > 1:
             flat = torch.cat([grads[i].flatten() for i in (3, 5, 2, 6, 7)] + ([app_flat] if app else []))
             dist.all_reduce(flat)
+        return color, radii, grads
 
     for s in range(args.warmup):
         step_device(s)
@@ -663,11 +683,17 @@ def run_reference(args, rank, world, dev):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for s in range(args.steps):
-        step_device(args.warmup + s)
+        out = step_device(args.warmup + s)
+        last = out if args.dump_outputs and s == args.steps - 1 else None      # only the dumped step's outputs outlive it
+        del out
     e1.record()
     barrier_sync(world)
     clocks = sampler.stop()
     ms = max_over_ranks(e0.elapsed_time(e1), world, dev)
+    if args.dump_outputs and rank == 0:      # per-rank gradients: the reference arm's exchange sums a copy
+        color, radii, grads = last
+        dump_outputs(args.dump_outputs, {"color": image_rows(color), "radii": radii, **dict(zip(GRAD_NAMES, grads))})
+    del last
 
     # end to end: the SAME harness as our arm, driving the reference's own public API -- its unmodified Python package
     # (autograd Function + GaussianRasterizer module, staged by baseline/stage_ref.sh) on top of its compiled extension
@@ -688,10 +714,10 @@ def run_reference(args, rank, world, dev):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD_FMT.format(cfg=args.config, P=wl.P, W=wl.W, H=wl.H, seed=wl.cfg["seed"]) + (APPEARANCE_NOTE if app else ""),
                    "visible": int((st["radii"] > 0).sum()), "num_rendered": int(st["R"]), "stats_view": stats_view,
-                   "reference": "unmodified diff-gaussian-rasterization of GOF compiled for sm_100a (oracle/build_ref.sh), on the GPU"},
+                   "reference": "unmodified diff-gaussian-rasterization of GOF compiled for sm_90a (oracle/build_ref.sh), on the GPU"},
         "cpu_baseline": {"kind": "reference", "cores": 0, "value": world * args.steps / (ms * 1e-3), "unit": "views/s",
                          "sample": "the reference has no CPU path (rasterize_points.cu:75-79 allocates CUDA tensors); this arm "
-                                   "runs its own CUDA kernels on the same B200"},
+                                   "runs its own CUDA kernels on the same GPU"},
         "e2e": {"value": world * args.steps / (e2e_ms * 1e-3), "unit": "views/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                 "ms_per_step": e2e_ms / args.steps, "api": E2E_API + "; " + api_note},
         "clocks": clocks,
@@ -699,7 +725,7 @@ def run_reference(args, rank, world, dev):
 
 
 # ==============================================================================================================
-# Config C5: opacity-field mesh extraction (BASELINE.json configs[4]): 3 M Gaussians, 50 M query points, 64 views
+# Config C5: opacity-field mesh extraction (BASELINE.json configs[4]): 3 M Gaussians, 27 M query points, 64 views
 # ==============================================================================================================
 EXTRACT_METRIC = "opacity-field query points/sec (integrate, one 1080p view per step) over 3M Gaussians"
 EXTRACT_WORKLOAD_FMT = ("{cfg}: {P} Gaussians, {PN} query points (9 per Gaussian like get_tetra_points + samples in the 3-sigma boxes), "
@@ -798,12 +824,17 @@ def run_extract_ours(args, rank, world, dev):
     barrier_sync(world)
     e0.record()
     for s in range(args.steps):
-        step_device(args.warmup + s)
+        out = step_device(args.warmup + s)
+        last = out if args.dump_outputs and s == args.steps - 1 else None      # only the dumped step's outputs outlive it
+        del out
     e1.record()
     barrier_sync(world)
     clocks = sampler.stop()
     ms = max_over_ranks(e0.elapsed_time(e1), world, dev)
     launches = _C.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(zip(("alpha_integrated", "color_integrated"), last)))
+    del last
     prof_steps = min(args.steps, 3)
     _C.profile_reset(); _C.profile_enable(True)
     for s in range(prof_steps):
@@ -848,7 +879,7 @@ def run_extract_ours(args, rank, world, dev):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     # SURVEY 8(d), extraction: the query kernel gathers 72 B per tile instance (records of the tile lists), reads 16 B and writes
     # 16 B per projected point, writes the 9-channel image; the point side in front of it reads 12 B/point and writes 24 B/projected point
     k_bytes = 72 * Rg + 32 * PNv + 36 * N
@@ -864,7 +895,7 @@ def run_extract_ours(args, rank, world, dev):
                    "parallelism": f"view-parallel dp{world}" if world > 1 else "single GPU",
                    "gaussian_side": f"prepared once per view and cached ({prepare_ms:.2f} ms/view, outside the timed steps; the e2e "
                                     f"number below repeats it every step like the reference)",
-                   "l2": "no explicit flush: a step streams the 50 M points (> 1 GB, > 126 MB L2) and every step is a new view"},
+                   "l2": "no explicit flush: a step streams the 27 M points (> 0.5 GB, > 50 MB L2) and every step is a new view"},
         "e2e": {"value": world * args.steps * wl.PN / (e2e_ms * 1e-3), "unit": "points/s", "h2d_bytes_per_step": 35 * 4,
                 "d2h_bytes_per_step": 4, "ms_per_step": e2e_ms / args.steps,
                 "api": "GaussianRasterizer(settings).integrate(points3D=...) incl. the Gaussian side; camera from pinned host memory every "
@@ -872,7 +903,7 @@ def run_extract_ours(args, rank, world, dev):
         "gpu_launches": int(launches), "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": "integrate", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": (achieved / peak) if achieved else None, "traffic": None,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet, 3350 GB/s HBM3",
                      "algorithmic_bytes_per_launch": k_bytes, "launch_ms": k_ms / max(cnt, 1), "step_algorithmic_bytes": view_bytes,
                      "step_frac": view_bytes / ((ms / args.steps) * 1e-3) / 1e9 / peak},
         "kernels_ms_per_step": {k: v[1] / prof_steps for k, v in sorted(prof.items(), key=lambda kv: -kv[1][1])},
@@ -940,7 +971,7 @@ def run_extract_reference(args, rank, world, dev):
     ref = _util.load_ref()
     pkg = _refpy.ref_rasterizer_package()
     if ref is None or pkg is None:
-        return {"impl": "reference", "unavailable": "reference extension / staged Python not built here (needs /root/reference at build time)"}
+        return {"impl": "reference", "unavailable": "reference extension / staged Python not built here (needs the original project at build time)"}
     wl = ExtractWorkload(args, dev, rank, world)
     g = wl.gs
     e = torch.Tensor([])
@@ -959,11 +990,16 @@ def run_extract_reference(args, rank, world, dev):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for s in range(args.steps):
-        step_device(args.warmup + s)
+        out = step_device(args.warmup + s)
+        last = out if args.dump_outputs and s == args.steps - 1 else None      # only the dumped step's outputs outlive it
+        del out
     e1.record()
     barrier_sync(world)
     clocks = sampler.stop()
     ms = max_over_ranks(e0.elapsed_time(e1), world, dev)
+    if args.dump_outputs and rank == 0:      # (num_rendered, out_color, alpha_integrated, color_integrated, ...)
+        dump_outputs(args.dump_outputs, {"alpha_integrated": last[2], "color_integrated": last[3]})
+    del last
     sv = wl.view(args.warmup)
     o = step_device(args.warmup)
     Rg, PNv, Vg = int(o[0]), int(o[1][8].sum().item()), int((o[4] > 0).sum())
@@ -976,9 +1012,9 @@ def run_extract_reference(args, rank, world, dev):
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": EXTRACT_WORKLOAD_FMT.format(cfg=args.config, P=wl.P, PN=wl.PN, W=wl.W, H=wl.H, nv=wl.n_views),
                    "stats_view": sv, "visible": Vg, "num_rendered": Rg, "points_projected": PNv,
-                   "reference": "unmodified diff-gaussian-rasterization of GOF compiled for sm_100a (oracle/build_ref.sh), on the GPU"},
+                   "reference": "unmodified diff-gaussian-rasterization of GOF compiled for sm_90a (oracle/build_ref.sh), on the GPU"},
         "cpu_baseline": {"kind": "reference", "cores": 0, "value": val, "unit": "points/s",
-                         "sample": "the reference has no CPU path; this arm runs its own CUDA kernels on the same B200"},
+                         "sample": "the reference has no CPU path; this arm runs its own CUDA kernels on the same GPU"},
         "e2e": {"value": world * args.steps * wl.PN / (e2e_ms * 1e-3), "unit": "points/s", "h2d_bytes_per_step": 35 * 4,
                 "d2h_bytes_per_step": 4, "ms_per_step": e2e_ms / args.steps,
                 "api": "reference's own GaussianRasterizer(settings).integrate; same harness as our arm (bench.extract_e2e)"},
@@ -1025,7 +1061,7 @@ def run_train_step(args, rank, world, dev):
         pkg = _refpy.ref_rasterizer_package()
         lu, du = _refpy.ref_utils("loss_utils"), _refpy.ref_utils("depth_utils")
         if pkg is None or lu is None or du is None:
-            return {"impl": "reference", "unavailable": "reference extension / staged Python not built here (needs /root/reference at build time)"}
+            return {"impl": "reference", "unavailable": "reference extension / staged Python not built here (needs the original project at build time)"}
         GaussianRasterizer, GaussianRasterizationSettings = pkg.GaussianRasterizer, pkg.GaussianRasterizationSettings
         opt = torch.optim.Adam([{"params": [v], "lr": _LRS[k]} for k, v in raw.items()], lr=0.0, eps=1e-15)
     it = [0]
@@ -1108,6 +1144,8 @@ def run_train_step(args, rank, world, dev):
     clocks = sampler.stop()
     ms = max_over_ranks(e0.elapsed_time(e1), world, dev)
     final = float(loss_pin[0])
+    if args.dump_outputs and rank == 0:      # the parameters after the last step's update, and that step's loss
+        dump_outputs(args.dump_outputs, {"loss": loss_pin.clone(), **{k.lstrip("_"): v for k, v in raw.items()}})
     assert math.isfinite(final)
     h2d = 35 * 4 + wl.gt_host.numel() * 4
     line = {"metric": TRAIN_METRIC, "value": world * args.steps / (ms * 1e-3), "unit": "iterations/s", "n_gpus": world, "steps": args.steps,
@@ -1124,7 +1162,7 @@ def run_train_step(args, rank, world, dev):
     if not ours:
         line["impl"] = "reference"
         line["cpu_baseline"] = {"kind": "reference", "cores": 0, "value": line["value"], "unit": "iterations/s",
-                                "sample": "the reference has no CPU path; this arm runs its own CUDA kernels + torch on the same B200"}
+                                "sample": "the reference has no CPU path; this arm runs its own CUDA kernels + torch on the same GPU"}
     else:
         line["gpu_launches"] = int(_C.launch_count() - launches0)
     return line
@@ -1133,14 +1171,14 @@ def run_train_step(args, rank, world, dev):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 50; 16 for the extraction config C5)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="C3", choices=sorted(gof_synth.CONFIGS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--mode", default="raster", choices=["raster", "train_step"],
                     help="raster (default): the rasterizer fwd+bwd step of BASELINE.json; train_step: a whole training iteration around it")
-    ap.add_argument("--points", type=int, default=0, help="C5: number of query points (default: the config's 50 M)")
+    ap.add_argument("--points", type=int, default=0, help="C5: number of query points (default: the config's 27 M)")
     ap.add_argument("--views", type=int, default=0, help="C5: number of views on the ring (default 64)")
     ap.add_argument("--tets", type=int, default=0, help="C5: number of tetrahedra of the pipeline run (default 6.5 per point)")
     ap.add_argument("--no-pipeline", action="store_true", help="C5: skip the one full extraction run (evaluate_alpha + marching tets + bisection)")
@@ -1148,12 +1186,15 @@ def main():
                     help="N>1 gradient exchange: the library's multimem kernel through the NVSwitch (nvls), its NVLink peer-memory kernel "
                          "(p2p), NCCL's all-reduce (nccl), or auto = nvls, else p2p, else nccl -- each mode is adopted only after a "
                          "collective self-test on the live mapping")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float32, a seeded sample of "
+                         "rows where an output is larger; at most 64 MB in all)")
     ap.add_argument("--no-factor-sh", action="store_true", help="N>1: exchange the full dL_dsh (64 floats per Gaussian in the bucket) instead of "
                                                                "the per-view dL_dRGB records (16 reduced + 3 per view)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device: the B200 rasterizer has no CPU path")
+        raise SystemExit("bench.py needs a CUDA device: the rasterizer has no CPU path")
     # keep stdout clean for the ONE JSON line (NCCL prints its version banner to stdout): everything else -> stderr
     sys.stdout.flush()
     saved_stdout = os.dup(1)
@@ -1161,8 +1202,8 @@ def main():
     rank, world, local = dist_setup(args.gpus)
     dev = torch.device("cuda", local if world > 1 else 0)
     extract = "points" in gof_synth.CONFIGS[args.config]
-    if extract and args.steps == 50:
-        args.steps = 16          # a step is a 50 M-point query: keep the default run within minutes
+    if args.steps is None:
+        args.steps = 16 if extract else 50          # a C5 step is a 27 M-point query: keep the default run within minutes
     if args.mode == "train_step" and not extract:
         line = run_train_step(args, rank, world, dev)
     elif extract:

@@ -1,8 +1,7 @@
-"""Builds libgof_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libgof_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 No torch headers, no pybind: plain `nvcc -shared`.  The .so lands next to the Python package
-(gaussian-opacity-fields_b200/diff_gaussian_rasterization/libgof_b200.so), is git-ignored and travels
-to the GPU box with the repo snapshot.
+(gaussian-opacity-fields_b200/diff_gaussian_rasterization/libgof_b200.so), is git-ignored.
 """
 import os
 import subprocess
@@ -15,7 +14,7 @@ OUT_DIR = os.path.join(HERE, "diff_gaussian_rasterization")
 LIB = os.path.join(OUT_DIR, "libgof_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "binning_legacy.cu", "render_fwd.cu", "render_bwd.cu", "integrate.cu", "tetmesh.cu", "exchange.cu", "view_loss.cu", "param_ops.cu", "filter3d.cu", "densify.cu", "conv_wgrad.cu", "sh_views.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
 ]
 
@@ -61,7 +60,7 @@ def build(force=False, verbose=True):
     if failed:
         sys.stderr.write("\n".join(log))
         raise RuntimeError("nvcc failed building libgof_b200.so")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     subprocess.check_call(cmd)
     with open(stamp, "w") as f:
         f.write(digest)

@@ -468,7 +468,7 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count <= 0) sm_count = 148;
+    if (sm_count <= 0) sm_count = 132;
   }
   const GofPointLayout PL = gof_point_layout((size_t)PN);
   const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, sm_count);
@@ -492,7 +492,7 @@ static int int_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count <= 0) sm_count = 148;
+    if (sm_count <= 0) sm_count = 132;
   }
   return sm_count;
 }

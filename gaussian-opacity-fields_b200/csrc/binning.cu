@@ -331,7 +331,7 @@ int onesweep_passes(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, size_t n, co
 
 int sm_count() {
   static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
   return sms;
 }
 

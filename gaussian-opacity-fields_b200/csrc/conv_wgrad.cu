@@ -1,8 +1,8 @@
 // conv_wgrad.cu -- weight and bias gradient of a 3x3, stride-1, pad-1 convolution with few channels at full image resolution:
 // the two convolutions at the tail of the reference's AppearanceNetwork (scene/appearance_network.py:28-29, 16 -> 16 and 16 -> 3
 // channels at 1056x1920 in BASELINE config C4) and its last upsample block (8 -> 16 at half resolution).  Why hand-written:
-// profiled on B200 (profiles/r2_appearance_profile_cudnn.txt), cuDNN answers these shapes with its generic fp32
-// `wgrad_alg0_engine` -- 2.1 ms of the 5.2 ms appearance step, more than the whole forward of the network.
+// cuDNN answers these shapes with its generic fp32 `wgrad_alg0_engine`, which takes longer than the whole forward of the
+// network.
 //
 // dW[co][ci][ky][kx] = sum_p gy[co][p] * x[ci][p + (ky-1, kx-1)] is a reduction over two million pixels into at most 2304
 // numbers.  One thread owns COPT (co, ci) pairs and keeps their nine sums each in registers; persistent CTAs sweep 32x8 pixel
@@ -186,7 +186,7 @@ int launch_v(const float* x, const float* gy, int H, int W, float* dW, float* db
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     GOF_CUDA_OK(cudaFuncSetAttribute(k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE>, THREADS, SMEM) != cudaSuccess || per_sm < 1)
       per_sm = 1;

@@ -160,7 +160,7 @@ extern "C" GOF_API int gof_densify_plan(int P, const float* accum, const float* 
     gof_set_error("densify_plan: NULL argument");
     return GOF_E_INVALID;
   }
-  PlanArgs a;
+  PlanArgs a{};
   a.P = P; a.accum = accum; a.accum_abs = accum_abs; a.denom = denom; a.scaling = scaling_raw; a.opacity = opacity_raw;
   a.max_grad = max_grad; a.abs_threshold = abs_threshold; a.dense_extent = dense_extent; a.min_opacity = min_opacity;
   a.prune_scale = prune_scale; a.flags = flags;
@@ -184,7 +184,7 @@ extern "C" GOF_API int gof_densify_emit(int P, const uint32_t* flags, const uint
     gof_set_error("densify_emit: NULL argument");
     return GOF_E_INVALID;
   }
-  EmitArgs a;
+  EmitArgs a{};
   a.P = P; a.flags = flags; a.offsets = offsets;
   uint32_t b = 0;
   for (int k = 0; k < 4; ++k) { a.base[k] = b; b += totals_host[k]; }

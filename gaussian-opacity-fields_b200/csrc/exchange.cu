@@ -195,7 +195,7 @@ extern "C" GOF_API int gof_p2p_allreduce_sum_f32(float* const* peers, int world,
 
 static unsigned exchange_grid(size_t items) {
   static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
   const size_t want = (items + 511) / 512;
   return (unsigned)(want < (size_t)sms * 4 ? want : (size_t)sms * 4);
 }

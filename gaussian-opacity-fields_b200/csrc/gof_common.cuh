@@ -57,7 +57,7 @@ int gof_read_back(void* dst, const void* src_dev, size_t bytes, cudaStream_t st)
 unsigned long long* gof_stats_buffer();
 
 // ---- shared-memory access with an explicit base register ----------------------------------------------
-// On sm_100 a shared address carries the CTA's rank in its cluster; ptxas re-derives that window base
+// On sm_90 and later a shared address carries the CTA's rank in its cluster; ptxas re-derives that window base
 // (S2UR SR_CgaCtaId + UMOV + ULEA) next to every dynamically indexed access when registers are tight, which was
 // 5-8 issue slots per visited Gaussian in the blend kernels.  gof_smem_base() turns the base into an opaque
 // register value once; gof_lds* then compile to a bare LDS [R + imm].
@@ -192,7 +192,7 @@ struct GofGeomLayout {      // "geomBuffer": everything sized by P
   size_t hist;                         // radix sort scratch (gof_sort_scratch_bytes)
   size_t scan_tmp;                     // scan block sums / look-back status words
   size_t total;                        // u32 num_rendered (device copy)
-  size_t grad_acc;                     // float[P][16]: backward accumulators of the blend kernel (dv2g[10], dcolor[3], dmean2D[3])
+  size_t grad_acc;                     // double[P][16]: backward accumulators of the blend kernel (dv2g[10], dcolor[3], dmean2D[3])
   size_t reject_k;                     // float[P]: K' = (C + 2 thr)(1 - 4e-7), thr = -ln(255 opacity) - 2e-3: a pair with (B/2)^2 < A K' has alpha < 1/255
   size_t bytes;
 };
@@ -215,7 +215,7 @@ static inline GofGeomLayout gof_geom_layout(size_t P) {
   L.hist = take(gof_sort_scratch_bytes(P));
   L.scan_tmp = take((P / 256 + 8) * 4 + 4096);      // look-back status words of the fused scan+emit kernel (one per 256 Gaussians) + ticket
   L.total = take(256);
-  L.grad_acc = take(P * 64);
+  L.grad_acc = take(P * 128);
   L.reject_k = take(P * 4);
   L.bytes = o;
   return L;

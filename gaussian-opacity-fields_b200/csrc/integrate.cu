@@ -308,7 +308,7 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
                          const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, float* out_color, float* out_alpha,
                          float* out_color_int, cudaStream_t st) {
   const bool debug = s->debug != 0;
-  PtArgs pa;
+  PtArgs pa{};
   pa.PN = PN; pa.W = v.W; pa.H = v.H; pa.grid_x = v.grid_x; pa.grid_y = v.grid_y; pa.tiles = v.tiles;
   pa.focal_x = v.focal_x; pa.focal_y = v.focal_y; pa.points3D = points3D; pa.vm = s->viewmatrix;
   pa.xy = reinterpret_cast<float2*>(pts + PL.xy); pa.depth = reinterpret_cast<float*>(pts + PL.depth);
@@ -326,7 +326,7 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
                                    reinterpret_cast<uint32_t*>(pbin + PBL.hist), pranges, v.tiles, debug, st, &in_b);
   if (rc != GOF_OK) return rc;
 
-  IntArgs a;
+  IntArgs a{};
   a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.tiles = v.tiles; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
   a.ranges = ranges;
   a.point_list = point_list;

@@ -226,7 +226,7 @@ struct PreBwdArgs {
   const float* rotations;
   const float* viewmatrix;
   const float* cam_pos;
-  const float4* grad_acc;   // [P][4] float4: the blend kernel's accumulator rows (dv2g[10] | dcolor[3] | dmean2D[3])
+  const double2* grad_acc;  // [P][8] double2: the blend kernel's accumulator rows (dv2g[10] | dcolor[3] | dmean2D[3])
   const GofSplat* splat;    // for the effective opacity (dL_dopacity = -2/opacity * dL_dC)
   float* dL_dmean2D;        // outputs unpacked from the accumulator row
   float* dL_dopacity;
@@ -315,10 +315,14 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
   }
 
   if (active) {
-  // the blend kernel's 64-byte accumulator row -> the public gradient tensors
-  const float4 g0 = a.grad_acc[4 * (size_t)idx], g1 = a.grad_acc[4 * (size_t)idx + 1], g2 = a.grad_acc[4 * (size_t)idx + 2],
-               g3 = a.grad_acc[4 * (size_t)idx + 3];
-  const float accv[16] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w, g2.x, g2.y, g2.z, g2.w, g3.x, g3.y, g3.z, g3.w};
+  // the blend kernel's accumulator row -> the public gradient tensors (the double sums rounded once to float)
+  float accv[16];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const double2 g = a.grad_acc[8 * (size_t)idx + k];
+    accv[2 * k] = (float)g.x;
+    accv[2 * k + 1] = (float)g.y;
+  }
   {
     float* dv = a.dL_dv2g + 10 * (size_t)idx;
 #pragma unroll
@@ -573,7 +577,7 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
 
 int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& L,
                           int* radii, cudaStream_t st) {
-  PreArgs a;
+  PreArgs a{};
   a.P = s->P; a.D = s->D; a.M = s->M; a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.grid_y = v.grid_y;
   a.tan_fovx = s->tan_fovx; a.tan_fovy = s->tan_fovy; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
   a.kernel_size = s->kernel_size; a.scale_modifier = s->scale_modifier;
@@ -609,12 +613,12 @@ int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const
                                    float* dL_drot, float* dL_dcov3D, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
                                    cudaStream_t st) {
   (void)v;
-  PreBwdArgs a;
+  PreBwdArgs a{};
   a.P = s->P; a.D = s->D; a.M = s->M;
   a.means3D = s->means3D; a.radii = radii; a.shs = s->shs;
   a.clamped = reinterpret_cast<const unsigned char*>(geom + L.clamped);
   a.scales = s->scales; a.rotations = s->rotations; a.viewmatrix = s->viewmatrix; a.cam_pos = s->cam_pos;
-  a.grad_acc = reinterpret_cast<const float4*>(geom + L.grad_acc);
+  a.grad_acc = reinterpret_cast<const double2*>(geom + L.grad_acc);
   a.splat = reinterpret_cast<const GofSplat*>(geom + L.splat);
   a.dL_dmean2D = dL_dmean2D; a.dL_dopacity = dL_dopacity;
   a.dL_dcolor = dL_dcolor; a.dL_dv2g = dL_dv2g; a.dL_dmean3D = dL_dmean3D; a.dL_dsh = dL_dsh;

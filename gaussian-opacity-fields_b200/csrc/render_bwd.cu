@@ -3,7 +3,7 @@
 // The reference issues 17 global float atomics per contributing (pixel,Gaussian) pair
 // (backward.cu:836,905-912,943-952).  Here a warp owns an 8x4 pixel block; the partial gradients of its 32
 // pixels are summed with a 16-shuffle butterfly (dL_dopacity is -2/opacity * dL_dC, so 16 values carry all
-// 17 outputs) and leave the SM as 16 atomics per (warp,Gaussian) into that Gaussian's 64-byte accumulator row.
+// 17 outputs) and leave the SM as 16 atomics per (warp,Gaussian) into that Gaussian's accumulator row (16 doubles).
 // The forward leaves, per (warp, tile-list entry), the mask of pixels that blended it (GofBinLayout::vmask): the
 // backward visits exactly those (no box test, no reject arithmetic -- 44 % of the forward's visits blend nothing),
 // re-evaluating t, G and alpha with the forward's operation sequence (gof_math.cuh) so that they are bit-identical.
@@ -32,7 +32,11 @@ struct BwdArgs {
   size_t plane;
   const uint32_t* vmask;   // blend masks left by the forward (GofBinLayout::vmask)
   size_t vstride;
-  float* grad_acc;     // [P][16]: dL_dview2gaussian[10] | dL_dcolor[3] | dL_dmean2D[3] (64-byte rows, zeroed per call)
+  double* grad_acc;    // [P][16]: dL_dview2gaussian[10] | dL_dcolor[3] | dL_dmean2D[3] (128-byte rows, zeroed per call).  Double:
+                       // the float partials arrive in scheduling order.  A float sum differs from run to run by ulps, which
+                       // the view2gaussian chain rule amplifies to percents in dL_dscale / dL_drot; the order moves a double
+                       // sum only in its last bits, so after k_preprocess_backward's one rounding to float the gradients
+                       // agree from run to run unless a sum lies that close to a float rounding boundary
   unsigned long long* stats;   // optional [8] counters (GOF_STATS=1), else nullptr
 };
 
@@ -349,17 +353,17 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_backward(const 
           float g[16];
           pair_grad(row, (uint32_t)(gstart + b), contrib, g);
           const float sum = warp_reduce16(g, lane);
-          // one red per even lane into the Gaussian's 64-byte accumulator row: 16 global float atomics per (warp, Gaussian)
-          // instead of 17 per (pixel, Gaussian); dL_dopacity = -2/opacity * sum(dL_dC) is formed by k_preprocess_backward
+          // one red per even lane into the Gaussian's accumulator row: 16 global atomics per (warp, Gaussian) instead of
+          // 17 per (pixel, Gaussian); dL_dopacity = -2/opacity * sum(dL_dC) is formed by k_preprocess_backward
           const uint32_t gid = __float_as_uint(gof_lds32<84>(row));   // GofSplatBwd::self
-          if (!(lane & 1) && sum != 0.f) atomicAdd(a.grad_acc + ((size_t)gid * 16 + vidx), sum);
+          if (!(lane & 1) && sum != 0.f) atomicAdd(a.grad_acc + ((size_t)gid * 16 + vidx), (double)sum);
         }
       } else {
         // Each 4x2 pixel block (a quarter of the warp: the lanes that differ in bits 0, 1, 3) walks ITS OWN list -- the entries one
         // of its 8 pixels blended -- in lockstep with the other three: an iteration handles up to four different Gaussians, one per
         // quarter.  A Gaussian of pixel-scale footprint touches 16 of a warp's 32 pixels on average, so the warp-wide walk leaves
         // half of the lanes idle; quarter-wide, 4.9 M instead of 5.9 M iterations cover the same 93 M pairs at the benchmark
-        // workload (profiles/r2_mask_stats_c3.json).  The partial gradients are reduced over the quarter (14 shuffles) and leave
+        // workload.  The partial gradients are reduced over the quarter (14 shuffles) and leave
         // as two reds per lane.
         uint32_t qb = mybits;
         qb |= __shfl_xor_sync(0xffffffffu, qb, 1);
@@ -378,9 +382,9 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_backward(const 
           quarter_reduce16(g, lane, &r0, &r1);
           if (act) {
             const uint32_t gid = __float_as_uint(gof_lds32<84>(row));   // GofSplatBwd::self
-            float* dst = a.grad_acc + ((size_t)gid * 16 + ((lane & 8) ? 8 : 0) + ((lane & 2) ? 4 : 0) + ((lane & 1) ? 2 : 0));
-            if (r0 != 0.f) atomicAdd(dst, r0);
-            if (r1 != 0.f) atomicAdd(dst + 1, r1);
+            double* dst = a.grad_acc + ((size_t)gid * 16 + ((lane & 8) ? 8 : 0) + ((lane & 2) ? 4 : 0) + ((lane & 1) ? 2 : 0));
+            if (r0 != 0.f) atomicAdd(dst, (double)r0);
+            if (r1 != 0.f) atomicAdd(dst + 1, (double)r1);
           }
         }
       }
@@ -398,7 +402,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_backward(const 
 int gof_launch_render_backward(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& GL,
                                const char* bin, const GofBinLayout& BL, const char* img, const GofImageLayout& IL,
                                const float* dL_dpix, cudaStream_t st) {
-  BwdArgs a;
+  BwdArgs a{};
   a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
   a.ranges = reinterpret_cast<const uint2*>(img + IL.ranges);
   a.point_list = reinterpret_cast<const uint32_t*>(bin + BL.point_list);
@@ -411,21 +415,21 @@ int gof_launch_render_backward(const gof_scene_t* s, const GofView& v, char* geo
   a.plane = (size_t)v.tiles * 256;
   a.vmask = reinterpret_cast<const uint32_t*>(bin + BL.vmask);
   a.vstride = BL.vmask_stride;
-  a.grad_acc = reinterpret_cast<float*>(geom + GL.grad_acc);
-  GOF_CUDA_OK(cudaMemsetAsync(a.grad_acc, 0, (size_t)s->P * 64, st));
+  a.grad_acc = reinterpret_cast<double*>(geom + GL.grad_acc);
+  GOF_CUDA_OK(cudaMemsetAsync(a.grad_acc, 0, (size_t)s->P * 128, st));
   a.stats = gof_stats_buffer();
   static int occ = -1, stage = -1;   // GOF_BWD_OCC=2|3|4 (tuning knob); GOF_STAGE: staging variant (see render_fwd.cu)
   if (occ < 0) { const char* e = getenv("GOF_BWD_OCC"); occ = e ? atoi(e) : 4; }
   if (stage < 0) {
     const char* e = getenv("GOF_STAGE_BWD");
     if (!e) e = getenv("GOF_STAGE");
-    // default: the round-1 staging.  Measured at the benchmark workload with right-sized carveouts (profiles/r2_ab_staging_call3.jsonl):
-    // regs 2.06 ms, cp.async 2.10 ms, bulk 2.14 ms -- the backward walks each batch once and four CTAs per SM already cover the
-    // gather latency, while the two per-thread bulk copies cost ~18 issue slots per record (ELECT loop) and the double buffer
-    // takes 96 KB of L1 away from the mask / spill traffic.  The forward gains 7 % from the same change and keeps it.
+    // default: the round-1 staging, which was not slower than cp.async or bulk copies at the benchmark workload with right-sized
+    // carveouts -- the backward walks each batch once and four CTAs per SM already cover the gather latency, while the two
+    // per-thread bulk copies cost ~18 issue slots per record (ELECT loop) and the double buffer takes 96 KB of L1 away from the
+    // mask / spill traffic.
     stage = !e ? 0 : (e[0] == 'r' ? 0 : (e[0] == 'c' ? 2 : 1));
   }
-  // GOF_SUBWARP_BWD=0: one list per warp (round 1); default: one list per 4x2 pixel block (2.09 -> 1.86 ms, profiles/r2_ab_subwarp_call5.jsonl)
+  // GOF_SUBWARP_BWD=0: one list per warp (round 1); default: one list per 4x2 pixel block
   static int sub = -1;
   if (sub < 0) { const char* e = getenv("GOF_SUBWARP_BWD"); sub = (e && e[0] == '0') ? 0 : 1; }
   const size_t smem = (size_t)(stage ? 2 : 1) * BATCH * 96;

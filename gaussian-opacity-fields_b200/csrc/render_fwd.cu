@@ -184,7 +184,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const F
         // tested against the four blocks (four ballots), and the walk below advances the four lists in lockstep -- an
         // iteration evaluates up to four different Gaussians, one per quarter.  The smaller rectangles cull more precisely and a
         // pixel-scale footprint no longer drags 32 lanes through a visit that concerns 8 of them: 9.2 M instead of 10.4 M
-        // iterations at the benchmark workload (profiles/r2_mask_stats_c3.json).
+        // iterations at the benchmark workload.
         const bool in = idx < nb;
         const uint32_t lo = __float_as_uint(qb.z), hi = __float_as_uint(qb.w);
         const uint32_t m0 = __ballot_sync(0xffffffffu, in && box_hits(lo, hi, wx0, wy0, wx0 + 3, wy0 + 1));
@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const F
 int gof_launch_render_forward(const gof_scene_t* s, const GofView& v, const char* geom, const GofGeomLayout& GL,
                               char* bin, const GofBinLayout& BL, char* img, const GofImageLayout& IL,
                               float* out_color, cudaStream_t st) {
-  FwdArgs a;
+  FwdArgs a{};
   a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
   a.ranges = reinterpret_cast<const uint2*>(img + IL.ranges);
   a.point_list = reinterpret_cast<const uint32_t*>(bin + BL.point_list);
@@ -328,10 +328,10 @@ int gof_launch_render_forward(const gof_scene_t* s, const GofView& v, const char
     }                                                                                                                         \
     GOF_LAUNCH("render_fwd", st, k_render_forward<MINB, STG, SUBW><<<v.tiles, GOF_BLOCK_SIZE, 0, st>>>(a));                  \
   } while (0)
-  // GOF_SUBWARP_FWD=1: one list per 4x2 pixel block.  Off by default: measured 1.50 ms against 1.29 ms for the warp-wide walk at the
-  // benchmark workload (profiles/r2_ab_subwarp_call5.jsonl) -- the forward's visit is short (44 % end in the 20-instruction reject),
+  // GOF_SUBWARP_FWD=1: one list per 4x2 pixel block.  Off by default: slower than the warp-wide walk at the benchmark
+  // workload -- the forward's visit is short (44 % end in the 20-instruction reject),
   // so four ballots per group, the per-lane loop control and 40 more bytes of spills cost more than the 11 % fewer iterations
-  // save.  The backward, whose visit is 320 instructions, gains 11 % from the same idea and uses it.
+  // save.  The backward, whose visit is 320 instructions, gains from the same idea and uses it.
   static int sub = -1;
   if (sub < 0) { const char* e = getenv("GOF_SUBWARP_FWD"); sub = (e && e[0] == '1') ? 1 : 0; }
 #define GOF_FWD_STAGES(MINB, SUBW) \

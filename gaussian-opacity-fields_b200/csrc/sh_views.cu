@@ -104,7 +104,7 @@ extern "C" GOF_API int gof_sh_grad_from_views(int P, int M, int n_views, const f
   }
   if (P == 0) return GOF_OK;
   if (!means3D || !dL_dsh || (reinterpret_cast<uintptr_t>(dL_dsh) & 15u)) { gof_set_error("sh_grad_from_views: NULL or unaligned argument"); return GOF_E_INVALID; }
-  ShvArgs a;
+  ShvArgs a{};
   a.P = P; a.M = M; a.n_views = n_views; a.means3D = means3D; a.dL_dsh = dL_dsh;
   for (int v = 0; v < SHV_MAX_VIEWS; ++v) a.slot[v] = v < n_views ? slots[v] : nullptr;
   for (int v = 0; v < n_views; ++v)

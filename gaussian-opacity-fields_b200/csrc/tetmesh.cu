@@ -271,7 +271,7 @@ int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, co
     gof_set_error("marching_tets_emit: sizes do not match the count phase");
     return GOF_E_INVALID;
   }
-  EmitArgs a;
+  EmitArgs a{};
   // rows per chunk: the reference splits with torch.chunk(tets, T // chunk_size + 1) (utils/tetmesh.py:56-58), i.e. ceil(T / n)
   // rows; a NEGATIVE chunk_tets states the rows per chunk directly (tet-sharded extraction: every shard must cut where the
   // unsharded call cuts)

@@ -9,6 +9,7 @@ loaded the import fails, and CPU tensors are rejected.
 import ctypes
 import os
 import sys
+import threading
 
 import torch
 
@@ -17,7 +18,7 @@ _LIB_PATH = os.path.join(_HERE, "libgof_b200.so")
 if not os.path.exists(_LIB_PATH):
     raise ImportError(
         f"{_LIB_PATH} is missing: build it with `python gaussian-opacity-fields_b200/build.py` "
-        "(or __graft_entry__.build()). The B200 rasterizer has no CPU / PyTorch fallback."
+        "(or __graft_entry__.build()). The rasterizer has no CPU / PyTorch fallback."
     )
 _lib = ctypes.CDLL(_LIB_PATH)
 
@@ -68,8 +69,15 @@ _lib.gof_export_state.restype = ctypes.c_int
 _lib.gof_export_state.argtypes = [ctypes.c_int] * 4 + [_fp] * 4 + [ctypes.POINTER(_StateView), ctypes.c_void_p]
 
 
+_ALLOC_ERROR = threading.local()   # per thread: what a scratch allocation raised inside the ctypes callback (see _Scratch)
+
+
 def _check(rc):
+    err = getattr(_ALLOC_ERROR, "exc", None)
+    _ALLOC_ERROR.exc = None
     if rc != 0:
+        if err is not None:
+            raise err
         raise RuntimeError(f"gof_b200 (code {rc}): {_lib.gof_last_error().decode()}")
 
 
@@ -153,6 +161,13 @@ class _Scratch:
         pooled = bool(_USE_POOL and role)
 
         def alloc(_user, nbytes):
+            try:
+                return _alloc(nbytes)
+            except BaseException as e:      # noqa: BLE001 -- an exception cannot cross the C frame (ctypes would hand the
+                _ALLOC_ERROR.exc = e        # library an undefined pointer): NULL makes the call fail, and _check raises e
+                return 0
+
+        def _alloc(nbytes):
             if not nbytes:
                 return 0
             if pooled:

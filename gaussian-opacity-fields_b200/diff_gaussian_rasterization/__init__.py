@@ -1,4 +1,4 @@
-"""diff_gaussian_rasterization -- B200-native drop-in for GOF's rasterizer package.
+"""diff_gaussian_rasterization -- H100-native drop-in for GOF's rasterizer package.
 
 Same import surface as the reference package of the same name
 (submodules/diff-gaussian-rasterization/diff_gaussian_rasterization/__init__.py):
@@ -10,7 +10,7 @@ Same import surface as the reference package of the same name
 * rasterize_gaussians(...) and the autograd Function _RasterizeGaussians (reference :21-165)
 
 so gaussian_renderer/__init__.py:14,99-108,199-209 of the reference runs unmodified on top of it.
-The native side is libgof_b200.so (hand-written sm_100a CUDA, C ABI in include/gof_rasterizer.h) reached
+The native side is libgof_b200.so (hand-written sm_90a CUDA, C ABI in include/gof_rasterizer.h) reached
 through `_C`; there is no CPU or PyTorch fallback.
 """
 from typing import NamedTuple

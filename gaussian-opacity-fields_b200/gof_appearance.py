@@ -38,7 +38,7 @@ def _wgrad_lib():
 class _Conv3x3(torch.autograd.Function):
     """3x3 / stride 1 / pad 1 convolution whose WEIGHT and BIAS gradients come from the library's kernel (csrc/conv_wgrad.cu):
     for the few-channel, full-resolution layers at the network's tail cuDNN falls back to a generic fp32 weight-gradient engine
-    that alone costs 2.1 ms of a 5.2 ms appearance step on B200 (profiles/r2_appearance_profile_cudnn.txt).  Forward and data
+    that takes longer than the network's whole forward.  Forward and data
     gradient stay on cuDNN."""
 
     @staticmethod
@@ -94,7 +94,7 @@ class AppearanceNetwork(nn.Module):   # scene/appearance_network.py:18-46
         self.sigmoid = nn.Sigmoid()
 
     def forward(self, x):
-        if x.is_cuda and _USE_NHWC:      # measured on B200: no gain (cuDNN converts back and forth around its NCHW engines)
+        if x.is_cuda and _USE_NHWC:      # no gain measured (cuDNN converts back and forth around its NCHW engines)
             x = x.contiguous(memory_format=torch.channels_last)
         x = self.relu(self.conv1(x))
         x = self.up4(self.up3(self.up2(self.up1(x))))

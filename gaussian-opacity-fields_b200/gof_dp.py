@@ -331,8 +331,8 @@ class GradBucket:
 
     def autotune_exchange(self, group=None, modes=("nvls", "p2p", "nccl"), iters=5):
         """Measures the exchange with every mode this box supports (each adopted only after its collective self-test) and keeps
-        the fastest: which one wins depends on the world size -- on two B200s the peer-memory kernel (0.42 ms for the 256 MB
-        bucket) beats NCCL (0.54) and the in-switch reduction (0.76), while the switch saves NVLink traffic as ranks are added.
+        the fastest: which one wins depends on the machine and the world size -- at two ranks a peer-memory kernel moves the
+        fewest bytes per rank, while the in-switch reduction saves NVLink traffic as ranks are added.
         Collective; every rank takes the same decision (times are max-reduced).  Returns {mode: ms or the reason it is
         unavailable}; the views are re-created."""
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:

@@ -92,7 +92,7 @@ class CachedIntegrator:
     (`_C.integrate_prepare`: preprocess, depth sort, instance emission, tile sort) and afterwards runs only the point side
     (`_C.integrate_points_cached`).  The reference repeats the whole Gaussian side in each of its 9-10 passes over the same
     views (extract_mesh.py:56,92,107).  Results are bit-identical to GaussianRasterizer.integrate.  Memory: 64 B/Gaussian +
-    4 B/tile instance per cached view (3 M Gaussians: ~0.23 GB/view; 64 views on one 180 GB GPU, or 8 per GPU on 8)."""
+    4 B/tile instance per cached view (3 M Gaussians: ~0.23 GB/view; 64 views = 14.4 GB on one 80 GB GPU, or 8 per GPU on 8)."""
 
     def __init__(self, means3D, opacities, scales, rotations, shs, sh_degree, settings_for_view):
         self.gs = (means3D, opacities, scales, rotations, shs)

@@ -92,8 +92,10 @@ CONFIGS = {
     "C2": dict(P=200_000, width=800, height=800, seed=1),
     "C3": dict(P=1_000_000, width=1920, height=1080, seed=2),
     "C4": dict(P=2_500_000, width=1920, height=1080, seed=3, appearance=True),
-    # mesh extraction: 3 M Gaussians, 50 M tetrahedra vertices (query points), 64 views, ~6.5 tets per point
-    "C5": dict(P=3_000_000, width=1920, height=1080, seed=4, points=50_000_000, tets_per_point=6.5, n_views=64),
+    # mesh extraction: 3 M Gaussians, 27 M tetrahedra vertices (9 per Gaussian, as get_tetra_points), 64 views, ~6.5 tets
+    # per point -- sized so that the whole extraction (64 cached views, ~176 M tets and the marching-tetrahedra scratch of
+    # ~150 B/tet) fits one 80 GB GPU
+    "C5": dict(P=3_000_000, width=1920, height=1080, seed=4, points=27_000_000, tets_per_point=6.5, n_views=64),
 }
 
 

@@ -1,5 +1,5 @@
 /*
- * gof_rasterizer.h -- C ABI of the B200-native Gaussian-opacity-field rasterizer (libgof_b200.so).
+ * gof_rasterizer.h -- C ABI of the H100-native Gaussian-opacity-field rasterizer (libgof_b200.so).
  *
  * Drop-in boundary for the reference's `CudaRasterizer::Rasterizer` static interface
  * (reference: submodules/diff-gaussian-rasterization/cuda_rasterizer/rasterizer.h:20-124) and for the

@@ -2,7 +2,7 @@
  * gof_oracle.c -- TEST INFRASTRUCTURE ONLY (never linked, imported or executed by the product path).
  *
  * CPU restatement, in plain C, of the reference Gaussian-opacity-field rasterizer
- *   /root/reference/submodules/diff-gaussian-rasterization/cuda_rasterizer/{forward.cu,backward.cu,
+ *   <original project>/submodules/diff-gaussian-rasterization/cuda_rasterizer/{forward.cu,backward.cu,
  *   rasterizer_impl.cu,auxiliary.h}
  * function by function; every block cites the reference lines it follows.  Only tests/,
  * __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may call it.

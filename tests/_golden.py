@@ -13,8 +13,14 @@ def fixture_paths():
 
 
 def load(path):
-    z = np.load(path, allow_pickle=False)
-    d = {k: z[k] for k in z.files}
+    """One fixture as a dict.  A fixture too large for one file keeps its backward (grad*) and opacity-field query (int_*)
+    arrays in bwd_<name>.npz / int_<name>.npz next to it; they are merged in here."""
+    d = {}
+    head, base = os.path.split(path)
+    for part in (path, os.path.join(head, "bwd_" + base), os.path.join(head, "int_" + base)):
+        if os.path.exists(part):
+            z = np.load(part, allow_pickle=False)
+            d.update({k: z[k] for k in z.files})
     d["cfg"] = ast.literal_eval(str(d["cfg"]))
     d["name"] = os.path.splitext(os.path.basename(path))[0]
     return d

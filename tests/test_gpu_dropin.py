@@ -50,7 +50,7 @@ def renderers():
     import diff_gaussian_rasterization as ours
     refpkg = _refpy.ref_rasterizer_package()
     if refpkg is None:
-        pytest.skip("baseline/_ref/gof_ref_py or oracle/_ref not staged (needs /root/reference at build time)")
+        pytest.skip("the original project's Python (baseline/stage_ref.sh) or its extension (oracle/_ref) is not staged")
     a, b = _refpy.ref_gaussian_renderer(ours, "gof_gr_on_ours"), _refpy.ref_gaussian_renderer(refpkg, "gof_gr_on_ref")
     assert a.GaussianRasterizer is ours.GaussianRasterizer and b.GaussianRasterizer is refpkg.GaussianRasterizer
     src = _refpy.ref_method_source("gaussian_model.py", "GaussianModel", "get_view2gaussian")

@@ -1,19 +1,20 @@
 """GPU: the callers of the opacity-field query (SURVEY 8(a) rows a24-a26, 8(f) rank 3) at extract_mesh.py's structure.
 
 * CachedIntegrator (Gaussian side prepared once per view) is bit-identical to GaussianRasterizer.integrate;
-* gof_extract.evaluate_alpha equals the reference's OWN `evaluage_alpha` (extract_mesh.py:17-34, compiled from the staged
-  source text) driving the reference's gaussian_renderer.integrate on the reference's compiled rasterizer;
-* the 8-step bisection (extract_mesh.py:88-102) on top of either gives the same mesh vertices;
+* gof_extract.evaluate_alpha equals the reference's OWN `evaluage_alpha` (extract_mesh.py:17-34) driving the reference's
+  gaussian_renderer.integrate on the reference's compiled rasterizer, and the 8-step bisection (extract_mesh.py:88-102) on
+  top of either gives the same mesh vertices -- the reference's side stored in tests/golden/extract_ref.npz
+  (tests/golden/make_golden_ref_python.py);
 * tet-sharded marching tetrahedra (shards run one after the other on this GPU, merged as the ranks would) equals the unsharded call;
 * extract_level_set end to end on an analytic blob."""
 import math
 import types
 
+import numpy as np
 import pytest
 import torch
 
-import _refpy
-import _util
+import _liveref
 import gof_extract
 import gof_synth
 
@@ -66,47 +67,42 @@ class _Stub:
     get_features = property(lambda s: s.g["shs"])
 
 
-@pytest.fixture(scope="module")
-def ref_eval():
-    """The reference's evaluage_alpha (its source text, unmodified) bound to its own gaussian_renderer.integrate."""
-    pkg = _refpy.ref_rasterizer_package()
-    if pkg is None or _refpy.staged("text", "extract_mesh.py") is None:
-        pytest.skip("staged reference Python / oracle/_ref absent")
-    gr = _refpy.ref_gaussian_renderer(pkg, "gof_gr_on_ref_extract")
-    glb = {"torch": torch, "integrate": gr.integrate, "tqdm": lambda it, **kw: it}
-    return _refpy.ref_function("extract_mesh.py", "evaluage_alpha", glb)
-
-
 def _ref_views(cams, dev):
     return [types.SimpleNamespace(FoVx=2.0 * math.atan(c.tanfovx), FoVy=2.0 * math.atan(c.tanfovy), image_height=c.image_height,
                                   image_width=c.image_width, world_view_transform=c.world_view_transform.to(dev),
                                   full_proj_transform=c.full_proj_transform.to(dev), camera_center=c.camera_center.to(dev)) for c in cams]
 
 
-def test_evaluate_alpha_and_bisection_equal_the_reference_loop(ref_eval):
+def extract_case():
+    """Scene, query points and this package's alpha / colour of the evaluate_alpha comparison, and the bisection edges built
+    from them (pairs of points inside / outside the 0.5 level set)."""
     dev, cams, gs, g = _scene()
-    pipe = types.SimpleNamespace(debug=False, compute_cov3D_python=False, compute_view2gaussian_python=False, convert_SHs_python=False)
-    bg = torch.zeros(3, device=dev)
     pts = _points(gs, 200_000, 5, dev)
     ci = gof_extract.CachedIntegrator(g["means3D"], g["opacities"], g["scales"], g["rotations"], g["shs"], 3, _settings_for(dev))
     alpha, color = gof_extract.evaluate_alpha(pts, cams, ci, return_color=True)
-    ralpha, rcolor = ref_eval(pts, _ref_views(cams, dev), _Stub(g), pipe, bg, 0.0, return_color=True)
-    assert float((alpha - ralpha).abs().max()) < 5e-6
-    same = (alpha - ralpha).abs() < 1e-7          # colour = the arg-min view's pixel colour: compare where the minima agree to the bit-ish
-    assert float(same.float().mean()) > 0.99 and _util.rel_err(color[same], rcolor[same])[0] < 1e-5
-    assert torch.equal(gof_extract.evaluate_alpha(pts, cams, ci), alpha)
-
-    # bisection: edges = random pairs straddling the 0.5 level set
     inside, outside = torch.nonzero(alpha > 0.6).flatten()[:20_000], torch.nonzero(alpha < 0.4).flatten()[:20_000]
     n = min(inside.numel(), outside.numel())
-    assert n > 1000
     end_points = torch.stack([pts[inside[:n]], pts[outside[:n]]], dim=1)
     end_sdf = torch.stack([alpha[inside[:n]], alpha[outside[:n]]], dim=1)[..., None] - 0.5
-    ours = gof_extract.binary_search(end_points, end_sdf, lambda p: gof_extract.evaluate_alpha(p, cams, ci))
+    return dict(dev=dev, cams=cams, g=g, pts=pts, ci=ci, alpha=alpha, color=color, end_points=end_points, end_sdf=end_sdf)
+
+
+def sample(n, k, seed):
+    return np.sort(np.random.default_rng(seed).choice(n, min(n, k), replace=False))
+
+
+def record(ref_eval):
+    """The reference's side of test_evaluate_alpha_and_bisection_equal_the_reference_loop: `ref_eval` is its evaluage_alpha
+    bound to its own gaussian_renderer.integrate on its compiled rasterizer."""
+    c = extract_case()
+    dev, g, end_points, end_sdf = c["dev"], c["g"], c["end_points"], c["end_sdf"]
+    pipe = types.SimpleNamespace(debug=False, compute_cov3D_python=False, compute_view2gaussian_python=False, convert_SHs_python=False)
+    bg = torch.zeros(3, device=dev)
+    rv = _ref_views(c["cams"], dev)
+    ralpha, rcolor = ref_eval(c["pts"], rv, _Stub(g), pipe, bg, 0.0, return_color=True)
     # extract_mesh.py:73-102 with the reference's evaluage_alpha
     lp, rp = end_points[:, 0, :].clone(), end_points[:, 1, :].clone()
     ls, rs_ = end_sdf[:, 0, :].clone(), end_sdf[:, 1, :].clone()
-    rv = _ref_views(cams, dev)
     for _step in range(8):
         mid = (lp + rp) / 2
         msdf = (ref_eval(mid, rv, _Stub(g), pipe, bg, 0.0) - 0.5).squeeze().unsqueeze(-1)
@@ -114,8 +110,33 @@ def test_evaluate_alpha_and_bisection_equal_the_reference_loop(ref_eval):
         ls[low] = msdf[low]; rs_[~low] = msdf[~low]
         lp[low.flatten()] = mid[low.flatten()]; rp[~low.flatten()] = mid[~low.flatten()]
     want = (lp + rp) / 2
+    ip = sample(ralpha.shape[0], 4096, 3)
+    tp = torch.from_numpy(ip).to(dev)
+    return {"end_points": _liveref.digest(end_points), "pt_rows": ip.astype(np.int32), "alpha": ralpha[tp].cpu().numpy(),
+            "color": rcolor[tp].cpu().numpy(), "color_absmax": float(rcolor.abs().max()), "want": want.cpu().numpy()}
+
+
+def test_evaluate_alpha_and_bisection_equal_the_reference_loop():
+    """Against the stored reference results: alpha and colour on a seeded sample of the points, the bisection's end points on
+    every edge.  As in test_integrate.py's 1080p comparison, the reference's sm_90a build rounds a few ray depths differently
+    from the sm_100a build this implementation restates, so alpha is compared as the share of points that agree to 5e-6, with
+    every sampled point within 0.02."""
+    z = _liveref.load_npz("extract_ref.npz")
+    c = extract_case()
+    dev, cams, ci, alpha, color, end_points, end_sdf = c["dev"], c["cams"], c["ci"], c["alpha"], c["color"], c["end_points"], c["end_sdf"]
+    assert _liveref.digest(end_points) == str(z["end_points"]) and end_points.shape[0] > 1000
+    ip = torch.from_numpy(z["pt_rows"]).to(dev)
+    a, ra = alpha[ip].cpu().double().numpy(), z["alpha"].astype(np.float64)
+    assert np.mean(np.abs(a - ra) < 5e-6) > 0.995 and np.abs(a - ra).max() <= 0.02
+    same = np.abs(a - ra) < 1e-7          # colour = the arg-min view's pixel colour: compare where the minima agree to the bit-ish
+    assert same.mean() > 0.99
+    got = color[ip].cpu().double().numpy()[same]
+    assert np.abs(got - z["color"][same]).max() / max(float(z["color_absmax"]), 1e-30) < 1e-5
+    assert torch.equal(gof_extract.evaluate_alpha(c["pts"], cams, ci), alpha)
+
+    ours = gof_extract.binary_search(end_points, end_sdf, lambda p: gof_extract.evaluate_alpha(p, cams, ci))
     # a mid-point whose alpha sits within 5e-6 of 0.5 may take the other branch: such an edge ends at most one interval off
-    d = (ours - want).norm(dim=1)
+    d = (ours - torch.from_numpy(z["want"]).to(dev)).norm(dim=1)
     edge = (end_points[:, 0] - end_points[:, 1]).norm(dim=1)
     assert float((d <= 1e-6 * edge.clamp_min(1e-3)).float().mean()) > 0.999
     assert bool((d <= edge / 2 + 1e-6).all())

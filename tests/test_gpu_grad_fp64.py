@@ -7,25 +7,20 @@ evaluation of the SAME formulas instead (oracle/gof_oracle.c: double accumulatio
 
     err(ours, fp64)  <=  max(2 * err(reference, fp64), 1e-6)          for every gradient tensor, max-norm and relative L2
 
-with err(reference, fp64) measured in the same run on the live reference extension; without it (oracle/_ref not built) the
-absolute bounds of the last column of the committed report apply.  Writes gpurun_out/parity_report.json (copied to profiles/)."""
-import json
-import os
-
+with err(reference, fp64) measured in the same run on the live reference extension, or, where that is not built, as stored by
+tests/golden/make_golden_live_ref.py in tests/golden/live_grad_fp64_c2.npz."""
 import numpy as np
 import pytest
 import torch
 
+import _liveref
 import _util
 import gof_oracle
 import gof_synth
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NAMES = ["dmeans2D", "dcolors", "dopacity", "dmeans3D", "dcov3D", "dsh", "dscales", "drot", "dv2g"]
 OMAP = dict(dmeans2D="dL_dmean2D", dopacity="dL_dopacity", dmeans3D="dL_dmean3D", dsh="dL_dsh", dscales="dL_dscale", drot="dL_drot", dv2g="dL_dv2g")
-# absolute fallbacks when the live reference is absent: 3x what round 2 measured for this scene
-ABS = dict(dmeans2D=3e-6, dopacity=3e-6, dsh=3e-6, dv2g=3e-6, dmeans3D=3e-2, dscales=3e-2, drot=3e-2)
 
 
 def _err(a, b):
@@ -33,26 +28,35 @@ def _err(a, b):
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)), float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
 
 
+def c2_inputs(dev):
+    cam, gs = gof_synth.make_scene("C2", view=3)
+    dL = torch.randn(9, cam.image_height, cam.image_width, generator=torch.Generator().manual_seed(77))
+    return cam, gs, _util.fwd_args(cam, gs, dev), dL
+
+
+def fp64_gradients(cam, gs, dL):
+    """The oracle's fp64 forward + backward of the C2 view: (radii, {name: gradient})."""
+    sc = gof_oracle.scene_from_synth(cam, gs)
+    _out, oradii, st = gof_oracle.forward(sc)
+    return oradii, gof_oracle.backward(sc, st, dL.numpy())
+
+
 def test_gradients_against_fp64_oracle_at_c2():
     from diff_gaussian_rasterization import _C as ours
     ref = _util.load_ref()
     dev = torch.device("cuda")
-    cam, gs = gof_synth.make_scene("C2", view=3)
-    fa = _util.fwd_args(cam, gs, dev)
-    H, W = cam.image_height, cam.image_width
-    dL = torch.randn(9, H, W, generator=torch.Generator().manual_seed(77))
+    cam, gs, fa, dL = c2_inputs(dev)
     R, color, radii, geom, binning, img = ours.rasterize_gaussians(*fa)
     go = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, radii, geom, R, binning, img, dL.to(dev)))
     gr = None
+    stored = _liveref.load("grad_fp64_c2") if ref is None else None
     if ref is not None:
         Rr, cr, radr, ger, binr, imr = ref.rasterize_gaussians(*fa)
         gr = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, dL.to(dev)))
         gr2 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, dL.to(dev)))
     torch.cuda.synchronize()
-    sc = gof_oracle.scene_from_synth(cam, gs)
-    _out, oradii, st = gof_oracle.forward(sc)
+    oradii, od = fp64_gradients(cam, gs, dL)
     assert np.array_equal(radii.cpu().numpy(), oradii)
-    od = gof_oracle.backward(sc, st, dL.numpy())
     report, failures = {"config": "C2 view 3: 200000 Gaussians, 800x800, sh_degree 3", "criterion": "err(ours,fp64) <= max(2*err(ref,fp64), 1e-6); (max-norm, relative L2)"}, []
     for i, n in enumerate(NAMES):
         if n not in OMAP:
@@ -62,14 +66,12 @@ def test_gradients_against_fp64_oracle_at_c2():
         if gr is not None:
             er = _err(gr[i].cpu().numpy(), od[OMAP[n]])
             row.update(ref_vs_fp64=er, ref_vs_ref=_err(gr2[i].cpu().numpy(), gr[i].cpu().numpy()), ours_vs_ref=_err(go[i].cpu().numpy(), gr[i].cpu().numpy()))
-            ok = eo[0] <= max(2 * er[0], 1e-6) and eo[1] <= max(2 * er[1], 1e-6)
         else:
-            ok = eo[0] <= ABS[n]
+            er = tuple(float(x) for x in stored[n])
+            row.update(ref_vs_fp64=er)
+        ok = eo[0] <= max(2 * er[0], 1e-6) and eo[1] <= max(2 * er[1], 1e-6)
         row["ok"] = bool(ok)
         report[n] = row
         if not ok:
             failures.append((n, row))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "parity_report.json"), "w") as f:
-        json.dump(report, f, indent=1)
-    assert not failures, failures
+    assert not failures, (failures, report)

@@ -1,200 +1,88 @@
-"""GPU: differential test against the LIVE unmodified reference extension (oracle/_ref, built from /root/reference
-by oracle/build_ref.sh; travels to the GPU box as a prebuilt .so).  Skipped when that build is absent.
-BASELINE configs 2 and 3 at full size: every integer / index buffer bit-exact, view2gaussian bit-exact, images
-<= 2e-6 relative, gradients within max(1e-4, 4 x the reference's own run-to-run noise measured in the same test)."""
+"""GPU: differential test against the unmodified reference extension, through its outputs stored in tests/golden/live_*.npz
+(tests/_liveref.py; regenerated on a GPU by tests/golden/make_golden_live_ref.py from oracle/_ref, the reference built by
+oracle/build_ref.sh).  BASELINE configs 2 and 3 at full size: every integer / index buffer bit-exact, view2gaussian
+bit-exact, images <= 2e-6 relative, gradients within max(1e-4, 6 x the reference's own run-to-run noise)."""
 import pytest
 import torch
 
+import _liveref
 import _util
 import gof_synth
 
 pytestmark = pytest.mark.gpu
-NAMES = ["dmeans2D", "dcolors", "dopacity", "dmeans3D", "dcov3D", "dsh", "dscales", "drot", "dv2g"]
 
 
-AMPLIFIED = ("dmeans3D", "dscales", "drot")
-
-
-def _grad_close(n, ours, ref1, ref2):
-    """ours-vs-reference against the reference's own run-to-run noise.  The accumulated gradients are compared in max-norm.  For
-    dL_dmeans3D / dL_dscales / dL_drot the view2gaussian chain rule multiplies the atomics' summation noise by ~1/scale^2: their
-    max-norm difference between two REFERENCE runs is a heavy-tailed random number (0.17 ... 0.88 for dscales on the same C2
-    scene), so those are compared in relative L2 -- stable to a few percent between runs -- and pinned deterministically against
-    the fp64 oracle in test_gpu_grad_fp64.py."""
-    k = 1 if n in AMPLIFIED else 0
-    noise = _util.rel_err(ref2, ref1)[k]
-    err = _util.rel_err(ours, ref1)[k]
-    assert err <= max(1e-4, (3.0 if k else 6.0) * noise), f"{n}: ours-vs-ref {err}, ref-vs-ref {noise} ({'L2' if k else 'max-norm'})"
-
-
-@pytest.fixture(scope="module")
-def ref():
-    m = _util.load_ref()
-    if m is None:
-        pytest.skip("oracle/_ref/gof_ref_C*.so not built (needs /root/reference at build time)")
-    return m
+def _run(name):
+    from diff_gaussian_rasterization import _C as ours
+    dev = torch.device("cuda")
+    fa, P, W, H, grad = _liveref.inputs(name, dev)
+    out = ours.rasterize_gaussians(*fa)
+    R, _color, radii, geom, binning, img = out
+    go = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, radii, geom, R, binning, img, grad))
+    return fa, P, W, H, grad, out, go
 
 
 @pytest.mark.parametrize("name,view", [("C2", 3), ("C3", 1)])
-def test_full_size_against_live_reference(ref, name, view):
-    from diff_gaussian_rasterization import _C as ours
-    dev = torch.device("cuda")
-    cam, gs = gof_synth.make_scene(name, view=view)
-    fa = _util.fwd_args(cam, gs, dev)
-    P, W, H = gs["means3D"].shape[0], cam.image_width, cam.image_height
-    Ro, co, rado, geo, bino, imo = ours.rasterize_gaussians(*fa)
-    Rr, cr, radr, ger, binr, imr = ref.rasterize_gaussians(*fa)
-    so = ours.export_state(P, W, H, Ro, geo, bino, imo, rado)
-    sg, si, sb = _util.carve_ref_geom(ger, P), _util.carve_ref_image(imr, W, H), _util.carve_ref_binning(binr, Rr)
-    vis = radr > 0
-    assert Ro == Rr
-    assert torch.equal(rado, radr)
-    assert torch.equal(so["tiles_touched"], sg["tiles_touched"])
-    assert torch.equal(so["point_list"], sb["point_list"])
-    assert torch.equal(so["ranges"], si["ranges"])
-    assert torch.equal(so["n_contrib"], si["n_contrib"])
-    for f in ("depths", "means2D", "conic_opacity", "view2gaussian"):
-        assert torch.equal(so[f][vis].view(torch.int32), sg[f][vis].view(torch.int32)), f
-    assert _util.rel_err(so["rgb"][vis], sg["rgb"][vis])[0] < 5e-7
-    for ch in range(9):
-        assert _util.rel_err(co[ch], cr[ch])[0] < (2e-5 if ch == 8 else 2e-6), f"channel {ch}"
-    assert torch.equal(co[6], cr[6]) and torch.equal(co[7], cr[7])
-
-    grad = torch.randn(9, H, W, generator=torch.Generator().manual_seed(9)).to(dev)
-    go = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, rado, geo, Ro, bino, imo, grad))
-    g1 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    g2 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    for n, a, b, c in zip(NAMES, go, g1, g2):
-        _grad_close(n, a, b, c)
+def test_full_size_against_live_reference(name, view):
+    gold = _liveref.load(f"{name}_v{view}")
+    fa, P, W, H, grad, out, go = _run(f"{name}_v{view}")
+    _liveref.check_forward(gold, out, P, W, H, buffers=_liveref.BUFFERS,
+                           vis_fields=("depths", "means2D", "conic_opacity", "view2gaussian"), depth_channels=True, rgb=True)
+    _liveref.check_grads(gold, go)
 
 
 @pytest.mark.parametrize("M,deg", [(4, 1), (9, 2), (16, 2)])
-def test_sh_layouts_against_live_reference(ref, M, deg):
+def test_sh_layouts_against_live_reference(M, deg):
     """SH tensors with M != 16 coefficients / degree below the maximum (scalar load path and partial dL_dsh rows of
     k_preprocess_backward), P not a multiple of the warp size, and backward called twice on the same saved buffers."""
     from diff_gaussian_rasterization import _C as ours
-    dev = torch.device("cuda")
-    cam, gs = gof_synth.make_scene(dict(P=30_011, width=400, height=300, seed=21), view=11)
-    gs = dict(gs)
-    gs["shs"] = gs["shs"][:, :M, :].contiguous()
-    fa = _util.fwd_args(cam, gs, dev, sh_degree=deg)
-    Ro, co, rado, geo, bino, imo = ours.rasterize_gaussians(*fa)
-    Rr, cr, radr, ger, binr, imr = ref.rasterize_gaussians(*fa)
-    assert Ro == Rr and torch.equal(rado, radr)
-    for ch in range(9):
-        assert _util.rel_err(co[ch], cr[ch])[0] < (2e-5 if ch == 8 else 2e-6), f"channel {ch}"
-    grad = torch.randn(9, 300, 400, generator=torch.Generator().manual_seed(3)).to(dev)
-    go = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, rado, geo, Ro, bino, imo, grad))
-    go2 = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, rado, geo, Ro, bino, imo, grad))
-    g1 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    g2 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    def q99(x, y):   # robust relative error: 99th percentile of |x-y| over the 99th percentile of |y|
-        d, m = (x.double() - y.double()).abs().flatten(), y.double().abs().flatten()
-        if d.numel() == 0:
-            return 0.0
-        k = max(1, int(0.99 * d.numel()))
-        return float(d.kthvalue(k).values / m.kthvalue(k).values.clamp_min(1e-30))
-
-    for n, a, a2, b, c in zip(NAMES, go, go2, g1, g2):
-        assert a.shape == b.shape, n
-        if n in ("dmeans3D", "dscales", "drot"):
-            # the view2gaussian chain rule multiplies the atomics' summation noise by ~1/scale^2: the reference differs from
-            # ITSELF by percents in max-norm here (DESIGN.md 2.2), single elements are meaningless -> compare the bulk
-            noise = q99(c, b)
-            assert q99(a, b) <= max(1e-3, 6.0 * noise), f"{n}: ours-vs-ref q99 {q99(a, b)}, ref-vs-ref q99 {noise}"
-            assert q99(a2, a) <= max(1e-3, 6.0 * noise), f"{n}: second backward on the same buffers differs"
+    gold = _liveref.load(f"sh{M}_deg{deg}")
+    fa, P, W, H, grad, out, go = _run(f"sh{M}_deg{deg}")
+    _liveref.check_forward(gold, out, P, W, H)
+    _liveref.check_grads(gold, go, amp_floor=1e-3, amp_factor=6.0)
+    R, _c, radii, geom, binning, img = out
+    go2 = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, radii, geom, R, binning, img, grad))
+    for n, a, a2 in zip(_liveref.NAMES, go, go2):
+        assert a.shape == a2.shape, n
+        if n in _liveref.AMPLIFIED:      # float atomics: the bulk, relative L2
+            assert _util.rel_err(a2, a)[1] <= max(1e-3, 6.0 * float(gold[n + "_noise"])), f"{n}: second backward on the same buffers differs"
         else:
-            noise = _util.rel_err(c, b)[0]
-            assert _util.rel_err(a, b)[0] <= max(1e-4, 6.0 * noise), f"{n}: ours-vs-ref {_util.rel_err(a, b)[0]}, ref-vs-ref {noise}"
-            assert _util.rel_err(a2, a)[0] <= max(1e-5, 2.0 * noise), f"{n}: second backward on the same buffers differs"
+            assert _util.rel_err(a2, a)[0] <= max(1e-5, 2.0 * float(gold[n + "_noise"])), f"{n}: second backward on the same buffers differs"
     # coefficients above the active degree receive no gradient (backward.cu:20-139 writes degree <= D only)
     used = (deg + 1) ** 2
     assert float(go[5][:, used:, :].abs().max()) == 0.0 if used < M else True
 
 
-def test_view2gaussian_precomp_against_live_reference(ref):
+def test_view2gaussian_precomp_against_live_reference():
     """`view2gaussian_precomp` supplied by the caller (gaussian_renderer/__init__.py: pipe.compute_view2gaussian_python):
     K1 must take the 10-float records as given, the backward must return dL_dview2gaussian and leave scale/rotation
     gradients to the caller's autograd."""
     from diff_gaussian_rasterization import _C as ours
-    dev = torch.device("cuda")
-    cam, gs = gof_synth.make_scene(dict(P=50_000, width=640, height=400, seed=31), view=5)
-    fa = list(_util.fwd_args(cam, gs, dev))
-    P, W, H = 50_000, 640, 400
-    R0, c0, rad0, geo0, bin0, im0 = ours.rasterize_gaussians(*fa)
-    v2g = ours.export_state(P, W, H, R0, geo0, bin0, im0, rad0)["view2gaussian"].contiguous()   # bit-exact to the reference's
-    fa[8] = v2g                                                                                 # view2gaussian_precomp
-    fa = tuple(fa)
-    Ro, co, rado, geo, bino, imo = ours.rasterize_gaussians(*fa)
-    Rr, cr, radr, ger, binr, imr = ref.rasterize_gaussians(*fa)
-    assert Ro == Rr and torch.equal(rado, radr)
-    for ch in range(9):
-        assert _util.rel_err(co[ch], cr[ch])[0] < (2e-5 if ch == 8 else 2e-6), f"channel {ch}"
-    assert torch.equal(co[6], c0[6]) and torch.equal(co[7], c0[7])          # same records -> same image as the computed path
-    grad = torch.randn(9, H, W, generator=torch.Generator().manual_seed(4)).to(dev)
-    go = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, rado, geo, Ro, bino, imo, grad))
-    g1 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    g2 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    for n, a, b, c in zip(NAMES, go, g1, g2):
-        _grad_close(n, a, b, c)
-
-
-def _cov3d_from(scales, rotations, mod):
-    """computeCov3D (forward.cu:129-163) in torch float64 -> float32: Sigma = (S R)^T (S R), upper triangle."""
-    s = scales.double() * mod
-    r, x, y, z = rotations.double().unbind(1)
-    R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
-                     2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x),
-                     2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], 1).view(-1, 3, 3)
-    M = R * s[:, None, :]
-    S = M @ M.transpose(1, 2)
-    return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], 1).float().contiguous()
+    gold = _liveref.load("v2g_precomp")
+    fa, P, W, H, grad, out, go = _run("v2g_precomp")
+    _liveref.check_forward(gold, out, P, W, H)
+    fa0 = list(fa)
+    fa0[8] = torch.Tensor([])
+    c0 = ours.rasterize_gaussians(*fa0)[1]
+    assert torch.equal(out[1][6], c0[6]) and torch.equal(out[1][7], c0[7])          # same records -> same image as the computed path
+    _liveref.check_grads(gold, go)
 
 
 @pytest.mark.parametrize("with_v2g", [False, True])
-def test_cov3d_precomp_against_live_reference(ref, with_v2g):
+def test_cov3d_precomp_against_live_reference(with_v2g):
     """`cov3D_precomp` (forward.cu:339-348): the EWA footprint (radii, tiles, 2D conic, coef) comes from the caller's 3D
     covariance -- here deliberately 1.7x the one scale/rotation would give, so a path that ignored it fails on radii --
     while view2gaussian comes from scale/rotation (with_v2g=False) or from the caller (with_v2g=True, forward.cu:395-403).
     The reference dereferences scales/rotations unconditionally (forward.cu:334-335), so they are always supplied here."""
     from diff_gaussian_rasterization import _C as ours
-    dev = torch.device("cuda")
-    cam, gs = gof_synth.make_scene(dict(P=40_000, width=512, height=384, seed=41), view=9)
-    P, W, H = 40_000, 512, 384
-    fa = list(_util.fwd_args(cam, gs, dev, kernel_size=0.1))
-    fa[7] = _cov3d_from(gs["scales"], gs["rotations"], 1.7).to(dev)       # cov3D_precomp
-    if with_v2g:
-        R0, c0, rad0, geo0, bin0, im0 = ours.rasterize_gaussians(*_util.fwd_args(cam, gs, dev, kernel_size=0.1))
-        v2g = ours.export_state(P, W, H, R0, geo0, bin0, im0, rad0)["view2gaussian"]
-        # the export holds records of the Gaussians visible with the ORIGINAL covariance; the inflated one makes a few more
-        # visible -- give those a well-formed record (an isotropic sigma = 0.01 Gaussian 5 units in front of the camera) rather
-        # than zeros (A = B = 0 -> NaN depth in both implementations)
-        filler = torch.tensor([1e4, 0.0, 0.0, 1e4, 0.0, 1e4, 0.0, 0.0, -5e4, 25e4], device=dev)
-        fa[8] = torch.where((rad0 > 0)[:, None], v2g, filler[None, :]).contiguous()
-        del geo0, bin0, im0
-    fa = tuple(fa)
-    Ro, co, rado, geo, bino, imo = ours.rasterize_gaussians(*fa)
-    Rr, cr, radr, ger, binr, imr = ref.rasterize_gaussians(*fa)
-    base = ours.rasterize_gaussians(*_util.fwd_args(cam, gs, dev, kernel_size=0.1))
-    assert not torch.equal(base[2], rado), "the inflated covariance must change the radii"
-    assert Ro == Rr and torch.equal(rado, radr)
-    so = ours.export_state(P, W, H, Ro, geo, bino, imo, rado)
-    sg, si, sb = _util.carve_ref_geom(ger, P), _util.carve_ref_image(imr, W, H), _util.carve_ref_binning(binr, Rr)
-    vis = radr > 0
-    assert torch.equal(so["tiles_touched"], sg["tiles_touched"])
-    assert torch.equal(so["point_list"], sb["point_list"])
-    assert torch.equal(so["ranges"], si["ranges"])
-    assert torch.equal(so["n_contrib"], si["n_contrib"])
-    for f in ("depths", "means2D", "conic_opacity"):
-        assert torch.equal(so[f][vis].view(torch.int32), sg[f][vis].view(torch.int32)), f
-    for ch in range(9):
-        assert _util.rel_err(co[ch], cr[ch])[0] < (2e-5 if ch == 8 else 2e-6), f"channel {ch}"
-    grad = torch.randn(9, H, W, generator=torch.Generator().manual_seed(6)).to(dev)
-    go = ours.rasterize_gaussians_backward(*_util.bwd_args(fa, rado, geo, Ro, bino, imo, grad))
-    g1 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    g2 = ref.rasterize_gaussians_backward(*_util.bwd_args(fa, radr, ger, Rr, binr, imr, grad))
-    for n, a, b, c in zip(NAMES, go, g1, g2):
-        _grad_close(n, a, b, c)
+    name = "cov3d_v2g" if with_v2g else "cov3d"
+    gold = _liveref.load(name)
+    fa, P, W, H, grad, out, go = _run(name)
+    base = list(fa)
+    base[7], base[8] = torch.Tensor([]), torch.Tensor([])
+    assert not torch.equal(ours.rasterize_gaussians(*base)[2], out[2]), "the inflated covariance must change the radii"
+    _liveref.check_forward(gold, out, P, W, H, buffers=_liveref.BUFFERS, vis_fields=("depths", "means2D", "conic_opacity"))
+    _liveref.check_grads(gold, go)
     assert float(go[4].abs().max()) == 0.0          # dL_dcov3D stays zero (backward.cu:991-1007: EWA backward disabled)
 
 
@@ -209,7 +97,7 @@ def test_precomp_through_public_api():
     fa0 = _util.fwd_args(cam, gs, dev)
     R0, c0, rad0, geo0, bin0, im0 = ours.rasterize_gaussians(*fa0)
     v2g = ours.export_state(P, W, H, R0, geo0, bin0, im0, rad0)["view2gaussian"].contiguous().requires_grad_(True)
-    cov = _cov3d_from(gs["scales"], gs["rotations"], 1.0).to(dev)
+    cov = _liveref.cov3d_from(gs["scales"], gs["rotations"], 1.0).to(dev)
     rs = gof_synth.raster_settings(cam, gs["sh_degree"], dev)
     means3D = gs["means3D"].to(dev).requires_grad_(True)
     means2D = torch.zeros_like(means3D, requires_grad=True)

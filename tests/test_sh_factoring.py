@@ -2,13 +2,13 @@
 fixtures (tests/golden/*.npz, generated from the live reference extension by make_golden.py) hold, for one view, the reference's
 dL_dcolors, its clamp flags and its dL_dsh: the claim that the exchange rests on -- dL_dsh[k][c] = w_k(dir(mean, camera)) *
 (dL_dcolor[c] unless clamped), backward.cu:45-139 -- must reproduce the reference's dL_dsh from the other two."""
-import ast
 import os
 
 import numpy as np
 import pytest
 import torch
 
+import _golden
 import gof_dp
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -16,9 +16,8 @@ GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 @pytest.mark.parametrize("name", ["f0_sh3", "f1_sh1_mip_bg", "f3_sh0_inside"])
 def test_reference_dsh_is_the_outer_product_of_basis_and_masked_dcolor(name):
-    d = np.load(os.path.join(GOLD, name + ".npz"), allow_pickle=True)
-    cfg = d["cfg"].item()
-    degree = int((ast.literal_eval(cfg) if isinstance(cfg, str) else cfg)["sh_degree"])
+    d = _golden.load(os.path.join(GOLD, name + ".npz"))
+    degree = int(d["cfg"]["sh_degree"])
     means = torch.from_numpy(d["means3D"]).double()
     cam = torch.from_numpy(d["campos"]).double()
     rgb = torch.from_numpy(d["grad_dcolors"]).double() * (1.0 - torch.from_numpy(d["clamped"].astype(np.float64)))

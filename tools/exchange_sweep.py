@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Developer tool (GPU box, under torchrun with N >= 2 ranks): sweeps the launch parameters of the gradient-bucket exchange
 kernels (csrc/exchange.cu probes) on the 256 MB C3 bucket -- NVLS (multimem) and peer-memory variants -- next to NCCL's
-all-reduce and torch's own multimem all-reduce, and writes one JSON line per variant to gpurun_out/exchange_sweep_n<N>.jsonl.
+all-reduce and torch's own multimem all-reduce, and writes one JSON line per variant to tool_out/exchange_sweep_n<N>.jsonl.
 
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 tools/exchange_sweep.py
 """
@@ -29,7 +29,7 @@ lib.gof_p2p_probe.restype = ctypes.c_int
 lib.gof_p2p_probe.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_size_t] + [ctypes.c_int] * 4 + [ctypes.c_void_p]
 
 P = 1_000_000
-out_path = os.path.join(ROOT, "gpurun_out", f"exchange_sweep_n{world}.jsonl")
+out_path = os.path.join(ROOT, "tool_out", f"exchange_sweep_n{world}.jsonl")
 sync = torch.zeros(1, device=dev)
 sms = torch.cuda.get_device_properties(dev).multi_processor_count
 ITERS = 6

@@ -65,7 +65,7 @@ def main():
         res["faces"] = int(faces.shape[0])
         out[f"tetmesh_{T}"] = res
         print("tetmesh", json.dumps(res), flush=True)
-    with open(os.path.join(ROOT, "gpurun_out", "extract_bench.json"), "w") as f:
+    with open(os.path.join(ROOT, "tool_out", "extract_bench.json"), "w") as f:
         json.dump(out, f, indent=1)
 
 

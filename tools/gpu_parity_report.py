@@ -72,8 +72,8 @@ def main():
             entry["grad_ref_vs_ref_relerr"] = {n: _util.rel_err(a, b) for n, a, b in zip(names, gr2, gr)}
         report[f"{name}_view{view}"] = entry
         print(name, view, json.dumps(entry)[:3000], flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "parity_report.json"), "w") as f:
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    with open(os.path.join(ROOT, "tool_out", "parity_report.json"), "w") as f:
         json.dump(report, f, indent=1)
 
 

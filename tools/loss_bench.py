@@ -77,8 +77,8 @@ def main():
         res["speedup"] = res["torch_ms"] / res["fused_ms"]
         out[f"{W}x{H}"] = res
         print(W, H, json.dumps(res), flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "loss_bench.json"), "w"), indent=1)
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "tool_out", "loss_bench.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

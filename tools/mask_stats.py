@@ -4,7 +4,7 @@
 For one view of a config it answers: how many (pixel block, Gaussian) visits do the forward (box hits) and the backward
 (blocks with >= 1 blended pixel) make for block shapes 8x4 (a warp today), 4x4, 4x2 and 2x2 -- and how many warp iterations
 result if the sub-blocks of a warp walk INDEPENDENT lists in lockstep (max over the sub-blocks, per group of 32 list
-entries or per batch of 256).  Developer tool; prints one JSON line and writes gpurun_out/mask_stats_<cfg>.json."""
+entries or per batch of 256).  Developer tool; prints one JSON line and writes tool_out/mask_stats_<cfg>.json."""
 import json
 import os
 import sys
@@ -155,8 +155,8 @@ def main():
                      "warp_iters_lockstep_batch256": lock(cnt_b)}
     out["forward_box_hits"] = fw
     print(json.dumps(out))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", f"mask_stats_{name}.json"), "w"), indent=1)
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "tool_out", f"mask_stats_{name}.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

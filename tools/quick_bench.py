@@ -57,8 +57,8 @@ def main():
                 res[label]["kernels_ms"] = {k: round(v[1] / 3, 4) for k, v in sorted(ours.profile_report().items(), key=lambda kv: -kv[1][1])}
         out[name] = res
         print(name, json.dumps(res), flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "quick_bench.json"), "w") as f:
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    with open(os.path.join(ROOT, "tool_out", "quick_bench.json"), "w") as f:
         json.dump(out, f, indent=1)
 
 

@@ -54,6 +54,6 @@ prof = {k: round(v[1] / 5, 4) for k, v in sorted(_C.profile_report().items(), ke
 out = {"label": label, "config": name, "ms_per_step": round(ms, 4), "views_per_s": round(1e3 / ms, 1), "kernels_ms": prof,
        "env": {k: v for k, v in os.environ.items() if k.startswith("GOF_")}}
 print(json.dumps(out), flush=True)
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-with open(os.path.join(ROOT, "gpurun_out", "step_time.jsonl"), "a") as f:
+os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+with open(os.path.join(ROOT, "tool_out", "step_time.jsonl"), "a") as f:
     f.write(json.dumps(out) + "\n")

@@ -96,8 +96,8 @@ def main():
     out["torch_around_our_rasterizer_ms"] = time_it(stock, n_warm=3, n=10)
     out["speedup"] = out["torch_around_our_rasterizer_ms"] / out["ours_ms"]
     print(name, json.dumps(out), flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "train_step_bench.json"), "w"), indent=1)
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "tool_out", "train_step_bench.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":
