@@ -43,7 +43,6 @@ namespace {
 
 constexpr int THREADS = GOF_BLOCK_SIZE;              // 256
 constexpr int WARPS = THREADS / 32;
-// keys per thread / per CTA of a one-sweep pass are template parameters (GOF_SORT_KEYS=8|16, default chosen by measurement)
 constexpr uint32_t LB_AGG = 1u << 30;                // status word = flag (2 bits) | count (30 bits): written and read as ONE word
 constexpr uint32_t LB_INC = 2u << 30;
 constexpr uint32_t LB_VAL = (1u << 30) - 1u;
@@ -182,7 +181,7 @@ __global__ void __launch_bounds__(THREADS) k_digit_hist(const KeyT* __restrict__
 // ------------------------------------------------------------------------------------------------
 // One stable LSD radix pass in one launch.  Chunk c = keys [c*4096, (c+1)*4096); warp w of the CTA owns a contiguous
 // 1/8 of it, 32 keys per round: (chunk, warp, round, lane) order == input order, ranks within a digit follow it.
-template <typename KeyT, int ITEMS>
+template <typename KeyT>
 __global__ void __launch_bounds__(THREADS, 3) k_onesweep(const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
                                                         KeyT* __restrict__ keys_out, uint32_t* __restrict__ vals_out, size_t n,
                                                         int shift, uint32_t mask, const uint32_t* __restrict__ ghist,
@@ -191,9 +190,8 @@ __global__ void __launch_bounds__(THREADS, 3) k_onesweep(const KeyT* __restrict_
   __shared__ uint32_t s_cnt[WARPS][GOF_RADIX];   // per-warp digit counters -> exclusive offsets over the warps
   __shared__ uint32_t s_gbase[GOF_RADIX];        // global position of this chunk's first key of each digit
   __shared__ uint32_t s_lbase[GOF_RADIX];        // chunk-local position of the first key of each digit
-  constexpr int CHUNK = THREADS * ITEMS;
-  __shared__ KeyT s_keys[CHUNK];
-  __shared__ uint32_t s_vals[CHUNK];
+  __shared__ KeyT s_keys[GOF_SORT_CHUNK];
+  __shared__ uint32_t s_vals[GOF_SORT_CHUNK];
   __shared__ uint32_t s_chunk;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) s_chunk = atomicAdd(ticket, 1u);   // chunk numbers follow launch order: predecessors are running
@@ -202,20 +200,20 @@ __global__ void __launch_bounds__(THREADS, 3) k_onesweep(const KeyT* __restrict_
   uint32_t dig_total;
   const uint32_t gstart = block_excl_scan(threadIdx.x <= mask ? ghist[threadIdx.x] : 0u, &dig_total);   // barrier inside
   const uint32_t chunk = s_chunk;
-  const size_t cbase = (size_t)chunk * CHUNK;
-  const size_t wbase = cbase + (size_t)warp * (ITEMS * 32);
+  const size_t cbase = (size_t)chunk * GOF_SORT_CHUNK;
+  const size_t wbase = cbase + (size_t)warp * (GOF_SORT_ITEMS * 32);
 
-  KeyT key[ITEMS];
-  uint32_t rank[ITEMS];
+  KeyT key[GOF_SORT_ITEMS];
+  uint32_t rank[GOF_SORT_ITEMS];
   // all 16 key loads of the thread are issued before the first one is used
 #pragma unroll
-  for (int r = 0; r < ITEMS; ++r) {
+  for (int r = 0; r < GOF_SORT_ITEMS; ++r) {
     const size_t i = wbase + (size_t)r * 32 + lane;
     key[r] = i < n ? keys_in[i] : (KeyT)0;
   }
   const uint32_t lt = (1u << lane) - 1u;
 #pragma unroll
-  for (int r = 0; r < ITEMS; ++r) {
+  for (int r = 0; r < GOF_SORT_ITEMS; ++r) {
     const size_t i = wbase + (size_t)r * 32 + lane;
     const bool valid = i < n;
     const uint32_t d = valid ? (((uint32_t)key[r] >> shift) & mask) : (uint32_t)GOF_RADIX;   // sentinel digit for the ragged tail
@@ -249,7 +247,7 @@ __global__ void __launch_bounds__(THREADS, 3) k_onesweep(const KeyT* __restrict_
   // reorder the chunk in shared memory (digit runs become contiguous); the values are fetched only now -- they are not
   // needed for ranking and 16 more live registers would cost a resident CTA per SM
 #pragma unroll
-  for (int r = 0; r < ITEMS; ++r) {
+  for (int r = 0; r < GOF_SORT_ITEMS; ++r) {
     const size_t i = wbase + (size_t)r * 32 + lane;
     if (i < n) {
       const uint32_t d = ((uint32_t)key[r] >> shift) & mask;
@@ -262,7 +260,7 @@ __global__ void __launch_bounds__(THREADS, 3) k_onesweep(const KeyT* __restrict_
   if (threadIdx.x <= mask) s_gbase[threadIdx.x] = gstart + lookback_digit_walk(status, threadIdx.x, chunk, count);
   __syncthreads();
 #pragma unroll
-  for (int r = 0; r < ITEMS; ++r) {
+  for (int r = 0; r < GOF_SORT_ITEMS; ++r) {
     const uint32_t i = (uint32_t)r * THREADS + threadIdx.x;
     if (i < chunk_n) {
       const KeyT k = s_keys[i];
@@ -280,20 +278,13 @@ struct SortScratch {
   uint32_t* status;    // [4][chunk groups][256][4]: look-back status words (lookback_digit)
   size_t pass_words;   // words per pass in status
 };
-int sort_keys_per_thread() {
-  static int k = 0;
-  // 16 keys per thread measured faster than 8 (0.175 vs 0.185 ms for the six passes at C3)
-  if (!k) { const char* e = getenv("GOF_SORT_KEYS"); k = (e && atoi(e) == 8) ? 8 : 16; }
-  return k;
-}
-size_t sort_chunks(size_t n) { const size_t c = (size_t)THREADS * sort_keys_per_thread(); return (n + c - 1) / c; }
 
 SortScratch carve_sort_scratch(uint32_t* scratch, size_t n) {
   SortScratch s;
   s.ghist = scratch;
   s.tickets = scratch + 4 * GOF_RADIX;
   s.status = scratch + GOF_SORT_HEAD_BYTES / 4;
-  s.pass_words = (size_t)((sort_chunks(n) + 3) / 4 + 1) * GOF_RADIX * 4;
+  s.pass_words = (size_t)((gof_sort_blocks(n) + 3) / 4 + 1) * GOF_RADIX * 4;
   return s;
 }
 
@@ -312,18 +303,12 @@ void split_digits(int nbits, Digits* dg) {   // as evenly as possible, low digit
 template <typename KeyT>
 int onesweep_passes(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, size_t n, const Digits& dg, const SortScratch& sc, bool debug,
                     cudaStream_t st) {
-  const unsigned nb = (unsigned)sort_chunks(n);
-  const bool k16 = sort_keys_per_thread() == 16;
+  const unsigned nb = (unsigned)gof_sort_blocks(n);
   for (int p = 0; p < dg.passes; ++p) {
     const bool a2b = (p % 2 == 0);
-    if (k16)
-      GOF_LAUNCH("radix_onesweep", st, (k_onesweep<KeyT, 16><<<nb, THREADS, 0, st>>>(
-          a2b ? ka : kb, a2b ? va : vb, a2b ? kb : ka, a2b ? vb : va, n, dg.shift[p], dg.mask[p], sc.ghist + p * GOF_RADIX,
-          sc.status + (size_t)p * sc.pass_words, sc.tickets + p)));
-    else
-      GOF_LAUNCH("radix_onesweep", st, (k_onesweep<KeyT, 8><<<nb, THREADS, 0, st>>>(
-          a2b ? ka : kb, a2b ? va : vb, a2b ? kb : ka, a2b ? vb : va, n, dg.shift[p], dg.mask[p], sc.ghist + p * GOF_RADIX,
-          sc.status + (size_t)p * sc.pass_words, sc.tickets + p)));
+    GOF_LAUNCH("radix_onesweep", st, (k_onesweep<KeyT><<<nb, THREADS, 0, st>>>(
+        a2b ? ka : kb, a2b ? va : vb, a2b ? kb : ka, a2b ? vb : va, n, dg.shift[p], dg.mask[p], sc.ghist + p * GOF_RADIX,
+        sc.status + (size_t)p * sc.pass_words, sc.tickets + p)));
     GOF_LAUNCH_CHECK(debug, st);
   }
   return GOF_OK;

@@ -116,11 +116,6 @@ __device__ __forceinline__ void gof_bulk_g2s(uint32_t dst, const void* src, uint
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
                "r"(bytes), "r"(bar) : "memory");
 }
-// 16-byte asynchronous copy global -> shared (LDGSTS), L2 only; completion through cp.async.wait_all + a CTA barrier
-__device__ __forceinline__ void gof_cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void gof_cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void gof_sts32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
 __device__ __forceinline__ void gof_sts32u(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 
@@ -173,17 +168,20 @@ static inline size_t gof_align_up(size_t v, size_t a) { return (v + a - 1) / a *
 #define GOF_SORT_CHUNK (GOF_BLOCK_SIZE * GOF_SORT_ITEMS) // keys per block in a radix pass
 #define GOF_RADIX 256
 
-static inline int gof_sort_blocks(size_t n) { return (int)((n + GOF_SORT_CHUNK - 1) / GOF_SORT_CHUNK); }
+static constexpr inline int gof_sort_blocks(size_t n) { return (int)((n + GOF_SORT_CHUNK - 1) / GOF_SORT_CHUNK); }
 
-// Scratch of one radix sort of n pairs (binning.cu): global digit histograms of up to 4 passes [4][256], 64 ticket/flag words,
-// and per pass one decoupled-look-back status word per (chunk, digit).  (The pre-onesweep kernels, kept for A/B runs under
-// GOF_BINNING=legacy, need 256 * (blocks + 1) words of it.)
+// Scratch of one radix sort of n pairs (binning.cu) in c = gof_sort_blocks(n) chunks of GOF_SORT_CHUNK keys: global digit
+// histograms of up to 4 passes [4][256], 64 ticket/flag words, and per pass one decoupled-look-back status word per
+// (chunk, digit), padded to whole groups of four chunks: at most 4 * (c + 7) * 256 words.
 #define GOF_SORT_HEAD_BYTES (4 * GOF_RADIX * 4 + 256)
-#define GOF_SORT_MIN_CHUNK 2048   /* the one-sweep passes may run with 8 keys per thread: size the status words for that */
-static inline size_t gof_sort_scratch_bytes(size_t n) {
-  const size_t blocks = (n + GOF_SORT_MIN_CHUNK - 1) / GOF_SORT_MIN_CHUNK;
-  return (size_t)GOF_SORT_HEAD_BYTES + (size_t)4 * (blocks + 8) * GOF_RADIX * 4;
+static constexpr inline size_t gof_sort_scratch_bytes(size_t n) {
+  return (size_t)GOF_SORT_HEAD_BYTES + (size_t)4 * ((size_t)gof_sort_blocks(n) + 8) * GOF_RADIX * 4;
 }
+// The round-1 kernels (binning_legacy.cu, GOF_BINNING=legacy) use the same scratch as a [256][c] histogram and 256 digit
+// totals: 256 * (c + 1) words.  Both sizes are affine in c, so holding at both ends of the range of n holds for every n in it.
+static_assert(gof_sort_scratch_bytes(1) >= (size_t)GOF_RADIX * (gof_sort_blocks(1) + 1) * 4 &&
+                  gof_sort_scratch_bytes((size_t)1 << 40) >= (size_t)GOF_RADIX * (gof_sort_blocks((size_t)1 << 40) + 1) * 4,
+              "the legacy radix passes' histogram and digit totals must fit in gof_sort_scratch_bytes");
 
 struct GofGeomLayout {      // "geomBuffer": everything sized by P
   size_t splat, splat_bwd, rect, tiles, clamped, depth;

@@ -5,11 +5,9 @@
 //  * each (tile,Gaussian) instance is gathered as ONE 64-byte record (two sectors).  The per-tile slab is staged by the
 //    copy engine: every thread issues one 64-byte cp.async.bulk (global -> shared, completing on the mbarrier of the
 //    staging buffer) for its entry of batch i+1 while batch i is blended out of the other buffer (forward.cu:472-491 is a
-//    load/store/__syncthreads loop).  No registers hold records in flight (the register double buffer of round 1 cost
-//    16 registers and spills at 4 CTAs/SM) and a batch needs ONE CTA barrier instead of two.  ptxas issues a per-thread
-//    bulk copy from the uniform datapath, one elected lane at a time (UBLKCP inside an ELECT loop, ~9 issue slots per
-//    record); the third variant uses four 16-byte cp.async (LDGSTS) per record instead -- same double buffer, completion by
-//    cp.async.wait_all + the batch barrier.  GOF_STAGE=bulk|cpasync|regs selects the variant (regs = round 1) for A/B timing;
+//    load/store/__syncthreads loop).  No registers hold records in flight (a register double buffer costs 16 registers and
+//    spills at 4 CTAs/SM) and a batch needs ONE CTA barrier instead of two.  ptxas issues a per-thread bulk copy from the
+//    uniform datapath, one elected lane at a time (UBLKCP inside an ELECT loop, ~9 issue slots per record);
 //  * every record carries a conservative pixel box of the region where its alpha can reach 1/255
 //    (gof_cull_bbox); each warp ballots the 256 staged boxes against its own 8x4 pixel block and only visits
 //    the Gaussians that can touch it;
@@ -20,8 +18,6 @@
 //  * the quantities that only feed float outputs (mapped depth of the distortion term, the normalised normal)
 //    use cheaper evaluations accurate to ~1e-16 / 2e-7 instead of a double division, a double sqrt and three
 //    IEEE float divisions per blended pair.
-#include <stdlib.h>
-
 #include "gof_common.cuh"
 #include "gof_math.cuh"
 
@@ -51,14 +47,10 @@ __device__ __forceinline__ bool box_hits(uint32_t lo, uint32_t hi, int wx0, int 
   return x0 <= wx1 && x1 >= wx0 && y0 <= wy1 && y1 >= wy0;
 }
 
-// STAGE: 0 = registers + st.shared (round 1), 1 = cp.async.bulk + mbarrier, 2 = cp.async (LDGSTS)
-// SUB: the four 4x2 pixel blocks of a warp walk their own lists (see the group loop); otherwise one list per warp (round 1)
-template <int MINB, int STAGE, bool SUB>
-__global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const FwdArgs a) {
+__global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_forward(const FwdArgs a) {
   // Rows of 80 bytes = the 64-byte record of a staged Gaussian + (K', -, -, -), K' = the reject constant (see
-  // GofGeomLayout::reject_k).  One row base serves every load of a visit.  BULK: two buffers (40 KB), filled by bulk copies.
-  constexpr bool BULK = STAGE == 1, CPA = STAGE == 2;
-  __shared__ __align__(128) float4 s_rec[STAGE ? 2 : 1][BATCH][5];
+  // GofGeomLayout::reject_k).  One row base serves every load of a visit.  Two buffers (40 KB), filled by bulk copies.
+  __shared__ __align__(128) float4 s_rec[2][BATCH][5];
   __shared__ __align__(8) unsigned long long s_bar[2];
   const uint32_t s_base = gof_smem_base(&s_rec[0][0][0]);
   const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(&s_bar[0]);
@@ -86,11 +78,9 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const F
   float dist1 = 0.f, dist2 = 0.f, distortion = 0.f;
 
   // ---- staging ------------------------------------------------------------------------------------------------
-  // BULK: meta_id / meta_k hold this thread's list entry of the batch that is issued NEXT.
+  // meta_id / meta_k hold this thread's list entry of the batch that is issued NEXT.
   uint32_t meta_id = 0;
   float meta_k = 0.f;
-  float4 nx0, nx1, nx2, nx3;   // !BULK: the record in flight
-  nx0 = nx1 = nx2 = nx3 = make_float4(0.f, 0.f, 0.f, 0.f);
   auto load_meta = [&](int batch) {
     const int e = batch * BATCH + (int)threadIdx.x;
     if (e < total) {
@@ -101,72 +91,41 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const F
   auto issue = [&](int batch) {
     const bool has = batch * BATCH + (int)threadIdx.x < total;
     const uint32_t row = s_base + (uint32_t)((batch & 1) * BATCH + (int)threadIdx.x) * 80u;
-    if (BULK) {   // every thread arrives once per batch on the buffer's mbarrier; threads with an entry add 64 bytes
-      const uint32_t bar = bar0 + 8u * (uint32_t)(batch & 1);
-      if (has) {
-        gof_mbar_arrive_expect_tx(bar, 64u);
-        gof_bulk_g2s(row, a.splat + meta_id, 64u, bar);
-      } else {
-        gof_mbar_arrive(bar);
-      }
-    } else if (has) {
-      const char* src = reinterpret_cast<const char*>(a.splat + meta_id);
-      gof_cp_async16(row, src); gof_cp_async16(row + 16u, src + 16);
-      gof_cp_async16(row + 32u, src + 32); gof_cp_async16(row + 48u, src + 48);
+    // every thread arrives once per batch on the buffer's mbarrier; threads with an entry add 64 bytes
+    const uint32_t bar = bar0 + 8u * (uint32_t)(batch & 1);
+    if (has) {
+      gof_mbar_arrive_expect_tx(bar, 64u);
+      gof_bulk_g2s(row, a.splat + meta_id, 64u, bar);
+      gof_sts32(row + 64u, meta_k);
+    } else {
+      gof_mbar_arrive(bar);
     }
-    if (has) gof_sts32(row + 64u, meta_k);
   };
-  if (STAGE) {
-    if (BULK) {
-      if (threadIdx.x == 0) {
-        gof_mbar_init(bar0, GOF_BLOCK_SIZE);
-        gof_mbar_init(bar0 + 8u, GOF_BLOCK_SIZE);
-        gof_mbar_init_fence();
-      }
-      __syncthreads();
-    }
-    load_meta(0);
-    issue(0);
-    load_meta(1);
-  } else if ((int)threadIdx.x < total) {
-    const uint32_t g = a.point_list[range.x + threadIdx.x];
-    const float4* src = reinterpret_cast<const float4*>(a.splat + g);
-    nx0 = __ldg(src); nx1 = __ldg(src + 1); nx2 = __ldg(src + 2); nx3 = __ldg(src + 3);
-    meta_k = __ldg(a.reject_k + g);
+  if (threadIdx.x == 0) {
+    gof_mbar_init(bar0, GOF_BLOCK_SIZE);
+    gof_mbar_init(bar0 + 8u, GOF_BLOCK_SIZE);
+    gof_mbar_init_fence();
   }
+  __syncthreads();
+  load_meta(0);
+  issue(0);
+  load_meta(1);
 
   int toDo = total;
   int i = 0;
   for (; i < rounds; ++i, toDo -= BATCH) {
     // forward.cu:475-477: stop when every pixel of the tile is saturated.  The barrier also says: every warp has finished
     // with the buffer of batch i-1, and the K' values of batch i (plain stores) are visible.
-    if (CPA) gof_cp_async_wait_all();   // this thread's copies of batch i have landed; the barrier publishes everybody's
     if (__syncthreads_and(done)) break;
-    uint32_t buf_base = s_base;
-    if (STAGE) {
-      buf_base = s_base + (uint32_t)(i & 1) * (uint32_t)(BATCH * 80);
-      if (i + 1 < rounds) {
-        issue(i + 1);        // lands while this batch is blended
-        load_meta(i + 2);
-      }
-    } else {
-      s_rec[0][threadIdx.x][0] = nx0; s_rec[0][threadIdx.x][1] = nx1;
-      s_rec[0][threadIdx.x][2] = nx2; s_rec[0][threadIdx.x][3] = nx3;
-      s_rec[0][threadIdx.x][4].x = meta_k;
-      __syncthreads();
-      // issue the gather for the next batch; it completes while this batch is blended
-      const int nxt = (i + 1) * BATCH + (int)threadIdx.x;
-      if (nxt < total) {
-        const uint32_t g = a.point_list[range.x + nxt];
-        const float4* src = reinterpret_cast<const float4*>(a.splat + g);
-        nx0 = __ldg(src); nx1 = __ldg(src + 1); nx2 = __ldg(src + 2); nx3 = __ldg(src + 3);
-        meta_k = __ldg(a.reject_k + g);
-      }
+    const uint32_t buf_base = s_base + (uint32_t)(i & 1) * (uint32_t)(BATCH * 80);
+    if (i + 1 < rounds) {
+      issue(i + 1);        // lands while this batch is blended
+      load_meta(i + 2);
     }
 
     const int nb = toDo < BATCH ? toDo : BATCH;
     if (__all_sync(0xffffffffu, done)) continue;   // this warp's 32 pixels are saturated (it still takes part in the staging)
-    if (BULK) gof_mbar_wait(bar0 + 8u * (uint32_t)(i & 1), (uint32_t)(i >> 1) & 1u);   // batch i has landed
+    gof_mbar_wait(bar0 + 8u * (uint32_t)(i & 1), (uint32_t)(i >> 1) & 1u);   // batch i has landed
 
     // Sub-batches of 32: ballot which of these 32 staged Gaussians can reach this warp's 8x4 pixels at all, then
     // visit only those.  (The loop is deliberately NOT unrolled: the body is ~10 KB of SASS and eight copies
@@ -176,37 +135,14 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const F
       if (k * 32 >= nb) break;
       const int idx = k * 32 + lane;
       const float4 qb = gof_lds128<48>(buf_base + (uint32_t)idx * 80u);
-      uint32_t m;
-      if (!SUB) {
-        m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
-      } else {
-        // Each 4x2 pixel block (a quarter of the warp: lanes that differ in bits 0, 1, 3) gets ITS OWN list: the staged boxes are
-        // tested against the four blocks (four ballots), and the walk below advances the four lists in lockstep -- an
-        // iteration evaluates up to four different Gaussians, one per quarter.  The smaller rectangles cull more precisely and a
-        // pixel-scale footprint no longer drags 32 lanes through a visit that concerns 8 of them: 9.2 M instead of 10.4 M
-        // iterations at the benchmark workload.
-        const bool in = idx < nb;
-        const uint32_t lo = __float_as_uint(qb.z), hi = __float_as_uint(qb.w);
-        const uint32_t m0 = __ballot_sync(0xffffffffu, in && box_hits(lo, hi, wx0, wy0, wx0 + 3, wy0 + 1));
-        const uint32_t m1 = __ballot_sync(0xffffffffu, in && box_hits(lo, hi, wx0 + 4, wy0, wx0 + 7, wy0 + 1));
-        const uint32_t m2 = __ballot_sync(0xffffffffu, in && box_hits(lo, hi, wx0, wy0 + 2, wx0 + 3, wy0 + 3));
-        const uint32_t m3 = __ballot_sync(0xffffffffu, in && box_hits(lo, hi, wx0 + 4, wy0 + 2, wx0 + 7, wy0 + 3));
-        m = (lane & 16) ? ((lane & 4) ? m3 : m2) : ((lane & 4) ? m1 : m0);
-        // a block whose 8 pixels are all saturated has nothing left to walk
-        uint32_t d = done ? 1u : 0u;
-        d &= __shfl_xor_sync(0xffffffffu, d, 1);
-        d &= __shfl_xor_sync(0xffffffffu, d, 2);
-        d &= __shfl_xor_sync(0xffffffffu, d, 8);
-        if (d) m = 0u;
-      }
+      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
       uint32_t mybits = 0u;   // bit b: this pixel blended entry k*32+b of the batch
-      while (SUB ? __any_sync(0xffffffffu, m != 0u) : (m != 0u)) {
-        const bool act = m != 0u;
-        const int b = act ? __ffs(m) - 1 : 0;
+      while (m != 0u) {
+        const int b = __ffs(m) - 1;
         const int j = k * 32 + b;
-        m &= m - 1;          // (0 stays 0)
+        m &= m - 1;
         bool blended = false;
-        if (act && !done) {
+        if (!done) {
           const uint32_t contributor = (uint32_t)(i * BATCH + j + 1);   // 1-based position in the tile list
           const uint32_t row = buf_base + (uint32_t)j * 80u;
           const float4 q0 = gof_lds128<0>(row), q1 = gof_lds128<16>(row), q2 = gof_lds128<32>(row);
@@ -264,8 +200,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, MINB) k_render_forward(const F
   }
 
   // a CTA must not exit with copies in flight towards its shared memory: after an early break batch i may still be landing
-  if (BULK && i < rounds) gof_mbar_wait(bar0 + 8u * (uint32_t)(i & 1), (uint32_t)(i >> 1) & 1u);
-  if (CPA) gof_cp_async_wait_all();
+  if (i < rounds) gof_mbar_wait(bar0 + 8u * (uint32_t)(i & 1), (uint32_t)(i >> 1) & 1u);
 
   // forward.cu:584-611
   const size_t slot = (size_t)tile * 256 + threadIdx.x;
@@ -310,36 +245,14 @@ int gof_launch_render_forward(const gof_scene_t* s, const GofView& v, const char
   a.plane = (size_t)v.tiles * 256;
   a.vmask = reinterpret_cast<uint32_t*>(bin + BL.vmask);
   a.vstride = BL.vmask_stride;
-  static int occ = -1, stage = -1;   // GOF_FWD_OCC=3|4: resident CTAs per SM the kernel is compiled for; GOF_STAGE: staging variant
-  if (occ < 0) { const char* e = getenv("GOF_FWD_OCC"); occ = e ? atoi(e) : 4; }
-  if (stage < 0) {
-    const char* e = getenv("GOF_STAGE_FWD");
-    if (!e) e = getenv("GOF_STAGE");
-    stage = !e ? 1 : (e[0] == 'r' ? 0 : (e[0] == 'c' ? 2 : 1));
+  static bool attr_set = false;   // 4 CTAs x (40 KB + 1 KB) per SM: ask for just that much shared memory -- the rest
+  if (!attr_set) {                // stays L1 (local-memory spills and the mask / output traffic go through it)
+    const int need = 4 * (2 * BATCH * 80 + 1024 + 64);
+    GOF_CUDA_OK(cudaFuncSetAttribute(k_render_forward, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
+    attr_set = true;
   }
-#define GOF_FWD_LAUNCH(MINB, STG, SUBW)                                                                                              \
-  do {                                                                                                                        \
-    static bool attr_set = false;   /* MINB CTAs x (20 or 40 KB + 1 KB) per SM: ask for just that much shared memory --      */ \
-    if (!attr_set) {                /* the rest stays L1 (local-memory spills and the mask / output traffic go through it)    */ \
-      const int need = MINB * ((STG ? 2 : 1) * BATCH * 80 + 1024 + 64);                                                       \
-      GOF_CUDA_OK(cudaFuncSetAttribute(k_render_forward<MINB, STG, SUBW>, cudaFuncAttributePreferredSharedMemoryCarveout,           \
-                                       (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));        \
-      attr_set = true;                                                                                                        \
-    }                                                                                                                         \
-    GOF_LAUNCH("render_fwd", st, k_render_forward<MINB, STG, SUBW><<<v.tiles, GOF_BLOCK_SIZE, 0, st>>>(a));                  \
-  } while (0)
-  // GOF_SUBWARP_FWD=1: one list per 4x2 pixel block.  Off by default: slower than the warp-wide walk at the benchmark
-  // workload -- the forward's visit is short (44 % end in the 20-instruction reject),
-  // so four ballots per group, the per-lane loop control and 40 more bytes of spills cost more than the 11 % fewer iterations
-  // save.  The backward, whose visit is 320 instructions, gains from the same idea and uses it.
-  static int sub = -1;
-  if (sub < 0) { const char* e = getenv("GOF_SUBWARP_FWD"); sub = (e && e[0] == '1') ? 1 : 0; }
-#define GOF_FWD_STAGES(MINB, SUBW) \
-  do { if (stage == 1) GOF_FWD_LAUNCH(MINB, 1, SUBW); else if (stage == 2) GOF_FWD_LAUNCH(MINB, 2, SUBW); else GOF_FWD_LAUNCH(MINB, 0, SUBW); } while (0)
-  if (occ >= 4) { if (sub) GOF_FWD_STAGES(4, true); else GOF_FWD_STAGES(4, false); }
-  else { if (sub) GOF_FWD_STAGES(3, true); else GOF_FWD_STAGES(3, false); }
-#undef GOF_FWD_STAGES
-#undef GOF_FWD_LAUNCH
+  GOF_LAUNCH("render_fwd", st, k_render_forward<<<v.tiles, GOF_BLOCK_SIZE, 0, st>>>(a));
   GOF_LAUNCH_CHECK(s->debug, st);
   return GOF_OK;
 }
