@@ -10,9 +10,10 @@
 // re-evaluating t, G and alpha with the forward's operation sequence (gof_math.cuh) so that they are bit-identical.
 // The traversal starts at the last Gaussian any pixel of the tile blended.
 // The per-tile slab (64-byte record + 32-byte backward record per list entry) is staged through registers into one 24 KB
-// buffer of dynamic shared memory.  The bulk-copy double buffer of render_fwd.cu does not pay here: the backward walks each
-// batch once, four resident CTAs already cover the gather latency, the two per-thread bulk copies cost ~18 issue slots per
-// record (ELECT loop) and the second buffer takes 96 KB per SM away from L1, which carries the mask / spill traffic.
+// buffer of dynamic shared memory, and each warp's masks of the batch into an 8 KB slab next to it.  The bulk-copy double
+// buffer of render_fwd.cu does not pay here: the backward walks each batch once, four resident CTAs already cover the gather
+// latency, the two per-thread bulk copies cost ~18 issue slots per record (ELECT loop) and the second buffer takes 96 KB per
+// SM away from L1, which carries the gather / spill traffic.
 #include "gof_common.cuh"
 #include "gof_math.cuh"
 
@@ -41,6 +42,12 @@ struct BwdArgs {
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
+constexpr int GROUPS = BATCH / 32;   // groups of 32 list entries per batch: one mask word per (warp, group, lane)
+constexpr int WARPS = GOF_BLOCK_SIZE / 32;
+// dynamic shared memory: [BATCH] records of 96 bytes | [WARPS][GROUPS][32] u32 blend masks of the batch.  32 KB in all, so that
+// four CTAs (plus 1 KB reserved per CTA) fill the 132 KB shared-memory carveout exactly and L1 keeps the rest of the SM's 256 KB
+constexpr int SMEM_RECORDS = BATCH * 96;
+constexpr int SMEM_BYTES = SMEM_RECORDS + WARPS * GROUPS * 32 * 4;
 
 // Sum 16 per-lane values over a QUARTER of the warp -- the 8 lanes of a 4x2 pixel block: lanes that differ in bits 0, 1 (x)
 // and 3 (y) only -- with 14 shuffles: at every step each lane keeps half of its values and trades the other half with its
@@ -78,12 +85,14 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
   // rows of 96 bytes per staged Gaussian = GofSplat (64 B) | GofSplatBwd (32 B: means2D, 2D conic, own index); one row base
   // register serves every load of a visit (see gof_smem_base)
   extern __shared__ __align__(128) float4 s_dyn[];
-  __shared__ uint32_t s_max;
   const uint32_t s_base = gof_smem_base(s_dyn);
 
   const int tile = blockIdx.x;
   const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // this warp's mask slab [GROUPS][32]; its first word also carries the tile's deepest contributor before the first batch
+  uint32_t* const s_mask = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(s_dyn) + SMEM_RECORDS) + warp * GROUPS * 32;
+  uint32_t* const s_max = s_mask - warp * GROUPS * 32;
   const int wx0 = tile_x * 16 + (warp & 1) * 8, wy0 = tile_y * 16 + (warp >> 1) * 4;
   const uint32_t pix_x = wx0 + (lane & 7);
   const uint32_t pix_y = wy0 + (lane >> 3);
@@ -118,11 +127,11 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
   uint32_t warp_last = last_contributor;
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) warp_last = max(warp_last, __shfl_xor_sync(0xffffffffu, warp_last, d));
-  if (threadIdx.x == 0) s_max = 0u;
+  if (threadIdx.x == 0) *s_max = 0u;
   __syncthreads();
-  if (lane == 0) atomicMax(&s_max, warp_last);
+  if (lane == 0) atomicMax(s_max, warp_last);
   __syncthreads();
-  const int used = (int)min(s_max, range.y - range.x);
+  const int used = (int)min(*s_max, range.y - range.x);
   const int rounds = (used + BATCH - 1) / BATCH;
 
   float last_alpha = 0.f;
@@ -151,145 +160,166 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
       const float4* srcb = reinterpret_cast<const float4*>(a.splat_bwd + g);
       dst[4] = __ldg(srcb); dst[5] = __ldg(srcb + 1);
     }
+    // the batch's masks, one coalesced 128-byte row per group as the forward wrote them.  The forward wrote the rows of every
+    // group up to this warp's deepest contributor; nothing behind it blended, and the rows past it read as empty.
+#pragma unroll
+    for (int k = 0; k < GROUPS; ++k) {
+      const int gstart = base + k * 32;
+      s_mask[k * 32 + lane] = (uint32_t)gstart < warp_last ? __ldg(vm_row + gstart) : 0u;
+    }
     __syncthreads();
 
-    // the loop is NOT unrolled (one copy of the body, see render_fwd.cu)
-#pragma unroll 1
-    for (int k = BATCH / 32 - 1; k >= 0; --k) {
-      const int gstart = base + k * 32;
-      // the forward wrote the masks of every group up to this warp's deepest contributor; nothing behind it blended
-      if ((uint32_t)gstart >= warp_last) continue;
-      const uint32_t mybits = __ldg(vm_row + gstart);        // bit b: this pixel blended entry gstart+b
-
-      // the 16 partial gradients of ONE (pixel, Gaussian) pair: row = the staged record, contributor = its zero-based index in the
-      // tile list (the reference's `contributor` after its decrement, backward.cu:763), contrib = this pixel blended it
-      auto pair_grad = [&](const uint32_t row, const uint32_t contributor, const bool contrib, float (&g)[16]) {
-        if (STATS) { st_eval += contrib; st_pass += contrib; }
-        const float4 q0 = gof_lds128<0>(row), q1 = gof_lds128<16>(row), q2 = gof_lds128<32>(row);
-        const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
-        GofPair p;
-        float t = 0.f, G = 0.f, alpha = 0.f;
-        double qd = 0.0, rA = 0.0;
-        if (contrib) {
-          // re-evaluated with the forward's operation sequence: bit-identical t, G, alpha
-          p = gof_pair_geom(v, rx, ry);
-          float power;
-          gof_pair_t_power(p, v[9], &t, &power, &qd, &rA);
-          G = F_EXP(power);
-          alpha = fminf(F_MUL(q2.z, G), GOF_ALPHA_MAX);
-        }
-        if (STATS) st_contrib += contrib;
+    // the 16 partial gradients of ONE (pixel, Gaussian) pair: row = the staged record, contributor = its zero-based index in the
+    // tile list (the reference's `contributor` after its decrement, backward.cu:763), contrib = this pixel blended it
+    auto pair_grad = [&](const uint32_t row, const uint32_t contributor, const bool contrib, float (&g)[16]) {
+      if (STATS) { st_eval += contrib; st_pass += contrib; }
+      const float4 q0 = gof_lds128<0>(row), q1 = gof_lds128<16>(row), q2 = gof_lds128<32>(row);
+      const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
+      GofPair p;
+      float t = 0.f, G = 0.f, alpha = 0.f;
+      double qd = 0.0, rA = 0.0;
+      if (contrib) {
+        // re-evaluated with the forward's operation sequence: bit-identical t, G, alpha
+        p = gof_pair_geom(v, rx, ry);
+        float power;
+        gof_pair_t_power(p, v[9], &t, &power, &qd, &rA);
+        G = F_EXP(power);
+        alpha = fminf(F_MUL(q2.z, G), GOF_ALPHA_MAX);
+      }
+      if (STATS) st_contrib += contrib;
 
 #pragma unroll
-        for (int q = 0; q < 16; ++q) g[q] = 0.f;
-        if (contrib) {
-          // backward.cu:806-817
-          float rt;
-          const float mt = gof_mapped_t_fast(t, &rt);
-          const float dm_dt = ((20.0f / 99.8f) * rt) * rt;   // d/dt of 100/99.8 - (20/99.8)/t
-          // 1/|n| to ~1 ulp (Newton-refined rsqrt; as accurate as an IEEE sqrt followed by an IEEE reciprocal -- the
-          // plain 2-ulp rsqrt is not: this feeds dL_dview2gaussian, whose chain rule amplifies every ulp by ~1/scale^2)
-          const float rlen = gof_rsqrt_newton(F_FMA(p.n2, p.n2, F_FMA(p.n0, p.n0, F_MUL(p.n1, p.n1))) + 1e-7f);
-          const float nn0 = -p.n0 * rlen, nn1 = -p.n1 * rlen, nn2 = -p.n2 * rlen;
-          const float r1a = gof_rcp_newton(1.f - alpha);   // 1 - alpha in [0.01, 1]
-          T = T * r1a;
-          const float w = alpha * T;
-          float dL_dalpha = 0.f;
-          // colour, :824-837
-          const float2 q3 = gof_lds64<48>(row);
-          const float c0 = q2.w, c1 = q3.x, c2 = q3.y;
-          acc_c0 = last_alpha * last_c0 + (1.f - last_alpha) * acc_c0; last_c0 = c0;
-          acc_c1 = last_alpha * last_c1 + (1.f - last_alpha) * acc_c1; last_c1 = c1;
-          acc_c2 = last_alpha * last_c2 + (1.f - last_alpha) * acc_c2; last_c2 = c2;
-          dL_dalpha += (c0 - acc_c0) * dpix0;
-          dL_dalpha += (c1 - acc_c1) * dpix1;
-          dL_dalpha += (c2 - acc_c2) * dpix2;
-          g[10] = w * dpix0; g[11] = w * dpix1; g[12] = w * dpix2;
-          // distortion: only the depth path survives ("detach weight", :848-858)
-          const float dL_dmax_t = 2.0f * (T * alpha) * (mt * final_A - final_D) * dreg * dm_dt;
-          // normal, :860-877
-          acc_n0 = last_alpha * last_n0 + (1.f - last_alpha) * acc_n0; last_n0 = nn0;
-          acc_n1 = last_alpha * last_n1 + (1.f - last_alpha) * acc_n1; last_n1 = nn1;
-          acc_n2 = last_alpha * last_n2 + (1.f - last_alpha) * acc_n2; last_n2 = nn2;
-          dL_dalpha += (nn0 - acc_n0) * dn0;
-          dL_dalpha += (nn1 - acc_n1) * dn1;
-          dL_dalpha += (nn2 - acc_n2) * dn2;
-          const float dnn0 = w * dn0, dnn1 = w * dn1, dnn2 = w * dn2;
-          const float dL_dlength = (dnn0 * p.n0 + dnn1 * p.n1 + dnn2 * p.n2) * (rlen * rlen);
-          float dnrm0 = (-dnn0 + dL_dlength * p.n0) * rlen;
-          float dnrm1 = (-dnn1 + dL_dlength * p.n1) * rlen;
-          float dnrm2 = (-dnn2 + dL_dlength * p.n2) * rlen;
-          // :879-893
-          float dL_dt = dL_dmax_t;
-          if (contributor == max_contributor - 1u) dL_dt += ddepth;
-          dL_dalpha *= T;
-          last_alpha = alpha;
-          dL_dalpha += (-T_final * r1a) * bg_dot_dpixel;
-          // :896-912  2D-mean statistic and opacity
-          const float4 b0 = gof_lds128<64>(row);   // (mx, my, cx, cy)
-          const float b1x = gof_lds32<80>(row);    // cz
-          const float dx = b0.x - (float)pix_x, dy = b0.y - (float)pix_y;
-          const float dL_dG = q2.z * dL_dalpha;
-          const float gdx = G * dx, gdy = G * dy;
-          const float dG_ddelx = -gdx * b0.z - gdy * b0.w;
-          const float dG_ddely = -gdy * b1x - gdx * b0.w;
-          g[13] = dL_dG * dG_ddelx * ddelx_dx;
-          g[14] = dL_dG * dG_ddely * ddely_dy;
-          g[15] = fabsf(g[13]) + fabsf(g[14]);
-          // :914-928 in double like the reference; BB/AA = -qd is reused from the forward evaluation
-          const float dL_dmin = dL_dG * G * -0.5f;
-          g[9] = dL_dmin;   // dL_dC; dL_dopacity = G*dL_dalpha = dL_dC * (-2/opacity) is derived from its sum below
-          // A and B enter in double like the reference; 1/AA comes from the forward division (rA), -BB/AA = qd.
-          // The sums below are formed by single float FMAs on the rounded dL_dA / dL_dB: one rounding each, like
-          // the reference's double expression stored to float.
-          const double inv2A = 0.5 * rA;
-          const float dA = (float)((double)dL_dmin * qd * qd * 0.25 - (double)dL_dt * qd * inv2A);
-          const float dB2 = (float)((double)dL_dmin * qd - (double)dL_dt * rA);   // 2 * dL_dB
-          // :938-952
-          dnrm0 = fmaf(dA, rx, dnrm0);
-          dnrm1 = fmaf(dA, ry, dnrm1);
-          dnrm2 = dnrm2 + dA;
-          g[0] = dnrm0 * rx;
-          g[1] = dnrm0 * ry + dnrm1 * rx;
-          g[2] = dnrm0 + dnrm2 * rx;
-          g[3] = dnrm1 * ry;
-          g[4] = dnrm1 + dnrm2 * ry;
-          g[5] = dnrm2;
-          g[6] = dB2 * rx;
-          g[7] = dB2 * ry;
-          g[8] = dB2;
-        }
-      };
-
-      // Each 4x2 pixel block (a quarter of the warp: the lanes that differ in bits 0, 1, 3) walks ITS OWN list -- the entries one
-      // of its 8 pixels blended -- in lockstep with the other three: an iteration handles up to four different Gaussians, one per
-      // quarter.  A Gaussian of pixel-scale footprint touches 16 of a warp's 32 pixels on average, so a warp-wide walk leaves
-      // half of the lanes idle; quarter-wide, 4.9 M instead of 5.9 M iterations cover the same 93 M pairs at the benchmark
-      // workload.  The partial gradients are reduced over the quarter (14 shuffles) and leave as two reds per lane; no red
-      // carries dL_dopacity, which k_preprocess_backward forms as -2/opacity * sum(dL_dC).
-      uint32_t qb = mybits;
-      qb |= __shfl_xor_sync(0xffffffffu, qb, 1);
-      qb |= __shfl_xor_sync(0xffffffffu, qb, 2);
-      qb |= __shfl_xor_sync(0xffffffffu, qb, 8);
-      while (__any_sync(0xffffffffu, qb != 0u)) {
-        const bool act = qb != 0u;
-        const int b = act ? 31 - __clz(qb) : 0;
-        if (act) qb &= ~(1u << b);
-        const uint32_t row = s_base + (uint32_t)(k * 32 + b) * 96u;
-        const bool contrib = act && ((mybits >> b) & 1u) != 0u;
-        if (STATS) { st_visit += (lane == 0); st_anyhit += act && !(lane & 11); }
-        float g[16];
-        pair_grad(row, (uint32_t)(gstart + b), contrib, g);
-        float r0, r1;
-        quarter_reduce16(g, lane, &r0, &r1);
-        if (act) {
-          const uint32_t gid = __float_as_uint(gof_lds32<84>(row));   // GofSplatBwd::self
-          double* dst = a.grad_acc + ((size_t)gid * 16 + ((lane & 8) ? 1 : 0) + ((lane & 2) ? 2 : 0) + ((lane & 1) ? 4 : 0));
-          if (r0 != 0.f) atomicAdd(dst, (double)r0);
-          if (r1 != 0.f) atomicAdd(dst + 8, (double)r1);
-          if (STATS) st_red += (r0 != 0.f) + (r1 != 0.f);
-        }
+      for (int q = 0; q < 16; ++q) g[q] = 0.f;
+      if (contrib) {
+        // backward.cu:806-817
+        float rt;
+        const float mt = gof_mapped_t_fast(t, &rt);
+        const float dm_dt = ((20.0f / 99.8f) * rt) * rt;   // d/dt of 100/99.8 - (20/99.8)/t
+        // 1/|n| to ~1 ulp (Newton-refined rsqrt; as accurate as an IEEE sqrt followed by an IEEE reciprocal -- the
+        // plain 2-ulp rsqrt is not: this feeds dL_dview2gaussian, whose chain rule amplifies every ulp by ~1/scale^2)
+        const float rlen = gof_rsqrt_newton(F_FMA(p.n2, p.n2, F_FMA(p.n0, p.n0, F_MUL(p.n1, p.n1))) + 1e-7f);
+        const float nn0 = -p.n0 * rlen, nn1 = -p.n1 * rlen, nn2 = -p.n2 * rlen;
+        const float r1a = gof_rcp_newton(1.f - alpha);   // 1 - alpha in [0.01, 1]
+        T = T * r1a;
+        const float w = alpha * T;
+        // Every sum of two products below names the product that is fused (F_FMA) and the one that is rounded (F_MUL), as
+        // gof_math.cuh does for the forward: left to ptxas, the choice differs between instantiations of this kernel, and
+        // the view2gaussian chain rule turns the last-ulp difference into percents in dL_dscale / dL_drot.
+        // colour, :824-837
+        const float2 q3 = gof_lds64<48>(row);
+        const float c0 = q2.w, c1 = q3.x, c2 = q3.y;
+        const float one_m_last = 1.f - last_alpha;
+        acc_c0 = F_FMA(last_alpha, last_c0, F_MUL(one_m_last, acc_c0)); last_c0 = c0;
+        acc_c1 = F_FMA(last_alpha, last_c1, F_MUL(one_m_last, acc_c1)); last_c1 = c1;
+        acc_c2 = F_FMA(last_alpha, last_c2, F_MUL(one_m_last, acc_c2)); last_c2 = c2;
+        float dL_dalpha = F_FMA(c0 - acc_c0, dpix0, 0.f);
+        dL_dalpha = F_FMA(c1 - acc_c1, dpix1, dL_dalpha);
+        dL_dalpha = F_FMA(c2 - acc_c2, dpix2, dL_dalpha);
+        g[10] = w * dpix0; g[11] = w * dpix1; g[12] = w * dpix2;
+        // distortion: only the depth path survives ("detach weight", :848-858)
+        const float dL_dmax_t = 2.0f * (T * alpha) * F_FMA(mt, final_A, -final_D) * dreg * dm_dt;
+        // normal, :860-877
+        acc_n0 = F_FMA(last_alpha, last_n0, F_MUL(one_m_last, acc_n0)); last_n0 = nn0;
+        acc_n1 = F_FMA(last_alpha, last_n1, F_MUL(one_m_last, acc_n1)); last_n1 = nn1;
+        acc_n2 = F_FMA(last_alpha, last_n2, F_MUL(one_m_last, acc_n2)); last_n2 = nn2;
+        dL_dalpha = F_FMA(nn0 - acc_n0, dn0, dL_dalpha);
+        dL_dalpha = F_FMA(nn1 - acc_n1, dn1, dL_dalpha);
+        dL_dalpha = F_FMA(nn2 - acc_n2, dn2, dL_dalpha);
+        const float dnn0 = w * dn0, dnn1 = w * dn1, dnn2 = w * dn2;
+        const float dL_dlength = F_MUL(F_FMA(dnn2, p.n2, F_FMA(dnn0, p.n0, F_MUL(dnn1, p.n1))), F_MUL(rlen, rlen));
+        const float dnrm0_l = F_FMA(dL_dlength, p.n0, -dnn0);   // before the factor rlen
+        const float dnrm1_l = F_FMA(dL_dlength, p.n1, -dnn1);
+        const float dnrm2_l = F_FMA(dL_dlength, p.n2, -dnn2);
+        // :879-893
+        float dL_dt = dL_dmax_t;
+        if (contributor == max_contributor - 1u) dL_dt += ddepth;
+        last_alpha = alpha;
+        dL_dalpha = F_FMA(dL_dalpha, T, F_MUL(F_MUL(-T_final, r1a), bg_dot_dpixel));
+        // :896-912  2D-mean statistic and opacity
+        const float4 b0 = gof_lds128<64>(row);   // (mx, my, cx, cy)
+        const float b1x = gof_lds32<80>(row);    // cz
+        const float dx = b0.x - (float)pix_x, dy = b0.y - (float)pix_y;
+        const float dL_dG = q2.z * dL_dalpha;
+        const float gdx = G * dx, gdy = G * dy;
+        const float dG_ddelx = F_FMA(-gdx, b0.z, -F_MUL(gdy, b0.w));
+        const float dG_ddely = F_FMA(-gdy, b1x, -F_MUL(gdx, b0.w));
+        g[13] = dL_dG * dG_ddelx * ddelx_dx;
+        g[14] = dL_dG * dG_ddely * ddely_dy;
+        g[15] = fabsf(g[13]) + fabsf(g[14]);
+        // :914-928 in double like the reference; BB/AA = -qd is reused from the forward evaluation
+        const float dL_dmin = dL_dG * G * -0.5f;
+        g[9] = dL_dmin;   // dL_dC; dL_dopacity = G*dL_dalpha = dL_dC * (-2/opacity) is derived from its sum below
+        // A and B enter in double like the reference; 1/AA comes from the forward division (rA), -BB/AA = qd.
+        // The sums below are formed by single float FMAs on the rounded dL_dA / dL_dB: one rounding each, like
+        // the reference's double expression stored to float.
+        const double inv2A = 0.5 * rA;
+        const float dA = (float)D_FMA(D_MUL(D_MUL((double)dL_dmin, qd), qd), 0.25, -D_MUL(D_MUL((double)dL_dt, qd), inv2A));
+        const float dB2 = (float)D_FMA((double)dL_dt, -rA, D_MUL((double)dL_dmin, qd));   // 2 * dL_dB
+        // :938-952
+        const float dnrm0 = F_FMA(dA, rx, F_MUL(dnrm0_l, rlen));
+        const float dnrm1 = F_FMA(dA, ry, F_MUL(dnrm1_l, rlen));
+        const float dnrm2 = F_FMA(dnrm2_l, rlen, dA);
+        g[0] = dnrm0 * rx;
+        g[1] = F_FMA(dnrm0, ry, F_MUL(dnrm1, rx));
+        g[2] = F_FMA(dnrm2, rx, dnrm0);
+        g[3] = dnrm1 * ry;
+        g[4] = F_FMA(dnrm2, ry, dnrm1);
+        g[5] = dnrm2;
+        g[6] = dB2 * rx;
+        g[7] = dB2 * ry;
+        g[8] = dB2;
       }
+    };
+
+    // Each 4x2 pixel block (a quarter of the warp: the lanes that differ in bits 0, 1, 3) walks ITS OWN list -- the entries one
+    // of its 8 pixels blended -- in lockstep with the other three: an iteration handles up to four different Gaussians, one per
+    // quarter.  A Gaussian of pixel-scale footprint touches 16 of a warp's 32 pixels on average, so a warp-wide walk leaves
+    // half of the lanes idle.  The lockstep spans the whole batch: a quarter whose group runs out moves on to its next
+    // non-empty group while the others are still in theirs, so an iteration waits only for the quarter with the most entries
+    // in the batch, not in each group of 32 (4.4 M instead of 4.9 M iterations for the same 93 M pairs at the benchmark
+    // workload).  The partial gradients are reduced over the quarter (14 shuffles) and leave as two reds per lane; no red
+    // carries dL_dopacity, which k_preprocess_backward forms as -2/opacity * sum(dL_dC).
+    const uint32_t* const s_quarter = s_mask + (lane & 20);   // the words of this lane's quarter: + {0..3, 8..11} + 32*group
+    // bit 4*group + quarter of `nonempty`: that quarter blended something in that group; lane l forms the bit of group l/4
+    // and of the quarter whose first lane is ((l & 1) << 2) | ((l & 2) << 3)
+    auto quarter_word = [](const uint32_t* w) {
+      const uint4 x = *reinterpret_cast<const uint4*>(w), y = *reinterpret_cast<const uint4*>(w + 8);
+      return x.x | x.y | x.z | x.w | y.x | y.y | y.z | y.w;
+    };
+    const uint32_t nonempty = __ballot_sync(0xffffffffu,
+                                            quarter_word(s_mask + (lane >> 2) * 32 + ((lane & 1) << 2) + ((lane & 2) << 3)) != 0u);
+    // the cursor: the groups still to visit (bit 4*group), the current group's first entry, the quarter's entries left in it
+    // and this pixel's own mask of it
+    uint32_t left = (nonempty >> (((lane >> 2) & 1) | ((lane >> 3) & 2))) & 0x11111111u;
+    uint32_t first = 0u, qb = 0u, mybits = 0u;
+    auto next_group = [&]() {
+      if (left == 0u) return;
+      const int hb = 31 - __clz(left);   // 4 * group
+      left ^= 1u << hb;
+      first = (uint32_t)hb * 8u;
+      qb = quarter_word(s_quarter + first);
+      mybits = s_mask[first + lane];
+    };
+    next_group();
+    while (__any_sync(0xffffffffu, qb != 0u)) {
+      const bool act = qb != 0u;
+      const int b = act ? 31 - __clz(qb) : 0;
+      if (act) qb &= ~(1u << b);
+      const uint32_t row = s_base + (first + (uint32_t)b) * 96u;
+      const bool contrib = act && ((mybits >> b) & 1u) != 0u;
+      if (STATS) { st_visit += (lane == 0); st_anyhit += act && !(lane & 11); }
+      float g[16];
+      pair_grad(row, (uint32_t)base + first + (uint32_t)b, contrib, g);
+      float r0, r1;
+      quarter_reduce16(g, lane, &r0, &r1);
+      if (act) {
+        const uint32_t gid = __float_as_uint(gof_lds32<84>(row));   // GofSplatBwd::self
+        double* dst = a.grad_acc + ((size_t)gid * 16 + ((lane & 8) ? 1 : 0) + ((lane & 2) ? 2 : 0) + ((lane & 1) ? 4 : 0));
+        if (r0 != 0.f) atomicAdd(dst, (double)r0);
+        if (r1 != 0.f) atomicAdd(dst + 8, (double)r1);
+        if (STATS) st_red += (r0 != 0.f) + (r1 != 0.f);
+      }
+      if (qb == 0u) next_group();
     }
   }
   if (STATS && a.stats) {
@@ -303,12 +333,12 @@ template <bool STATS>
 int launch_backward(const BwdArgs& a, int tiles, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    const int need = (STATS ? 3 : 4) * (BATCH * 96 + 1024 + 128);   // only what the resident CTAs need: the rest stays L1
+    const int need = (STATS ? 3 : 4) * (SMEM_BYTES + 1024);   // only what the resident CTAs need: the rest stays L1
     GOF_CUDA_OK(cudaFuncSetAttribute(k_render_backward<STATS>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                      (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
     attr_set = true;
   }
-  GOF_LAUNCH("render_bwd", st, k_render_backward<STATS><<<tiles, GOF_BLOCK_SIZE, BATCH * 96, st>>>(a));
+  GOF_LAUNCH("render_bwd", st, k_render_backward<STATS><<<tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
   return GOF_OK;
 }
 
