@@ -451,30 +451,58 @@ void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const u
   }
 }
 
+/* |x - ref| within n float ulp of ref */
+static int near_ulp(float x, float ref, int n) { return fabsf(x - ref) <= n * (nextafterf(ref, INFINITY) - ref); }
+
+/* The t and alpha of the forward's blend test (forward.cu:499-535) for the pair (v, opacity, ray). */
+static void pair_t_alpha(const float* v, float opac, float rx, float ry, float* t_out, float* alpha_out) {
+  const pair_t p = pair_geom(v, rx, ry);
+  const double AA = p.AA, BB = p.BB;
+  *t_out = (float)(-BB / (2 * AA));
+  const double min_value = fma(-BB / AA, BB / 4., (double)v[9]);
+  float power = (float)(-0.5 * min_value);
+  if (power > 0.0f) power = 0.0f;
+  *alpha_out = fminf(0.99f, opac * expf(power));
+}
+
 /* backward.cu:634-955 renderCUDA.  Gradients are accumulated in per-thread double buffers, then reduced.
- * dL_dmean2D [P,3], dL_dopacity [P], dL_dcolors [P,3], dL_dview2gaussian [P,10] (float outputs). */
+ * dL_dmean2D [P,3], dL_dopacity [P], dL_dcolors [P,3], dL_dview2gaussian [P,10] (float outputs).
+ *
+ * Optional error scales, [P,17] doubles each (NULL: not computed; the gradients do not depend on it), in the order of the
+ * accumulator (dL_dcolors 0-2 | dL_dmean2D 3-5 | dL_dopacity 6 | dL_dview2gaussian 7-16):
+ *   mag       for every Gaussian and component, the sum over its pairs of the pair term's magnitude: the term with every sum
+ *             and difference replaced by the sum of the absolute values of its operands, down to the pair's inputs (T,
+ *             accum_rec, colours, dL_dpix, G, conic, AA, BB, rx, ry, normal).  A rounding of any intermediate moves a
+ *             component by a multiple of 2^-24 of this, whatever cancels inside the term or across terms.
+ *   marginal  the same sum over the pairs whose value depends on a blend decision that a last-ulp difference in expf can
+ *             flip: a pair whose alpha lies within 8 ulp of 1/255 or whose t lies within 8 ulp of the near plane
+ *             (alpha < 1/255 and t <= 0.2 reject a pair), and every pair in front of it at that pixel, whose T and
+ *             accum_rec the decision changes.  Pairs behind it do not depend on it (the walk runs back to front). */
 void oracle_render_backward(int P, int W, int H, float tan_fovx, float tan_fovy, const uint32_t* ranges,
                             const uint32_t* point_list, const float* bg, const float* means2D,
                             const float* conic_opacity, const float* colors, const float* view2gaussian,
                             const float* final_Ts, const uint32_t* n_contrib, const float* dL_dpixels,
-                            float* dL_dmean2D, float* dL_dopacity, float* dL_dcolors, float* dL_dview2gaussian) {
+                            float* dL_dmean2D, float* dL_dopacity, float* dL_dcolors, float* dL_dview2gaussian,
+                            double* mag, double* marginal) {
   const float focal_y = H / (2.0f * tan_fovy), focal_x = W / (2.0f * tan_fovx);
   const int gx = (W + BLOCK_X - 1) / BLOCK_X;
   const size_t HW = (size_t)H * W;
   const int NG = 17;
+  const int bounds = mag != NULL && marginal != NULL;
+  const int NS = bounds ? 3 * NG : NG;   /* per Gaussian and thread: the sums, then mag, then marginal */
   int nthreads = 1;
 #ifdef _OPENMP
   nthreads = omp_get_max_threads();
-  if (nthreads > 8 && (size_t)P * NG * 8 * nthreads > ((size_t)4 << 30)) nthreads = 8;
+  if (nthreads > 8 && (size_t)P * NS * 8 * nthreads > ((size_t)4 << 30)) nthreads = 8;
 #endif
-  double* acc = (double*)calloc((size_t)nthreads * P * NG, sizeof(double));
+  double* acc = (double*)calloc((size_t)nthreads * P * NS, sizeof(double));
 #pragma omp parallel for schedule(dynamic, 8) num_threads(nthreads)
   for (int py = 0; py < H; ++py) {
     int tid = 0;
 #ifdef _OPENMP
     tid = omp_get_thread_num();
 #endif
-    double* my = acc + (size_t)tid * P * NG;
+    double* my = acc + (size_t)tid * P * NS;
     for (int px = 0; px < W; ++px) {
       const size_t pix_id = (size_t)W * py + px;
       const float pixfx = (float)px + 0.5f, pixfy = (float)py + 0.5f;
@@ -494,6 +522,18 @@ void oracle_render_backward(int P, int W, int H, float tan_fovx, float tan_fovy,
       const float dL_dmax_depth = dL_dpixels[6 * HW + pix_id];
       float last_alpha = 0, last_color[3] = {0}, last_normal[3] = {0}, accum_normal_rec[3] = {0};
       const float ddelx_dx = 0.5f * W, ddely_dy = 0.5f * H;
+      /* error scales: the magnitudes of accum_rec / accum_normal_rec, and the deepest pair of the walk whose blend decision
+       * is marginal (-1: none) */
+      double accum_abs[3] = {0, 0, 0}, accum_normal_abs[3] = {0, 0, 0};
+      long marginal_upto = -1;
+      if (bounds) {
+        for (int c = 0; c < last_contributor && range[0] + (uint32_t)c < range[1]; ++c) {
+          const uint32_t gid = point_list[range[0] + c];
+          float t, alpha;
+          pair_t_alpha(view2gaussian + 10 * (size_t)gid, conic_opacity[4 * (size_t)gid + 3], rx, ry, &t, &alpha);
+          if (near_ulp(alpha, 1.0f / 255.0f, 8) || near_ulp(t, (float)NEAR_PLANE, 8)) marginal_upto = c;
+        }
+      }
       for (uint32_t k = range[1]; k-- > range[0];) {
         contributor--;
         if (contributor >= (uint32_t)last_contributor) continue;
@@ -505,13 +545,28 @@ void oracle_render_backward(int P, int W, int H, float tan_fovx, float tan_fovy,
         const double AA = p.AA, BB = p.BB;
         const float CC = v[9];
         const float t = (float)(-BB / (2 * AA));
-        if (t <= NEAR_PLANE) continue;
+        const int near_t = bounds && near_ulp(t, (float)NEAR_PLANE, 8);
+        if (t <= NEAR_PLANE && !near_t) continue;
         const double min_value = fma(-BB / AA, BB / 4., (double)CC);
         float power = (float)(-0.5 * min_value);
         if (power > 0.0f) power = 0.0f;
         const float G = expf(power);
-        const float alpha = fminf(0.99f, con_o[3] * G);
-        if (alpha < 1.0f / 255.0f) continue;
+        const float alpha0 = fminf(0.99f, con_o[3] * G);
+        const int near_a = bounds && near_ulp(alpha0, 1.0f / 255.0f, 8);
+        if (alpha0 < 1.0f / 255.0f && !near_a) continue;
+        /* a "ghost": a pair this walk rejects by a marginal decision, which a 2-ulp expf may have blended.  Its term, evaluated
+         * as if it blended, goes to `marginal` only; the gradients and the walk's state stay as without it */
+        const int ghost = t <= NEAR_PLANE || alpha0 < 1.0f / 255.0f;
+        const float alpha = ghost ? fmaxf(alpha0, 1.0f / 255.0f) : alpha0;
+        float saved_f[14];
+        double saved_d[6], ghost_acc[3 * 17];
+        if (ghost) {
+          memset(ghost_acc, 0, sizeof ghost_acc);
+          saved_f[0] = T; saved_f[1] = last_alpha;
+          memcpy(saved_f + 2, accum_rec, sizeof accum_rec); memcpy(saved_f + 5, last_color, sizeof last_color);
+          memcpy(saved_f + 8, accum_normal_rec, sizeof accum_normal_rec); memcpy(saved_f + 11, last_normal, sizeof last_normal);
+          memcpy(saved_d, accum_abs, sizeof accum_abs); memcpy(saved_d + 3, accum_normal_abs, sizeof accum_normal_abs);
+        }
         const float max_t = t;
         const float mapped_max_t = (float)((FAR_PLANE * max_t - FAR_PLANE * NEAR_PLANE) / ((FAR_PLANE - NEAR_PLANE) * max_t));
         const float dmax_t_dd = (float)((FAR_PLANE * NEAR_PLANE) / ((FAR_PLANE - NEAR_PLANE) * max_t * max_t));
@@ -521,9 +576,10 @@ void oracle_render_backward(int P, int W, int H, float tan_fovx, float tan_fovy,
         T = T / (1.f - alpha);
         const float dchannel_dcolor = alpha * T;
         float dL_dalpha = 0.0f;
-        double* gacc = my + (size_t)gid * NG;
+        double* gacc = ghost ? ghost_acc : my + (size_t)gid * NS;
         for (int ch = 0; ch < 3; ++ch) {
           const float c = colors[3 * (size_t)gid + ch];
+          accum_abs[ch] = last_alpha * fabs((double)last_color[ch]) + (1. - last_alpha) * accum_abs[ch];
           accum_rec[ch] = last_alpha * last_color[ch] + (1.f - last_alpha) * accum_rec[ch];
           last_color[ch] = c;
           dL_dalpha += (c - accum_rec[ch]) * dL_dpixel[ch];
@@ -532,6 +588,7 @@ void oracle_render_backward(int P, int W, int H, float tan_fovx, float tan_fovy,
         const float dL_dmax_t = 2.0f * (T * alpha) * (mapped_max_t * final_A - final_D) * dL_dreg * dmax_t_dd;
         float dL_dnn[3];
         for (int ch = 0; ch < 3; ++ch) {
+          accum_normal_abs[ch] = last_alpha * fabs((double)last_normal[ch]) + (1. - last_alpha) * accum_normal_abs[ch];
           accum_normal_rec[ch] = last_alpha * last_normal[ch] + (1.f - last_alpha) * accum_normal_rec[ch];
           last_normal[ch] = nn[ch];
           dL_dalpha += (nn[ch] - accum_normal_rec[ch]) * dL_dnormal2D[ch];
@@ -577,16 +634,71 @@ void oracle_render_backward(int P, int W, int H, float tan_fovx, float tan_fovy,
         gacc[14] += (double)(float)(dL_dB * 2 * ry);
         gacc[15] += (double)(float)(dL_dB * 2);
         gacc[16] += (double)(float)dL_dC;
+        if (bounds) {
+          /* the magnitude of every term above, operand by operand */
+          const double Td = T, wT = (double)alpha * T, Gd = G, op = con_o[3];
+          double m[17];
+          double mA = 0, mbg = 0;
+          for (int ch = 0; ch < 3; ++ch) {
+            m[ch] = wT * fabs((double)dL_dpixel[ch]);
+            mA += (fabs((double)colors[3 * (size_t)gid + ch]) + accum_abs[ch]) * fabs((double)dL_dpixel[ch]);
+            mA += (fabs((double)nn[ch]) + accum_normal_abs[ch]) * fabs((double)dL_dnormal2D[ch]);
+            mbg += fabs((double)bg[ch]) * fabs((double)dL_dpixel[ch]);
+          }
+          mA = mA * Td + T_final / (1. - alpha) * mbg;                 /* dL_dalpha */
+          const double mG = op * mA;                                    /* dL_dG */
+          m[3] = mG * Gd * (fabs((double)dx) * fabs((double)con_o[0]) + fabs((double)dy) * fabs((double)con_o[1])) * ddelx_dx;
+          m[4] = mG * Gd * (fabs((double)dy) * fabs((double)con_o[2]) + fabs((double)dx) * fabs((double)con_o[1])) * ddely_dy;
+          m[5] = m[3] + m[4];
+          m[6] = Gd * mA;
+          const double mMin = 0.5 * mG * Gd;                            /* dL_dmin_value */
+          double mDt = 2.0 * wT * (fabs((double)mapped_max_t) * fabs((double)final_A) + fabs((double)final_D)) *
+                       fabs((double)dL_dreg) * fabs((double)dmax_t_dd);
+          if (contributor == (uint32_t)(max_contributor - 1)) mDt += fabs((double)dL_dmax_depth);
+          const double q = fabs(BB / AA);
+          const double mdA = mMin * q * q / 4. + mDt * fabs(BB) / (2 * AA * AA);
+          const double mdB = mMin * q / 2. + mDt / (2 * fabs(AA));
+          const double il = 1.0 / length;
+          double mdnn[3], mlen = 0;
+          for (int ch = 0; ch < 3; ++ch) { mdnn[ch] = wT * fabs((double)dL_dnormal2D[ch]); mlen += mdnn[ch] * fabs((double)normal[ch]); }
+          mlen *= il * il;
+          const double arx = fabs((double)rx), ary = fabs((double)ry);
+          const double mN0 = (mdnn[0] + mlen * fabs((double)normal[0])) * il + mdA * arx;
+          const double mN1 = (mdnn[1] + mlen * fabs((double)normal[1])) * il + mdA * ary;
+          const double mN2 = (mdnn[2] + mlen * fabs((double)normal[2])) * il + mdA;
+          m[7] = mN0 * arx;
+          m[8] = mN0 * ary + mN1 * arx;
+          m[9] = mN0 + mN2 * arx;
+          m[10] = mN1 * ary;
+          m[11] = mN1 + mN2 * ary;
+          m[12] = mN2;
+          m[13] = 2 * mdB * arx;
+          m[14] = 2 * mdB * ary;
+          m[15] = 2 * mdB;
+          m[16] = mMin;
+          for (int i = 0; i < NG; ++i) gacc[NG + i] += m[i];
+          double* gmarg = my + (size_t)gid * NS + 2 * NG;
+          if (ghost || (long)contributor <= marginal_upto)
+            for (int i = 0; i < NG; ++i) gmarg[i] += m[i];
+        }
+        if (ghost) {
+          T = saved_f[0]; last_alpha = saved_f[1];
+          memcpy(accum_rec, saved_f + 2, sizeof accum_rec); memcpy(last_color, saved_f + 5, sizeof last_color);
+          memcpy(accum_normal_rec, saved_f + 8, sizeof accum_normal_rec); memcpy(last_normal, saved_f + 11, sizeof last_normal);
+          memcpy(accum_abs, saved_d, sizeof accum_abs); memcpy(accum_normal_abs, saved_d + 3, sizeof accum_normal_abs);
+        }
       }
     }
   }
 #pragma omp parallel for schedule(static)
   for (int g = 0; g < P; ++g) {
-    double s[17] = {0};
+    double s[3 * 17] = {0};
     for (int t = 0; t < nthreads; ++t) {
-      const double* a = acc + ((size_t)t * P + g) * NG;
-      for (int k = 0; k < NG; ++k) s[k] += a[k];
+      const double* a = acc + ((size_t)t * P + g) * NS;
+      for (int k = 0; k < NS; ++k) s[k] += a[k];
     }
+    if (bounds)
+      for (int k = 0; k < NG; ++k) { mag[(size_t)NG * g + k] = s[NG + k]; marginal[(size_t)NG * g + k] = s[2 * NG + k]; }
     for (int k = 0; k < 3; ++k) dL_dcolors[3 * (size_t)g + k] = (float)s[k];
     for (int k = 0; k < 3; ++k) dL_dmean2D[3 * (size_t)g + k] = (float)s[3 + k];
     dL_dopacity[g] = (float)s[6];

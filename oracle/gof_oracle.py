@@ -140,17 +140,25 @@ def render_forward(scene, g, point_list, ranges):
     return out, final_T, n_contrib
 
 
-def render_backward(scene, g, point_list, ranges, final_T, n_contrib, dL_dpix):
+BOUND_COMPONENTS = 17   # columns of `mag` / `marginal`: dL_dcolors 0-2 | dL_dmean2D 3-5 | dL_dopacity 6 | dL_dv2g 7-16
+
+
+def render_backward(scene, g, point_list, ranges, final_T, n_contrib, dL_dpix, bounds=False):
+    """Blend backward from a given forward state.  bounds=True adds the error scales "mag" and "marginal", [P,17] float64
+    each (see oracle_render_backward); the gradients are the same either way."""
     P, W, H = scene.P, scene.W, scene.H
     d = dict(dL_dmean2D=np.zeros((P, 3), np.float32), dL_dopacity=np.zeros((P, 1), np.float32),
              dL_dcolors=np.zeros((P, 3), np.float32), dL_dv2g=np.zeros((P, 10), np.float32))
+    if bounds:
+        d.update(mag=np.zeros((P, BOUND_COMPONENTS), np.float64), marginal=np.zeros((P, BOUND_COMPONENTS), np.float64))
     _lib.oracle_render_backward(P, W, H, ctypes.c_float(scene.tan_fovx), ctypes.c_float(scene.tan_fovy),
                                 _p(np.ascontiguousarray(ranges, np.uint32)), _p(np.ascontiguousarray(point_list, np.uint32)),
                                 _p(scene.arr["background"]), _p(np.ascontiguousarray(g["means2D"], np.float32)),
                                 _p(np.ascontiguousarray(g["conic_opacity"], np.float32)), _p(np.ascontiguousarray(g["rgb"], np.float32)),
                                 _p(np.ascontiguousarray(g["view2gaussian"], np.float32)), _p(np.ascontiguousarray(final_T, np.float32)),
                                 _p(np.ascontiguousarray(n_contrib, np.uint32)), _p(np.ascontiguousarray(dL_dpix, np.float32)),
-                                _p(d["dL_dmean2D"]), _p(d["dL_dopacity"]), _p(d["dL_dcolors"]), _p(d["dL_dv2g"]))
+                                _p(d["dL_dmean2D"]), _p(d["dL_dopacity"]), _p(d["dL_dcolors"]), _p(d["dL_dv2g"]),
+                                _p(d.get("mag")), _p(d.get("marginal")))
     return d
 
 

@@ -105,6 +105,17 @@ def bwd_args(fa, radii, geom, R, binning, img, grad):
             tfy, ks, subpix, grad, sh, deg, campos, geom, R, binning, img, debug)
 
 
+def same_up_to_summation_order(a, b):
+    """Two backward runs over the same forward state: max|a - b| <= 1e-6 max|b| (test_gpu_repro's criterion).  The blend backward
+    sums each Gaussian's partials in double and rounds once, so the order of its atomics moves a gradient only where a double sum
+    lies next to a float rounding boundary."""
+    a, b = a.double(), b.double()
+    scale = float(b.abs().max()) if b.numel() else 0.0
+    if scale == 0.0:
+        return a.numel() == 0 or float(a.abs().max()) == 0.0
+    return float((a - b).abs().max()) <= 1e-6 * scale
+
+
 def rel_err(a, b):
     """max-abs-diff / max-abs-ref and relative L2 (the parity metric of SURVEY.md section 4.1)."""
     a = a.double().flatten()
