@@ -86,6 +86,66 @@ def make_gaussians(P, seed, focal_x, sh_degree=3, sigma_px=2.0, sigma_spread=0.7
             "sh_degree": sh_degree}
 
 
+class SurfaceView(NamedTuple):
+    """A camera with the attributes of the reference's scene.cameras.Camera that rendering and TSDF fusion read."""
+    image_height: int
+    image_width: int
+    tanfovx: float
+    tanfovy: float
+    world_view_transform: torch.Tensor   # (4,4) = W2V^T
+    projection_matrix: torch.Tensor      # (4,4) = P^T
+    full_proj_transform: torch.Tensor    # (4,4)
+    camera_center: torch.Tensor          # (3,)
+    focal_x: float
+    gt_alpha_mask: object = None
+
+
+def make_surface_views(width, height, n_views, radius=4.0, fovx_deg=60.0, max_elevation=1.2, znear=0.01, zfar=100.0):
+    """`n_views` cameras looking at the origin from rings of make_camera at elevations spread over
+    [-max_elevation, max_elevation] (five rings, more views on the wider rings), so a sphere at the origin is seen all over,
+    poles included."""
+    elevs = [max_elevation * (2.0 * i / 4 - 1.0) for i in range(5)]
+    wts = [math.cos(e) + 0.35 for e in elevs]
+    counts = [max(1, int(round(n_views * w / sum(wts)))) for w in wts]
+    counts[2] += n_views - sum(counts)
+    views = []
+    tan_x = math.tan(math.radians(fovx_deg) / 2.0)
+    proj = _projection(znear, zfar, tan_x, tan_x * height / width).t().contiguous()
+    for ring, (e, n) in enumerate(zip(elevs, counts)):
+        for k in range(n):
+            # successive rings are turned by half a step so that their cameras interleave
+            cam = make_camera(width, height, view=2 * k + ring % 2, n_views=2 * n, radius=radius, fovx_deg=fovx_deg, elevation=e,
+                              znear=znear, zfar=zfar)
+            views.append(SurfaceView(cam.image_height, cam.image_width, cam.tanfovx, cam.tanfovy, cam.world_view_transform, proj,
+                                     cam.full_proj_transform, cam.camera_center, cam.focal_x))
+    return views
+
+
+def make_surface_gaussians(P, seed, radius=1.0, sigma=None, opacity=0.98):
+    """P flat Gaussians tangent to a sphere of `radius` at the origin: scales (sigma, sigma, 0.05 sigma) with the thin axis
+    along the normal, opacities `opacity`, and a colour that varies smoothly with the position (SH degree 0), so that
+    the rendered median depth is a real surface.  sigma defaults to the mean spacing of the centres.  Drawn in float64,
+    rounded to float32 once (see make_gaussians)."""
+    g = torch.Generator().manual_seed(int(seed))
+    f64 = torch.float64
+    n = torch.randn(P, 3, generator=g, dtype=f64)
+    n = n / n.norm(dim=1, keepdim=True)
+    if sigma is None:
+        sigma = math.sqrt(4.0 * math.pi * radius * radius / P)
+    scales = torch.tensor([sigma, sigma, 0.05 * sigma], dtype=f64).expand(P, 3)
+    # the rotation taking +z to n: q = (1 + n.z, (+z) x n) normalised
+    q = torch.stack([1.0 + n[:, 2], -n[:, 1], n[:, 0], torch.zeros(P, dtype=f64)], dim=1)
+    qn = q.norm(dim=1, keepdim=True)
+    flip = qn[:, 0] < 1e-9                     # n = -z: a half turn about x
+    q = torch.where(flip[:, None], torch.tensor([0.0, 1.0, 0.0, 0.0], dtype=f64), q / qn.clamp_min(1e-30))
+    shs = torch.zeros(P, 16, 3, dtype=f64)
+    rgb = 0.5 + 0.4 * torch.stack([n[:, 0], n[:, 1] * n[:, 2], torch.cos(3.0 * n[:, 1])], dim=1)
+    shs[:, 0, :] = (rgb - 0.5) / 0.28209479177387814
+    f32 = lambda t: t.to(torch.float32).contiguous()   # noqa: E731
+    return {"means3D": f32(n * radius), "scales": f32(scales), "rotations": f32(q), "opacities": torch.full((P, 1), float(opacity)),
+            "shs": f32(shs), "sh_degree": 0}
+
+
 # the configurations of BASELINE.json / BASELINE.md section 2.2
 CONFIGS = {
     "C1": dict(P=10_000, width=256, height=256, seed=0),

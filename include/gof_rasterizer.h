@@ -207,6 +207,53 @@ GOF_API int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_
                                    const float* vertices, const float* scales,
                                    float* edge_pos, float* edge_sdf, float* edge_scales, void* stream);
 
+/* TSDF fusion of rendered depth into a sparse voxel-block volume and marching-cubes extraction (extract_mesh_tsdf.py:16-83,
+ * which uses Open3D's VoxelBlockGrid; the specification is DESIGN section 4.4).  Stateless: the caller owns the block table
+ * (block keys sorted ascending + the pool slot of each block) and the voxel pool [slots][5][B^3] float32 (tsdf, weight,
+ * colour r, g, b planes per block, voxel i + B j + B^2 k).  A block key packs block coordinates (bx, by, bz), each in
+ * [-2^20, 2^20), as (bz + 2^20) << 42 | (by + 2^20) << 21 | (bx + 2^20); a touched block outside that range fails with
+ * GOF_E_INVALID.  Sizes that depend on the data come from a count call, then the caller allocates and calls emit with the
+ * count call's scratch. */
+typedef struct {
+  float voxel_size;       /* s */
+  int block_resolution;   /* B, 1..64 */
+  float trunc;            /* tau = fl(trunc_voxel_multiplier * s) */
+  float depth_max;
+} gof_tsdf_params_t;
+typedef struct {
+  int width, height;
+  float fx, fy, cx, cy;
+  float extrinsic[12];    /* world -> camera [R | t], row-major 3x4 */
+} gof_tsdf_camera_t;
+/* Touch: the sorted unique keys of the blocks within tau of the unprojected depth of every 4th pixel in x and y with
+ * 0 < depth < depth_max.  depth: [H,W] float32 (0 = none). */
+GOF_API int gof_tsdf_touch_count(const gof_tsdf_params_t* params, const gof_tsdf_camera_t* cam, const float* depth,
+                                 gof_alloc_fn scratch_alloc, void* scratch_user, int64_t* num_blocks_out, void* stream);
+GOF_API int gof_tsdf_touch_emit(const gof_tsdf_params_t* params, const gof_tsdf_camera_t* cam, void* scratch, int64_t num_blocks,
+                                int64_t* keys_out, void* stream);
+/* Activate: merge a view's sorted unique keys into the table.  count returns how many are new; emit writes the merged table
+ * (out_keys / out_slots, num_table + num_new entries, must not alias the inputs; new blocks take slots num_table,
+ * num_table + 1, ... in key order, which the caller must have zeroed) and the pool slot of every view block. */
+GOF_API int gof_tsdf_activate_count(int64_t num_table, const int64_t* table_keys, int64_t num_view, const int64_t* view_keys,
+                                    gof_alloc_fn scratch_alloc, void* scratch_user, int64_t* num_new_out, void* stream);
+GOF_API int gof_tsdf_activate_emit(int64_t num_table, const int64_t* table_keys, const int32_t* table_slots, int64_t num_view,
+                                   const int64_t* view_keys, void* scratch, int64_t num_new, int64_t* out_keys, int32_t* out_slots,
+                                   int32_t* view_slots, void* stream);
+/* Integrate one view into the voxels of its blocks (view_keys / view_slots from touch + activate).  depth [H,W],
+ * color [3,H,W] float32.  num_updates (optional, device uint64) accumulates the number of voxels updated. */
+GOF_API int gof_tsdf_integrate(const gof_tsdf_params_t* params, const gof_tsdf_camera_t* cam, const float* depth, const float* color,
+                               int64_t num_view, const int64_t* view_keys, const int32_t* view_slots, float* pool,
+                               unsigned long long* num_updates, void* stream);
+/* Marching cubes over the whole table (cubes whose 8 corners exist with weight > weight_threshold).  count returns the
+ * vertex and face counts; emit writes vertices [V,3], colors [V,3] float32 and faces [F,3] int64 in canonical order. */
+GOF_API int gof_tsdf_extract_count(const gof_tsdf_params_t* params, int64_t num_table, const int64_t* table_keys,
+                                   const int32_t* table_slots, const float* pool, float weight_threshold, gof_alloc_fn scratch_alloc,
+                                   void* scratch_user, int64_t* num_vertices_out, int64_t* num_faces_out, void* stream);
+GOF_API int gof_tsdf_extract_emit(const gof_tsdf_params_t* params, int64_t num_table, const int64_t* table_keys,
+                                  const int32_t* table_slots, const float* pool, float weight_threshold, void* scratch,
+                                  int64_t num_vertices, int64_t num_faces, float* vertices, float* colors, int64_t* faces,
+                                  void* stream);
+
 /* Launch accounting and live per-kernel timing (CUDA events on the launching stream; not a profiler).
  * gof_launch_count(): kernels launched by this library so far.  gof_profile_report(): lines of
  * "<kernel> <launches> <total_ms>" accumulated while profiling was enabled. */

@@ -4,7 +4,7 @@
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python tools/sanitize_run.py [parts...]
 
 parts: render (forward + backward, SH and precomputed-colour paths, multi-batch tile lists), integrate, tetmesh, loss,
-params, filter.  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
+params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
 import os
 import sys
 
@@ -91,7 +91,25 @@ def filt(dev):
     print("filter mean", float(out.mean()), flush=True)
 
 
-PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt}
+def tsdf(dev):
+    import gof_tsdf
+    # a few 64x48 views with B = 8: noisy depth around a plane (ambiguous cubes, blocks shared between views), one view with no
+    # depth, a pool that starts at one block and grows; then the whole extraction
+    rng = np.random.default_rng(5)
+    vol = gof_tsdf.TSDFVolume(voxel_size=0.05, block_resolution=8, block_count=1, device=dev)
+    for i in range(6):
+        d = (3.0 + 0.15 * rng.standard_normal((48, 64))).astype(np.float32)
+        if i == 3:
+            d[:] = 0
+        E = np.eye(4, dtype=np.float32)
+        E[:3, 3] = rng.normal(0, 0.05, 3)
+        vol.integrate(torch.from_numpy(d).to(dev), torch.rand(3, 48, 64, device=dev), 40.0, 40.0, 31.5, 23.5, E)
+    mesh = vol.extract_triangle_mesh(3.0)
+    torch.cuda.synchronize()
+    print("tsdf blocks", vol.num_blocks, "V", tuple(mesh["vertices"].shape), "F", tuple(mesh["faces"].shape), flush=True)
+
+
+PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf}
 
 if __name__ == "__main__":
     dev = torch.device("cuda")
