@@ -137,7 +137,6 @@ int gof_read_back(void* dst, const void* src_dev, size_t bytes, cudaStream_t st)
 // itself sums tiles_touched; the 4-byte copy runs on a side stream as soon as that kernel has finished, while the launching
 // stream carries on with the depth sort, and the host waits for the copy only: by the time it has sized the buffer and queued
 // the emit kernel the GPU is still busy sorting.
-bool gof_binning_legacy();
 namespace {
 struct SideCopy { cudaStream_t st = nullptr; cudaEvent_t after_kernel = nullptr, copied = nullptr; uint32_t* pin = nullptr; bool ok = false, tried = false; };
 SideCopy* side_copy_for_current_device() {
@@ -181,8 +180,8 @@ static int preprocess_sort_count(const gof_scene_t* s, const GofView& v, char* g
                                  cudaStream_t st, uint32_t* R) {
   int rc;
   if ((rc = gof_launch_preprocess(s, v, geom, GL, radii, st)) != GOF_OK) return rc;
-  SideCopy* sc = (gof_binning_legacy() || s->debug) ? nullptr : begin_async_read_u32(geom + GL.total, st);
-  if ((rc = gof_depth_sort_and_offsets(s->P, geom, GL, s->debug != 0, st)) != GOF_OK) return rc;
+  SideCopy* sc = s->debug ? nullptr : begin_async_read_u32(geom + GL.total, st);
+  if ((rc = gof_depth_sort(s->P, geom, GL, s->debug != 0, st)) != GOF_OK) return rc;
   if (sc) return finish_async_read_u32(sc, R);
   return gof_read_back(R, geom + GL.total, sizeof(uint32_t), st);
 }

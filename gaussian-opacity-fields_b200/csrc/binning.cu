@@ -14,30 +14,10 @@
 // obtains the number of keys with the same digit in all earlier chunks by decoupled look-back over single-word
 // (flag | count) status entries, reorders the chunk in shared memory and writes digit runs coalesced.  Positions are a
 // pure function of the input (no atomic decides an output position; the only atomic hands out chunk numbers in launch
-// order so that a chunk never waits for one that has not started).  Round 1 used histogram + row scan + scatter
-// launches per pass and a three-kernel scan: 26 launches, 0.44 ms at the benchmark workload; kept in binning_legacy.cu
-// behind GOF_BINNING=legacy.
-#include <stdlib.h>
-
+// order so that a chunk never waits for one that has not started).  This replaced a design with histogram + row scan +
+// scatter launches per pass and a three-kernel scan: 26 launches and 0.44 ms at the benchmark workload, against 10 launches
+// and 0.25 ms (DESIGN §4.1); that code is in the repository history.
 #include "gof_common.cuh"
-
-// binning_legacy.cu
-int legacy_gof_depth_sort_and_offsets(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st);
-int legacy_gof_sort_points_by_tile(size_t n, int nbits, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist,
-                                   uint2* ranges, int num_tiles, bool debug, cudaStream_t st, int* result_in_b);
-int legacy_gof_sort_pairs_u32(uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist, size_t n, int nbits, bool debug,
-                              cudaStream_t st, int* result_in_b);
-int legacy_gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n, bool debug, cudaStream_t st);
-int legacy_gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin,
-                         const GofBinLayout& BL, char* img, const GofImageLayout& IL, bool debug, cudaStream_t st);
-
-static int g_binning_legacy = -1;
-bool gof_binning_legacy() {
-  if (g_binning_legacy < 0) { const char* e = getenv("GOF_BINNING"); g_binning_legacy = (e && e[0] == 'l') ? 1 : 0; }
-  return g_binning_legacy == 1;
-}
-// test / A-B hook: 1 = the round-1 multi-launch binning (binning_legacy.cu), 0 = one-sweep passes (default)
-extern "C" GOF_API void gof_set_binning_legacy(int on) { g_binning_legacy = on ? 1 : 0; }
 
 namespace {
 
@@ -501,8 +481,7 @@ int bin_tiles_t(int P, size_t R, const GofView& v, char* geom, const GofGeomLayo
 
 // Stable sort of the P (depth bits, gaussian id) pairs written by the preprocess kernel into key_a/val_a; 4 passes ->
 // result back in *_a.  (The scan of tiles_touched in that order happens inside the emit kernel, gof_bin_tiles.)
-int gof_depth_sort_and_offsets(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st) {
-  if (gof_binning_legacy()) return legacy_gof_depth_sort_and_offsets(P, geom, L, debug, st);
+int gof_depth_sort(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st) {
   int in_b = 0;
   return sort_pairs<uint32_t>(reinterpret_cast<uint32_t*>(geom + L.key_a), reinterpret_cast<uint32_t*>(geom + L.key_b),
                               reinterpret_cast<uint32_t*>(geom + L.val_a), reinterpret_cast<uint32_t*>(geom + L.val_b),
@@ -514,10 +493,6 @@ int gof_depth_sort_and_offsets(int P, char* geom, const GofGeomLayout& L, bool d
 // sentinel id given to points outside the image).  Buffers: keys/vals ping-pong (u32), scratch as in gof_sort_scratch_bytes.
 int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist,
                             uint2* ranges, int num_tiles, bool debug, cudaStream_t st, int* result_in_b) {
-  if (gof_binning_legacy()) {
-    if (key_shift != 0) { gof_set_error("legacy binning sorts plain tile ids"); return GOF_E_INVALID; }
-    return legacy_gof_sort_points_by_tile(n, nbits, ka, kb, va, vb, hist, ranges, num_tiles, debug, st, result_in_b);
-  }
   GOF_CUDA_OK(cudaMemsetAsync(ranges, 0, (size_t)(num_tiles + 1) * sizeof(uint2), st));
   *result_in_b = 0;
   if (n == 0) return GOF_OK;
@@ -533,13 +508,11 @@ int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, ui
 // *result_in_b tells where the result is.  hist: gof_sort_scratch_bytes(n).
 int gof_sort_pairs_u32(uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist, size_t n, int nbits, bool debug,
                        cudaStream_t st, int* result_in_b) {
-  if (gof_binning_legacy()) return legacy_gof_sort_pairs_u32(ka, kb, va, vb, hist, n, nbits, debug, st, result_in_b);
   return sort_pairs<uint32_t>(ka, kb, va, vb, hist, n, nbits, debug, st, result_in_b);
 }
 
 // exclusive scan of n u32 (in != out allowed); total (if non-NULL) receives the sum; tmp: n/2048 + 4 u32
 int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n, bool debug, cudaStream_t st) {
-  if (gof_binning_legacy()) return legacy_gof_exclusive_scan_u32(in, out, tmp, total, n, debug, st);
   if (n == 0) {
     if (total) GOF_CUDA_OK(cudaMemsetAsync(total, 0, 4, st));
     return GOF_OK;
@@ -553,7 +526,6 @@ int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uin
 
 int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin, const GofBinLayout& BL,
                   char* img, const GofImageLayout& IL, bool debug, cudaStream_t st) {
-  if (gof_binning_legacy()) return legacy_gof_bin_tiles(P, R, v, geom, GL, bin, BL, img, IL, debug, st);
   if (BL.key_bytes == 2) return bin_tiles_t<uint16_t>(P, R, v, geom, GL, bin, BL, img, IL, debug, st);
   return bin_tiles_t<uint32_t>(P, R, v, geom, GL, bin, BL, img, IL, debug, st);
 }

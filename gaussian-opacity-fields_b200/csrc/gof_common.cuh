@@ -177,16 +177,10 @@ static constexpr inline int gof_sort_blocks(size_t n) { return (int)((n + GOF_SO
 static constexpr inline size_t gof_sort_scratch_bytes(size_t n) {
   return (size_t)GOF_SORT_HEAD_BYTES + (size_t)4 * ((size_t)gof_sort_blocks(n) + 8) * GOF_RADIX * 4;
 }
-// The round-1 kernels (binning_legacy.cu, GOF_BINNING=legacy) use the same scratch as a [256][c] histogram and 256 digit
-// totals: 256 * (c + 1) words.  Both sizes are affine in c, so holding at both ends of the range of n holds for every n in it.
-static_assert(gof_sort_scratch_bytes(1) >= (size_t)GOF_RADIX * (gof_sort_blocks(1) + 1) * 4 &&
-                  gof_sort_scratch_bytes((size_t)1 << 40) >= (size_t)GOF_RADIX * (gof_sort_blocks((size_t)1 << 40) + 1) * 4,
-              "the legacy radix passes' histogram and digit totals must fit in gof_sort_scratch_bytes");
 
 struct GofGeomLayout {      // "geomBuffer": everything sized by P
   size_t splat, splat_bwd, rect, tiles, clamped, depth;
   size_t key_a, key_b, val_a, val_b;   // depth radix sort ping-pong
-  size_t offsets;                      // inclusive scan of tiles_touched in depth order (legacy binning only)
   size_t hist;                         // radix sort scratch (gof_sort_scratch_bytes)
   size_t scan_tmp;                     // scan block sums / look-back status words
   size_t total;                        // u32 num_rendered (device copy)
@@ -209,7 +203,6 @@ static inline GofGeomLayout gof_geom_layout(size_t P) {
   L.key_b = take(P * 4);
   L.val_a = take(P * 4);
   L.val_b = take(P * 4);
-  L.offsets = take(P * 4);
   L.hist = take(gof_sort_scratch_bytes(P));
   L.scan_tmp = take((P / 256 + 8) * 4 + 4096);      // look-back status words of the fused scan+emit kernel (one per 256 Gaussians) + ticket
   L.total = take(256);
@@ -321,11 +314,9 @@ int gof_launch_mark_visible(int P, const float* means3D, const float* vm, unsign
 int gof_sort_pairs_u32(uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist, size_t n, int nbits, bool debug,
                        cudaStream_t st, int* result_in_b);
 int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n, bool debug, cudaStream_t st);
-int gof_depth_sort_and_offsets(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st);
+int gof_depth_sort(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st);
 int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin,
                   const GofBinLayout& BL, char* img, const GofImageLayout& IL, bool debug, cudaStream_t st);
-
-bool gof_binning_legacy();
 int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist,
                             uint2* ranges, int num_tiles, bool debug, cudaStream_t st, int* result_in_b);
 

@@ -18,9 +18,10 @@
 
 namespace {
 
+constexpr int PT_KEY_SHIFT = 8;   // point key = tile << 8 | pixel slot inside the tile (points of one pixel become neighbours)
+
 struct PtArgs {
   int PN, W, H, grid_x, grid_y, tiles;
-  int key_shift;   // 8: key = tile << 8 | pixel slot inside the tile (points of one pixel become neighbours); 0: key = tile
   float focal_x, focal_y;
   const float* points3D;
   const float* vm;
@@ -36,7 +37,7 @@ __global__ void __launch_bounds__(256) k_preprocess_points(const PtArgs a) {
   if (idx >= a.PN) return;
   const float px = a.points3D[3 * (size_t)idx], py = a.points3D[3 * (size_t)idx + 1], pz = a.points3D[3 * (size_t)idx + 2];
   const float* vm = a.vm;
-  uint32_t key = (uint32_t)a.tiles << a.key_shift;   // sentinel: not projected
+  uint32_t key = (uint32_t)a.tiles << PT_KEY_SHIFT;   // sentinel: not projected
   const float tz = gof_affine(px, py, pz, __ldg(vm + 2), __ldg(vm + 6), __ldg(vm + 10), __ldg(vm + 14));
   if (!(tz <= 0.2f)) {
     const float tx = gof_affine(px, py, pz, __ldg(vm + 0), __ldg(vm + 4), __ldg(vm + 8), __ldg(vm + 12));
@@ -50,14 +51,11 @@ __global__ void __launch_bounds__(256) k_preprocess_points(const PtArgs a) {
       int cx = gof_f2i_rz(x * 0.0625f), cy = gof_f2i_rz(y * 0.0625f);
       cx = min(a.grid_x - 1, max(0, cx));
       cy = min(a.grid_y - 1, max(0, cy));
-      key = (uint32_t)(cy * a.grid_x + cx);
-      if (a.key_shift) {
-        // the thread slot of the pixel the point falls in (same mapping as k_integrate's pass 2): sorting on it makes the points
-        // of one pixel -- which replay the SAME contributor list -- neighbours, so a warp's record gathers coincide
-        int lx = gof_f2i_rz(x) - cx * 16, ly = gof_f2i_rz(y) - cy * 16;
-        lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
-        key = (key << a.key_shift) | (uint32_t)(((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7));
-      }
+      // the thread slot of the pixel the point falls in (same mapping as k_integrate's pass 2): sorting on it makes the points
+      // of one pixel -- which replay the SAME contributor list -- neighbours, so a warp's record gathers coincide
+      int lx = gof_f2i_rz(x) - cx * 16, ly = gof_f2i_rz(y) - cy * 16;
+      lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
+      key = ((uint32_t)(cy * a.grid_x + cx) << PT_KEY_SHIFT) | (uint32_t)(((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7));
     }
   }
   a.key[idx] = key;
@@ -317,12 +315,11 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
   uint32_t* va = reinterpret_cast<uint32_t*>(pbin + PBL.val_a);
   uint32_t* vb = reinterpret_cast<uint32_t*>(pbin + PBL.val_b);
   pa.key = ka; pa.val = va;
-  pa.key_shift = gof_binning_legacy() ? 0 : 8;
   GOF_LAUNCH("preprocess_points", st, k_preprocess_points<<<(PN + 255) / 256, 256, 0, st>>>(pa));
   GOF_LAUNCH_CHECK(debug, st);
   int in_b = 0;
   uint2* pranges = reinterpret_cast<uint2*>(pbin + PBL.pranges);
-  int rc = gof_sort_points_by_tile((size_t)PN, gof_bits_for(((uint32_t)v.tiles + 1u) << pa.key_shift), pa.key_shift, ka, kb, va, vb,
+  int rc = gof_sort_points_by_tile((size_t)PN, gof_bits_for(((uint32_t)v.tiles + 1u) << PT_KEY_SHIFT), PT_KEY_SHIFT, ka, kb, va, vb,
                                    reinterpret_cast<uint32_t*>(pbin + PBL.hist), pranges, v.tiles, debug, st, &in_b);
   if (rc != GOF_OK) return rc;
 

@@ -344,10 +344,6 @@ GOF_API int gof_conv3x3_wgrad(int CO, int CI, int H, int W, const float* x, cons
 GOF_API int gof_adam_step(size_t n, float* param, float* exp_avg, float* exp_avg_sq, const float* grad, double lr, double beta1,
                           double beta2, double eps, int step, void* stream);
 
-/* Test / A-B hook: 1 selects the round-1 binning kernels (three launches per radix pass), 0 the one-sweep passes (default;
- * also selectable with GOF_BINNING=legacy in the environment).  Results are identical. */
-GOF_API void gof_set_binning_legacy(int on);
-
 GOF_API const char* gof_last_error(void);
 GOF_API int gof_version(void);
 
