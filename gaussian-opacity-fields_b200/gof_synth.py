@@ -232,3 +232,83 @@ def raster_settings(cam, sh_degree, device, kernel_size=0.0, scale_modifier=1.0,
         bg=torch.tensor(bg, dtype=torch.float32, device=device), scale_modifier=scale_modifier,
         viewmatrix=cam.world_view_transform.to(device), projmatrix=cam.full_proj_transform.to(device),
         sh_degree=sh_degree, campos=cam.camera_center.to(device), prefiltered=False, debug=debug)
+
+
+POINT_CLOUD_KINDS = ("uniform", "colmap", "plane", "lattice", "core", "tiny", "huge", "nonfinite")
+
+
+def make_point_cloud(kind, P, seed):
+    """Seeded float32 [P,3] numpy point cloud for the distCUDA2 tests (simple_knn).  Generated in float64 with numpy's
+    default_rng and rounded to float32 once, so the bytes are the same on every host (torch's CPU generator is not: its
+    normal sampler differs in the last ulp between AVX2 and AVX-512 builds, DESIGN section 5).
+
+    uniform    the cube [-1, 1]^3
+    colmap     a few noisy surfaces (planes and a sphere) as a structure-from-motion cloud has them, ~1 % outliers at
+               100-1000x the scene radius and ~2 % exact duplicates of other points
+    plane      z = 0 exactly (zero extent on one axis)
+    lattice    points of an integer grid in shuffled order: every distance is an integer, so ties are everywhere
+    core       all but 8 points in a unit cube, 8 outliers at ~1e6: the core spans ~1e-6 of the bounding box
+    tiny       a cube of side 4e-18 whose points come in pairs ~1e-21 apart: nearest squared distances are subnormal
+    huge       |x| in 1e19 .. 1e30 with random signs (most squared distances overflow) plus tight pairs around 1e19
+    nonfinite  the uniform cube with ~3 % of the rows holding NaN, +inf or -inf in one or more coordinates
+    """
+    import numpy as np
+    rng = np.random.default_rng([seed, POINT_CLOUD_KINDS.index(kind)])
+    P = int(P)
+    if kind == "uniform":
+        x = rng.uniform(-1.0, 1.0, (P, 3))
+    elif kind == "colmap":
+        n_sphere = P // 3
+        d = rng.normal(size=(n_sphere, 3))
+        sphere = d / np.linalg.norm(d, axis=1, keepdims=True) * 1.5 + np.array([0.3, -0.2, 0.5])
+        rest = P - n_sphere
+        which = rng.integers(0, 3, rest)
+        uv = rng.uniform(-4.0, 4.0, (rest, 2))
+        planes = np.zeros((rest, 3))
+        planes[which == 0] = np.c_[uv[which == 0], np.full((which == 0).sum(), -2.0)]            # floor
+        planes[which == 1] = np.c_[uv[which == 1, 0], np.full((which == 1).sum(), 4.0), uv[which == 1, 1]]   # wall
+        planes[which == 2] = np.c_[np.full((which == 2).sum(), -4.0), uv[which == 2]]           # wall
+        x = np.concatenate([sphere, planes]) + rng.normal(scale=0.01, size=(P, 3))
+        x = x[rng.permutation(P)]
+        n_out = P // 100
+        if n_out:
+            d = rng.normal(size=(n_out, 3))
+            r = 4.0 * 10.0 ** rng.uniform(2.0, 3.0, n_out)
+            x[rng.choice(P, n_out, replace=False)] = d / np.linalg.norm(d, axis=1, keepdims=True) * r[:, None]
+        n_dup = P // 50
+        if n_dup:
+            x[rng.choice(P, n_dup, replace=False)] = x[rng.choice(P, n_dup, replace=True)]
+    elif kind == "plane":
+        x = np.c_[rng.uniform(-1.0, 1.0, (P, 2)), np.zeros(P)]
+    elif kind == "lattice":
+        n = max(1, int(math.ceil(round(P ** (1.0 / 3.0), 9))))
+        g = np.stack(np.meshgrid(np.arange(n), np.arange(n), np.arange(n), indexing="ij"), -1).reshape(-1, 3)[:P]
+        x = g[rng.permutation(P)].astype(np.float64) - n // 2
+    elif kind == "core":
+        x = rng.uniform(0.0, 1.0, (P, 3)) + np.array([0.25, -0.5, 0.75])
+        k = min(8, P)
+        d = rng.normal(size=(k, 3))
+        x[rng.choice(P, k, replace=False)] = d / np.linalg.norm(d, axis=1, keepdims=True) * 1.0e6
+    elif kind == "tiny":
+        x = rng.uniform(-2.0e-18, 2.0e-18, (P, 3))
+        half = P // 2
+        x[1::2] = x[0:2 * half:2] + rng.uniform(-1.0e-21, 1.0e-21, (half, 3))   # partners at subnormal squared distance
+        x = x[rng.permutation(P)]
+    elif kind == "huge":
+        x = rng.choice([-1.0, 1.0], (P, 3)) * 10.0 ** rng.uniform(19.0, 30.0, (P, 3))
+        half = P // 2
+        x[:half] = 1.0e19 * (1.0 + rng.uniform(-0.05, 0.05, (half, 3))) * rng.choice([-1.0, 1.0], (half, 1))
+        x = x[rng.permutation(P)]
+    elif kind == "nonfinite":
+        x = rng.uniform(-1.0, 1.0, (P, 3))
+        n_bad = max(1, (3 * P) // 100) if P else 0
+        rows = rng.choice(P, n_bad, replace=False)
+        mask = rng.random((n_bad, 3)) < 0.5
+        mask[np.arange(n_bad), rng.integers(0, 3, n_bad)] = True
+        vals = rng.choice(np.array([np.nan, np.inf, -np.inf]), (n_bad, 3))
+        sub = x[rows]
+        sub[mask] = vals[mask]
+        x[rows] = sub
+    else:
+        raise ValueError(f"unknown point cloud kind {kind!r}; one of {POINT_CLOUD_KINDS}")
+    return np.ascontiguousarray(x.reshape(P, 3).astype(np.float32))

@@ -344,6 +344,24 @@ GOF_API int gof_conv3x3_wgrad(int CO, int CI, int H, int W, const float* x, cons
 GOF_API int gof_adam_step(size_t n, float* param, float* exp_avg, float* exp_avg_sq, const float* grad, double lr, double beta1,
                           double beta2, double eps, int step, void* stream);
 
+/* simple_knn's distCUDA2 (submodules/simple-knn/spatial.cu:15-25, simple_knn.cu:147-183), which GaussianModel.create_from_pcd
+ * (scene/gaussian_model.py:327) uses to initialise the scales: for every point i of points [P,3] (device, float32) the mean
+ * squared distance to its three nearest neighbours, bit-identical to the reference (DESIGN section 4.5):
+ *   d(i,j) = fmaf(dz, dz, fmaf(dx, dx, dy*dy)), dx = x_j - x_i, ...  (updateKBest, simple_knn.cu:132-145: nvcc contracts
+ *   d.x*d.x + d.y*d.y + d.z*d.z to FMUL of dy, FFMA of dx, FFMA of dz)
+ *   over all j != i BY INDEX (coincident points count, at distance 0); d is accepted only if d < FLT_MAX, so NaN and inf
+ *   never enter; b0 <= b1 <= b2 = the three smallest accepted distances, padded with FLT_MAX;
+ *   mean_dists[i] = ((b0 + b1) + b2) / 3.0f, IEEE adds and a correctly rounded divide (simple_knn.cu:182).
+ * Hence P = 1, 2 and points with a non-finite coordinate give +inf, and such points are nobody's neighbour.  The reference's
+ * pruning is exact, so its output does not depend on its search order; this library searches a Morton-ordered 32-ary box
+ * tree instead of testing every 1024-point box (simple_knn.cu:168-181).  Scratch: gof_knn_scratch_bytes(P) device bytes,
+ * 256-byte aligned, contents irrelevant.  No allocation and no host synchronisation (the call can be captured in a CUDA
+ * graph); kernels run on `stream`.  P = 0 launches nothing; P < 0 fails with GOF_E_INVALID (the reference's int P bounds
+ * P below 2^31). */
+GOF_API size_t gof_knn_scratch_bytes(int P);
+GOF_API int gof_knn_mean_dist(int P, const float* points /*[P,3]*/, float* mean_dists /*[P]*/, void* scratch, size_t scratch_bytes,
+                              void* stream);
+
 GOF_API const char* gof_last_error(void);
 GOF_API int gof_version(void);
 

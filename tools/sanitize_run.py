@@ -4,7 +4,8 @@
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python tools/sanitize_run.py [parts...]
 
 parts: render (forward + backward, SH and precomputed-colour paths, multi-batch tile lists), integrate, tetmesh, loss,
-params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
+params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), knn (distCUDA2 on clouds of
+1-4097 points, coincident and non-finite rows included).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
 import os
 import sys
 
@@ -109,7 +110,16 @@ def tsdf(dev):
     print("tsdf blocks", vol.num_blocks, "V", tuple(mesh["vertices"].shape), "F", tuple(mesh["faces"].shape), flush=True)
 
 
-PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf}
+def knn(dev):
+    from simple_knn._C import distCUDA2
+    for kind, P in (("colmap", 4097), ("nonfinite", 1025), ("lattice", 33), ("uniform", 1)):
+        out = distCUDA2(torch.from_numpy(gof_synth.make_point_cloud(kind, P, seed=3)).to(dev))
+        torch.cuda.synchronize()
+        print("knn", kind, P, "finite", int(torch.isfinite(out).sum()), flush=True)
+
+
+PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf,
+         "knn": knn}
 
 if __name__ == "__main__":
     dev = torch.device("cuda")
