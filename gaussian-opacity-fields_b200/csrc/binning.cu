@@ -17,6 +17,9 @@
 // order so that a chunk never waits for one that has not started).  This replaced a design with histogram + row scan +
 // scatter launches per pass and a three-kernel scan: 26 launches and 0.44 ms at the benchmark workload, against 10 launches
 // and 0.25 ms (DESIGN §4.1); that code is in the repository history.
+// The same passes sort the wider keys of the extraction paths (tetmesh, TSDF, kNN): gof_sort_words_u32 sorts by a key of up
+// to three u32 words, one stable sort per word on the previous word's order, and gof_key_runs_u32 numbers the runs of equal
+// keys in that order.
 #include "gof_common.cuh"
 
 namespace {
@@ -29,36 +32,6 @@ constexpr uint32_t LB_VAL = (1u << 30) - 1u;
 
 __device__ __forceinline__ uint32_t ld_volatile(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
 __device__ __forceinline__ void st_volatile(uint32_t* p, uint32_t v) { *reinterpret_cast<volatile uint32_t*>(p) = v; }
-
-__device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v) {
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t n = __shfl_up_sync(0xffffffffu, v, d);
-    if ((threadIdx.x & 31) >= d) v += n;
-  }
-  return v;
-}
-
-// block-wide exclusive scan of one value per thread (256 threads); total in *total.  Ends with a barrier.
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total) {
-  __shared__ uint32_t s_warp[WARPS];
-  __shared__ uint32_t s_total;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t incl = warp_incl_scan(v);
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    const uint32_t w = lane < WARPS ? s_warp[lane] : 0u;
-    const uint32_t wi = warp_incl_scan(w);
-    if (lane < WARPS) s_warp[lane] = wi - w;
-    if (lane == WARPS - 1) s_total = wi;
-  }
-  __syncthreads();
-  const uint32_t r = s_warp[warp] + incl - v;
-  *total = s_total;
-  __syncthreads();
-  return r;
-}
 
 // Decoupled look-back: a chunk publishes its aggregate in a status word (flag | count, written and read as ONE word), walks
 // back over its predecessors' words until one carries an inclusive prefix, then publishes its own inclusive prefix.
@@ -320,10 +293,7 @@ int sort_pairs(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, uint32_t* scratch
 }
 
 // ------------------------------------------------------------------------------------------------
-// single-launch exclusive scan of u32 (decoupled look-back); chunk = 2048 values per CTA
-constexpr int SCAN_ITEMS = 8;
-constexpr int SCAN_CHUNK = THREADS * SCAN_ITEMS;
-
+// single-launch exclusive scan of u32 (decoupled look-back); chunk = GOF_SCAN_CHUNK values per CTA
 __global__ void __launch_bounds__(THREADS) k_scan_excl(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, size_t n,
                                                       uint32_t* __restrict__ status, uint32_t* __restrict__ ticket,
                                                       uint32_t* __restrict__ total_out, uint32_t nchunks) {
@@ -331,11 +301,11 @@ __global__ void __launch_bounds__(THREADS) k_scan_excl(const uint32_t* __restric
   if (threadIdx.x == 0) s_chunk = atomicAdd(ticket, 1u);
   __syncthreads();
   const uint32_t chunk = s_chunk;
-  const size_t base = (size_t)chunk * SCAN_CHUNK + (size_t)threadIdx.x * SCAN_ITEMS;
-  uint32_t v[SCAN_ITEMS];
+  const size_t base = (size_t)chunk * GOF_SCAN_CHUNK + (size_t)threadIdx.x * GOF_SCAN_ITEMS;
+  uint32_t v[GOF_SCAN_ITEMS];
   uint32_t s = 0;
 #pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; ++k) {
+  for (int k = 0; k < GOF_SCAN_ITEMS; ++k) {
     v[k] = (base + k < n) ? in[base + k] : 0u;
     s += v[k];
   }
@@ -351,7 +321,7 @@ __global__ void __launch_bounds__(THREADS) k_scan_excl(const uint32_t* __restric
   __syncthreads();
   run += s_prefix;
 #pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; ++k) {
+  for (int k = 0; k < GOF_SCAN_ITEMS; ++k) {
     if (base + k < n) out[base + k] = run;
     run += v[k];
   }
@@ -477,6 +447,41 @@ int bin_tiles_t(int P, size_t R, const GofView& v, char* geom, const GofGeomLayo
   return GOF_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Multi-word keys: one stable sort per word, least significant first, each on the previous word's order
+
+// values = identity; ka = w0 (nullptr: w0 is ka already)
+__global__ void __launch_bounds__(THREADS) k_sort_init(size_t n, const uint32_t* __restrict__ w0, uint32_t* __restrict__ ka,
+                                                      uint32_t* __restrict__ vals) {
+  const size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x;
+  if (i >= n) return;
+  vals[i] = (uint32_t)i;
+  if (w0) ka[i] = w0[i];
+}
+
+// the next word in the current order: keys[j] = word[ord[j]]
+__global__ void __launch_bounds__(THREADS) k_gather_word(size_t n, const uint32_t* __restrict__ word, const uint32_t* __restrict__ ord,
+                                                        uint32_t* __restrict__ keys) {
+  const size_t j = (size_t)blockIdx.x * THREADS + threadIdx.x;
+  if (j < n) keys[j] = word[ord[j]];
+}
+
+__global__ void __launch_bounds__(THREADS) k_run_heads(size_t n, const GofKeyWords key, const uint32_t* __restrict__ ord,
+                                                      uint32_t* __restrict__ head) {
+  const size_t j = (size_t)blockIdx.x * THREADS + threadIdx.x;
+  if (j >= n) return;
+  if (j == 0) { head[0] = 1; return; }
+  const uint32_t a = ord[j], b = ord[j - 1];
+  uint32_t diff = 0;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    if (k >= key.nw) break;
+    const uint32_t mask = key.bits[k] >= 32 ? 0xffffffffu : (1u << key.bits[k]) - 1u;
+    diff |= (key.w[k][a] ^ key.w[k][b]) & mask;
+  }
+  head[j] = diff ? 1u : 0u;
+}
+
 }  // namespace
 
 // Stable sort of the P (depth bits, gaussian id) pairs written by the preprocess kernel into key_a/val_a; 4 passes ->
@@ -504,24 +509,52 @@ int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, ui
   return GOF_OK;
 }
 
-// Stable LSD radix sort of n (u32 key, u32 value) pairs on the low `nbits` key bits.  Ping-pong buffers a/b (input in a);
-// *result_in_b tells where the result is.  hist: gof_sort_scratch_bytes(n).
-int gof_sort_pairs_u32(uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist, size_t n, int nbits, bool debug,
-                       cudaStream_t st, int* result_in_b) {
-  return sort_pairs<uint32_t>(ka, kb, va, vb, hist, n, nbits, debug, st, result_in_b);
-}
-
-// exclusive scan of n u32 (in != out allowed); total (if non-NULL) receives the sum; tmp: n/2048 + 4 u32
 int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n, bool debug, cudaStream_t st) {
   if (n == 0) {
     if (total) GOF_CUDA_OK(cudaMemsetAsync(total, 0, 4, st));
     return GOF_OK;
   }
-  const uint32_t nchunks = (uint32_t)((n + SCAN_CHUNK - 1) / SCAN_CHUNK);
+  const uint32_t nchunks = (uint32_t)((n + GOF_SCAN_CHUNK - 1) / GOF_SCAN_CHUNK);
   GOF_CUDA_OK(cudaMemsetAsync(tmp, 0, ((size_t)nchunks + 2) * 4, st));
   GOF_LAUNCH("scan", st, k_scan_excl<<<nchunks, THREADS, 0, st>>>(in, out, n, tmp, tmp + nchunks + 1, total, nchunks));
   GOF_LAUNCH_CHECK(debug, st);
   return GOF_OK;
+}
+
+int gof_sort_words_u32(const GofKeyWords& key, size_t n, const GofSortBufs& b, uint32_t* ord, bool debug, cudaStream_t st) {
+  if (key.nw < 1 || key.nw > 3 || (ord != b.va && ord != b.vb)) { gof_set_error("sort_words: 1-3 words, ord = va or vb"); return GOF_E_INVALID; }
+  int passes = 0;
+  for (int k = 0; k < key.nw; ++k) {
+    if (key.bits[k] < 1 || key.bits[k] > 32) { gof_set_error("sort_words: %d bits in word %d", key.bits[k], k); return GOF_E_INVALID; }
+    passes += (key.bits[k] + 7) / 8;
+  }
+  if (n == 0) return GOF_OK;
+  // every radix pass moves the values to the other buffer: start in the one from which the last pass ends in ord
+  uint32_t* vals = passes % 2 == 0 ? ord : (ord == b.va ? b.vb : b.va);
+  uint32_t* spare = vals == b.va ? b.vb : b.va;
+  const unsigned grid = (unsigned)((n + THREADS - 1) / THREADS);
+  GOF_LAUNCH("sort_init", st, k_sort_init<<<grid, THREADS, 0, st>>>(n, key.w[0] == b.ka ? nullptr : key.w[0], b.ka, vals));
+  GOF_LAUNCH_CHECK(debug, st);
+  for (int k = 0; k < key.nw; ++k) {
+    if (k > 0) {
+      GOF_LAUNCH("sort_gather", st, k_gather_word<<<grid, THREADS, 0, st>>>(n, key.w[k], vals, b.ka));
+      GOF_LAUNCH_CHECK(debug, st);
+    }
+    int in_b = 0;
+    const int rc = sort_pairs<uint32_t>(b.ka, b.kb, vals, spare, b.hist, n, key.bits[k], debug, st, &in_b);
+    if (rc != GOF_OK) return rc;
+    if (in_b) { uint32_t* t = vals; vals = spare; spare = t; }
+  }
+  return GOF_OK;
+}
+
+int gof_key_runs_u32(const GofKeyWords& key, const uint32_t* ord, size_t n, uint32_t* head, uint32_t* run, uint32_t* scan_tmp,
+                     uint32_t* num_runs, bool debug, cudaStream_t st) {
+  if (n > 0) {
+    GOF_LAUNCH("run_heads", st, k_run_heads<<<(unsigned)((n + THREADS - 1) / THREADS), THREADS, 0, st>>>(n, key, ord, head));
+    GOF_LAUNCH_CHECK(debug, st);
+  }
+  return gof_exclusive_scan_u32(head, run, scan_tmp, num_runs, n, debug, st);
 }
 
 int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin, const GofBinLayout& BL,

@@ -137,6 +137,37 @@ __device__ __forceinline__ float gof_rsqrt_newton(float x) {
   const float e = fmaf(-x * y, y, 1.0f);
   return fmaf(0.5f * y, e, y);
 }
+
+__device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v) {
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t n = __shfl_up_sync(0xffffffffu, v, d);
+    if ((threadIdx.x & 31) >= d) v += n;
+  }
+  return v;
+}
+
+// block-wide exclusive scan of one value per thread (GOF_BLOCK_SIZE threads); total in *total.  Ends with a barrier.
+__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total) {
+  constexpr int WARPS = GOF_BLOCK_SIZE / 32;
+  __shared__ uint32_t s_warp[WARPS];
+  __shared__ uint32_t s_total;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t incl = warp_incl_scan(v);
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t w = lane < WARPS ? s_warp[lane] : 0u;
+    const uint32_t wi = warp_incl_scan(w);
+    if (lane < WARPS) s_warp[lane] = wi - w;
+    if (lane == WARPS - 1) s_total = wi;
+  }
+  __syncthreads();
+  const uint32_t r = s_warp[warp] + incl - v;
+  *total = s_total;
+  __syncthreads();
+  return r;
+}
 #endif
 
 // ---- per-Gaussian records ---------------------------------------------------------------------
@@ -177,6 +208,13 @@ static constexpr inline int gof_sort_blocks(size_t n) { return (int)((n + GOF_SO
 static constexpr inline size_t gof_sort_scratch_bytes(size_t n) {
   return (size_t)GOF_SORT_HEAD_BYTES + (size_t)4 * ((size_t)gof_sort_blocks(n) + 8) * GOF_RADIX * 4;
 }
+
+#define GOF_SCAN_ITEMS 8                               // values per thread of the single-launch exclusive scan
+#define GOF_SCAN_CHUNK (GOF_BLOCK_SIZE * GOF_SCAN_ITEMS) // values per block of that scan
+
+// Scratch (`tmp`) of gof_exclusive_scan_u32 over n values: one look-back status word per chunk of GOF_SCAN_CHUNK values and a
+// ticket word, with slack.
+static constexpr inline size_t gof_scan_scratch_bytes(size_t n) { return (n / GOF_SCAN_CHUNK + 4) * 4 + 4096; }
 
 struct GofGeomLayout {      // "geomBuffer": everything sized by P
   size_t splat, splat_bwd, rect, tiles, clamped, depth;
@@ -311,8 +349,23 @@ int gof_launch_mark_visible(int P, const float* means3D, const float* vm, unsign
                             cudaStream_t st);
 
 // binning.cu
-int gof_sort_pairs_u32(uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist, size_t n, int nbits, bool debug,
-                       cudaStream_t st, int* result_in_b);
+// A sort key of 1-3 u32 words per item: w[0] is the least significant word, and only the low bits[k] (1..32) bits of w[k]
+// count.
+struct GofKeyWords {
+  const uint32_t* w[3];
+  int bits[3];
+  int nw;
+};
+// Buffers of gof_sort_words_u32 over n items, carved by the caller: ka, kb, va, vb n u32 each, hist gof_sort_scratch_bytes(n).
+// The sort never writes the key words, except w[0] when the caller made it ka; no other word may be one of these buffers.
+struct GofSortBufs { uint32_t *ka, *kb, *va, *vb, *hist; };
+// Stable sort of the items 0..n-1 by `key`: leaves ord[j] = the item at sorted position j in `ord`, which is va or vb.
+int gof_sort_words_u32(const GofKeyWords& key, size_t n, const GofSortBufs& b, uint32_t* ord, bool debug, cudaStream_t st);
+// Runs of equal keys along ord: head[j] = 1 where the key of ord[j] differs from that of ord[j - 1] (head[0] = 1), run[j] = the
+// exclusive scan of head, *num_runs (device) = the number of runs.  scan_tmp: gof_scan_scratch_bytes(n).
+int gof_key_runs_u32(const GofKeyWords& key, const uint32_t* ord, size_t n, uint32_t* head, uint32_t* run, uint32_t* scan_tmp,
+                     uint32_t* num_runs, bool debug, cudaStream_t st);
+// exclusive scan of n u32 (in != out allowed); total (if non-NULL, device) receives the sum; tmp: gof_scan_scratch_bytes(n)
 int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n, bool debug, cudaStream_t st);
 int gof_depth_sort(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st);
 int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin,

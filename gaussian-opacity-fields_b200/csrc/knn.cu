@@ -8,7 +8,7 @@
 //   bbox     order-free min / max of the finite points (ordered-integer atomics) into scratch
 //   keys     96-bit Morton code of each point over that box (32 bits per axis, quantised in double); non-finite points
 //            get the all-ones key, which no finite point can have, so they sort last
-//   sort     three rounds of the library's stable u32 radix sort (low word first)
+//   sort     the library's multi-word sort, the key as three u32 words
 //   gather   sorted coordinates into three planes, padded with NaN to whole leaves of 32
 //   boxes    one AABB per leaf of 32 consecutive points (finite points only), then an implicit 32-ary tree of unions
 //   search   one warp per leaf: seed from the leaf itself, then a depth-first walk from the root, nearest child first.  A
@@ -128,10 +128,10 @@ __device__ __forceinline__ uint32_t quantise(float v, float lo, float hi) {
   return (uint32_t)(t * 4294967294.0);
 }
 
-// 96-bit key, bit 3k + a = bit k of axis a: word 0 -> ka (sorted first), words 1, 2 -> hi1, hi2; va = identity
+// 96-bit key, bit 3k + a = bit k of axis a: word 0 -> ka (the sort's first key buffer), words 1, 2 -> hi1, hi2
 __global__ void __launch_bounds__(THREADS) k_knn_keys(int P, const float* __restrict__ pts, const uint32_t* __restrict__ bbox,
                                                       uint32_t* __restrict__ w0, uint32_t* __restrict__ hi1,
-                                                      uint32_t* __restrict__ hi2, uint32_t* __restrict__ va) {
+                                                      uint32_t* __restrict__ hi2) {
   const int i = blockIdx.x * THREADS + threadIdx.x;
   if (i >= P) return;
   const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
@@ -146,13 +146,7 @@ __global__ void __launch_bounds__(THREADS) k_knn_keys(int P, const float* __rest
     k1 = (uint32_t)(lo >> 32) | (uint32_t)(hi << 31);
     k2 = (uint32_t)(hi >> 1);
   }
-  w0[i] = k0; hi1[i] = k1; hi2[i] = k2; va[i] = (uint32_t)i;
-}
-
-__global__ void __launch_bounds__(THREADS) k_knn_gather_key(int P, const uint32_t* __restrict__ word, const uint32_t* __restrict__ order,
-                                                            uint32_t* __restrict__ out) {
-  const int s = blockIdx.x * THREADS + threadIdx.x;
-  if (s < P) out[s] = word[order[s]];
+  w0[i] = k0; hi1[i] = k1; hi2[i] = k2;
 }
 
 // sorted coordinates into planes; slots P .. padded-1 hold NaN (never accepted, never in a box)
@@ -348,19 +342,10 @@ extern "C" GOF_API int gof_knn_mean_dist(int P, const float* points, float* mean
   const int gb = gp < 1056 ? gp : 1056;
   GOF_LAUNCH("knn_bbox", st, k_knn_bbox<<<gb, THREADS, 0, st>>>(P, points, bbox));
   GOF_LAUNCH_CHECK(false, st);
-  GOF_LAUNCH("knn_keys", st, k_knn_keys<<<gp, THREADS, 0, st>>>(P, points, bbox, ka, hi1, hi2, va));
+  GOF_LAUNCH("knn_keys", st, k_knn_keys<<<gp, THREADS, 0, st>>>(P, points, bbox, ka, hi1, hi2));
   GOF_LAUNCH_CHECK(false, st);
-  // three stable rounds, low word first; the order after each round is kept in va
-  const uint32_t* words[3] = {nullptr, hi1, hi2};
-  for (int r = 0; r < 3; ++r) {
-    if (r > 0) {
-      GOF_LAUNCH("knn_gather_key", st, k_knn_gather_key<<<gp, THREADS, 0, st>>>(P, words[r], va, ka));
-      GOF_LAUNCH_CHECK(false, st);
-    }
-    int in_b = 0;
-    if ((rc = gof_sort_pairs_u32(ka, kb, va, vb, hist, (size_t)P, 32, false, st, &in_b)) != GOF_OK) return rc;
-    if (in_b) GOF_CUDA_OK(cudaMemcpyAsync(va, vb, (size_t)P * 4, cudaMemcpyDeviceToDevice, st));
-  }
+  const GofKeyWords key{{ka, hi1, hi2}, {32, 32, 32}, 3};
+  if ((rc = gof_sort_words_u32(key, (size_t)P, GofSortBufs{ka, kb, va, vb, hist}, va, false, st)) != GOF_OK) return rc;
   GOF_LAUNCH("knn_gather_points", st, k_knn_gather_points<<<blocks_for((size_t)padded, THREADS), THREADS, 0, st>>>(
                                           P, padded, points, va, xs, ys, zs));
   GOF_LAUNCH_CHECK(false, st);

@@ -4,8 +4,8 @@
 // int64 pairs plus an inverse map), keeps the edges with exactly one occupied endpoint and renumbers them, then
 // gathers faces through the triangle table, all 1-triangle tets before all 2-triangle tets (per chunk of 32 Mi tets).
 // Here only the CROSSING edges are ever materialised (3 or 4 per valid tet; the others are never referenced by the
-// triangle table), as (lo, hi) u32 pairs sorted with two rounds of the library's stable u32 radix sort; unique ids come
-// from head flags + a scan, so interp_v is the same lexicographically sorted list the reference produces, and faces
+// triangle table), as (lo, hi) u32 pairs sorted as a two-word key by the library's multi-word sort; unique ids number the
+// runs of equal pairs in that order, so interp_v is the same lexicographically sorted list the reference produces, and faces
 // are written at offsets given by scans of the 1-/2-triangle flags, reproducing the reference's face order exactly.
 #include "gof_common.cuh"
 
@@ -23,7 +23,7 @@ __device__ __constant__ int8_t c_eb[6] = {1, 2, 3, 2, 3, 3};
 
 struct TetLayout {   // scratch layout, a function of (T, capacity of edge instances = 4T)
   size_t header, code, cross, f1, f2, cross_off, f1_off, f2_off, scan_tmp;
-  size_t lo_a, lo_b, hi, val_a, val_b, hist, head, uid_sorted, inst_uid, bytes;
+  size_t lo, hi, val_a, val_b, hist, head, uid_sorted, inst_uid, bytes;
 };
 
 static TetLayout tet_layout(size_t T) {
@@ -34,8 +34,8 @@ static TetLayout tet_layout(size_t T) {
   L.code = take(T);
   L.cross = take(T * 4); L.f1 = take(T * 4); L.f2 = take(T * 4);
   L.cross_off = take(T * 4); L.f1_off = take(T * 4); L.f2_off = take(T * 4);
-  L.scan_tmp = take((I / 2048 + 4) * 4 + 4096);
-  L.lo_a = take(I * 4); L.lo_b = take(I * 4); L.hi = take(I * 4);
+  L.scan_tmp = take(gof_scan_scratch_bytes(I));
+  L.lo = take(I * 4); L.hi = take(I * 4);
   L.val_a = take(I * 4); L.val_b = take(I * 4);
   L.hist = take(gof_sort_scratch_bytes(I));
   L.head = take(I * 4); L.uid_sorted = take(I * 4); L.inst_uid = take(I * 4);
@@ -73,7 +73,7 @@ __global__ void __launch_bounds__(256) k_tet_classify(int64_t T, const float* __
 // one thread per tet: write its crossing edges (sorted endpoints) in base-edge order at cross_off[t]
 __global__ void __launch_bounds__(256) k_tet_edges(int64_t T, const int64_t* __restrict__ tets, const unsigned char* __restrict__ code,
                                                   const uint32_t* __restrict__ cross_off, uint32_t* __restrict__ lo,
-                                                  uint32_t* __restrict__ hi, uint32_t* __restrict__ val) {
+                                                  uint32_t* __restrict__ hi) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
   const uint32_t c = code[t];
@@ -89,26 +89,9 @@ __global__ void __launch_bounds__(256) k_tet_edges(int64_t T, const int64_t* __r
       const uint32_t x = v[a], y = v[b];
       lo[o] = x < y ? x : y;      // first column of the sorted pair
       hi[o] = x < y ? y : x;      // second column
-      val[o] = o;
       ++o;
     }
   }
-}
-
-__global__ void __launch_bounds__(256) k_gather_u32(size_t n, const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx,
-                                                   uint32_t* __restrict__ dst) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = src[idx[i]];
-}
-
-// sorted order `ord`: head[j] = 1 when (lo,hi)[ord[j]] differs from its predecessor
-__global__ void __launch_bounds__(256) k_heads(size_t n, const uint32_t* __restrict__ lo, const uint32_t* __restrict__ hi,
-                                              const uint32_t* __restrict__ ord, uint32_t* __restrict__ head) {
-  const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  if (j == 0) { head[0] = 1; return; }
-  const uint32_t a = ord[j], b = ord[j - 1];
-  head[j] = (lo[a] != lo[b] || hi[a] != hi[b]) ? 1u : 0u;
 }
 
 // uid_sorted = exclusive scan of head; unique id of sorted position j is uid_sorted[j] + head[j] - 1
@@ -216,34 +199,18 @@ int gof_marching_tets_count(int num_verts, const float* sdf, int64_t num_tets, c
   *num_faces_out = (int64_t)h.n1 + 2 * (int64_t)h.n2;
   const size_t I = h.n_inst;
   if (I == 0) return GOF_OK;
-  uint32_t *lo_a = (uint32_t*)(S + L.lo_a), *lo_b = (uint32_t*)(S + L.lo_b), *hi = (uint32_t*)(S + L.hi);
+  uint32_t *lo = (uint32_t*)(S + L.lo), *hi = (uint32_t*)(S + L.hi);
   uint32_t *va = (uint32_t*)(S + L.val_a), *vb = (uint32_t*)(S + L.val_b), *hist = (uint32_t*)(S + L.hist);
   uint32_t *head = (uint32_t*)(S + L.head), *uid_sorted = (uint32_t*)(S + L.uid_sorted), *inst_uid = (uint32_t*)(S + L.inst_uid);
-  // lo_b doubles as the unsorted copy of the first column: edges are written to (lo_b, hi), sorted through (lo_a, ...)
-  GOF_LAUNCH("tet_edges", st, k_tet_edges<<<grid, 256, 0, st>>>(num_tets, tets, code, cross_off, lo_b, hi, va));
+  GOF_LAUNCH("tet_edges", st, k_tet_edges<<<grid, 256, 0, st>>>(num_tets, tets, code, cross_off, lo, hi));
   GOF_LAUNCH_CHECK(false, st);
+  // lexicographic (first, second) order: the second column is the low word.  head / uid_sorted are written only after the
+  // sort, so they are its key buffers; the order lands in val_a.
   const int vbits = gof_bits_for((uint32_t)num_verts);
-  const unsigned gi = (unsigned)((I + 255) / 256);
-  // round 1: stable sort of instance ids by the SECOND column
-  uint32_t* k1a = head;          // reuse head / uid_sorted as key ping-pong for the two rounds
-  uint32_t* k1b = uid_sorted;
-  GOF_CUDA_OK(cudaMemcpyAsync(k1a, hi, I * 4, cudaMemcpyDeviceToDevice, st));
-  int in_b = 0;
-  if ((rc = gof_sort_pairs_u32(k1a, k1b, va, vb, hist, I, vbits, false, st, &in_b)) != GOF_OK) return rc;
-  uint32_t* ord1 = in_b ? vb : va;
-  uint32_t* ord1_other = in_b ? va : vb;
-  // round 2: stable sort of that order by the FIRST column -> lexicographic (first, second) order
-  GOF_LAUNCH("tet_gather", st, k_gather_u32<<<gi, 256, 0, st>>>(I, lo_b, ord1, k1a));
-  GOF_LAUNCH_CHECK(false, st);
-  if (ord1 != va) GOF_CUDA_OK(cudaMemcpyAsync(va, ord1, I * 4, cudaMemcpyDeviceToDevice, st));
-  (void)ord1_other;
-  if ((rc = gof_sort_pairs_u32(k1a, k1b, va, vb, hist, I, vbits, false, st, &in_b)) != GOF_OK) return rc;
-  uint32_t* ord = in_b ? vb : va;
-  if (ord != lo_a) GOF_CUDA_OK(cudaMemcpyAsync(lo_a, ord, I * 4, cudaMemcpyDeviceToDevice, st));   // final order lives in lo_a
-  GOF_LAUNCH("tet_heads", st, k_heads<<<gi, 256, 0, st>>>(I, lo_b, hi, lo_a, head));
-  GOF_LAUNCH_CHECK(false, st);
-  if ((rc = gof_exclusive_scan_u32(head, uid_sorted, tmp, &hd->n_edges, I, false, st)) != GOF_OK) return rc;
-  GOF_LAUNCH("tet_uid", st, k_scatter_uid<<<gi, 256, 0, st>>>(I, lo_a, head, uid_sorted, inst_uid));
+  const GofKeyWords key{{hi, lo, nullptr}, {vbits, vbits, 0}, 2};
+  if ((rc = gof_sort_words_u32(key, I, GofSortBufs{head, uid_sorted, va, vb, hist}, va, false, st)) != GOF_OK) return rc;
+  if ((rc = gof_key_runs_u32(key, va, I, head, uid_sorted, tmp, &hd->n_edges, false, st)) != GOF_OK) return rc;
+  GOF_LAUNCH("tet_uid", st, k_scatter_uid<<<(unsigned)((I + 255) / 256), 256, 0, st>>>(I, va, head, uid_sorted, inst_uid));
   GOF_LAUNCH_CHECK(false, st);
   { const int rb = gof_read_back(&h, hd, sizeof(Header), st); if (rb != GOF_OK) return rb; }
   *num_edges_out = (int64_t)h.n_edges;
@@ -280,8 +247,8 @@ int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, co
   else a.chunk = (chunk_tets > 0 && num_tets > chunk_tets) ? (num_tets + (num_tets / chunk_tets + 1) - 1) / (num_tets / chunk_tets + 1) : num_tets;
   a.tets = tets; a.code = (unsigned char*)(S + L.code);
   a.cross_off = (uint32_t*)(S + L.cross_off); a.f1_off = (uint32_t*)(S + L.f1_off); a.f2_off = (uint32_t*)(S + L.f2_off);
-  a.inst_uid = (uint32_t*)(S + L.inst_uid); a.lo = (uint32_t*)(S + L.lo_b); a.hi = (uint32_t*)(S + L.hi);
-  a.ord = (uint32_t*)(S + L.lo_a); a.head = (uint32_t*)(S + L.head); a.uid_sorted = (uint32_t*)(S + L.uid_sorted);
+  a.inst_uid = (uint32_t*)(S + L.inst_uid); a.lo = (uint32_t*)(S + L.lo); a.hi = (uint32_t*)(S + L.hi);
+  a.ord = (uint32_t*)(S + L.val_a); a.head = (uint32_t*)(S + L.head); a.uid_sorted = (uint32_t*)(S + L.uid_sorted);
   a.n_inst = h.n_inst; a.interp_v = interp_v; a.faces = faces; a.vertices = vertices; a.sdf = sdf; a.scales = scales;
   a.edge_pos = edge_pos; a.edge_sdf = edge_sdf; a.edge_scales = edge_scales;
   if (h.n_inst) {

@@ -6,8 +6,8 @@
 // float32 oracle reproduces it bit for bit.  The library keeps no state: the block table (sorted keys + pool slots) and
 // the voxel pool belong to the caller.
 //
-//   touch     one thread per sampled pixel: count its blocks -> scan -> emit 63-bit keys as (lo, hi) u32 words -> two
-//             rounds of the library's stable u32 radix sort (lo, then hi) -> head flags + scan -> unique keys
+//   touch     one thread per sampled pixel: count its blocks -> scan -> emit 63-bit keys as (lo, hi) u32 words -> the
+//             library's multi-word sort -> one unique key per run of equal keys
 //   activate  binary search of the view's keys in the table, scan of the "new" flags, merge by binary search
 //   integrate one CTA per block of the view's list; voxel data is structure-of-arrays per block, read coalesced, and
 //             only updated voxels are written; the depth and colour images are gathers that stay in L2
@@ -43,30 +43,6 @@ __device__ __forceinline__ int64_t lower_bound(const int64_t* __restrict__ keys,
     if (keys[mid] < k) lo = mid + 1; else hi = mid;
   }
   return lo;
-}
-
-// exclusive scan over the CTA (THREADS threads); *total receives the sum.  Ends with __syncthreads().
-__device__ uint32_t block_excl_scan(uint32_t v, uint32_t* total) {
-  __shared__ uint32_t s_warp[THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) s_warp[warp] = x;
-  __syncthreads();
-  uint32_t before = 0, sum = 0;
-#pragma unroll
-  for (int w = 0; w < THREADS / 32; ++w) {
-    const uint32_t t = s_warp[w];
-    before += w < warp ? t : 0u;
-    sum += t;
-  }
-  __syncthreads();
-  *total = sum;
-  return before + x - v;
 }
 
 struct Cam {
@@ -111,7 +87,7 @@ static int check_params(const gof_tsdf_params_t* p, const char* who) {
 // ---- touch -------------------------------------------------------------------------------------------------------
 
 struct TouchLayout {
-  size_t header, cnt, off, scan_tmp, lo_a, lo_b, hi_a, hi_b, val_a, val_b, hist, head, uid, bytes;
+  size_t header, cnt, off, scan_tmp, lo, hi, val_a, val_b, hist, head, uid, bytes;
   size_t npix, cap;
 };
 struct TouchHeader { uint32_t n_inst, err, n_unique, pad; };
@@ -125,8 +101,8 @@ static TouchLayout touch_layout(int W, int H, const Par& p) {
   const size_t I = L.cap > L.npix ? L.cap : L.npix;
   L.header = take(256);
   L.cnt = take(L.npix * 4); L.off = take(L.npix * 4);
-  L.scan_tmp = take((I / 2048 + 4) * 4 + 4096);
-  L.lo_a = take(L.cap * 4); L.lo_b = take(L.cap * 4); L.hi_a = take(L.cap * 4); L.hi_b = take(L.cap * 4);
+  L.scan_tmp = take(gof_scan_scratch_bytes(I));
+  L.lo = take(L.cap * 4); L.hi = take(L.cap * 4);
   L.val_a = take(L.cap * 4); L.val_b = take(L.cap * 4);
   L.hist = take(gof_sort_scratch_bytes(L.cap));
   L.head = take(L.cap * 4); L.uid = take(L.cap * 4);
@@ -178,7 +154,7 @@ __global__ void __launch_bounds__(THREADS) k_touch_count(int npix, const float* 
 
 __global__ void __launch_bounds__(THREADS) k_touch_emit(int npix, const float* __restrict__ depth, const Cam c, const Par p,
                                                        const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ off,
-                                                       uint32_t* __restrict__ lo_w, uint32_t* __restrict__ hi_w, uint32_t* __restrict__ val) {
+                                                       uint32_t* __restrict__ lo_w, uint32_t* __restrict__ hi_w) {
   const int pix = blockIdx.x * THREADS + threadIdx.x;
   if (pix >= npix || !cnt[pix]) return;
   float lo[3], hi[3];
@@ -188,27 +164,12 @@ __global__ void __launch_bounds__(THREADS) k_touch_emit(int npix, const float* _
     for (int y = (int)lo[1]; y <= (int)hi[1]; ++y)
       for (int x = (int)lo[0]; x <= (int)hi[0]; ++x) {
         const uint64_t k = (uint64_t)pack_key(x, y, z);
-        lo_w[o] = (uint32_t)k; hi_w[o] = (uint32_t)(k >> 32); val[o] = o;
+        lo_w[o] = (uint32_t)k; hi_w[o] = (uint32_t)(k >> 32);
         ++o;
       }
 }
 
-__global__ void __launch_bounds__(THREADS) k_gather_u32(size_t n, const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx,
-                                                       uint32_t* __restrict__ dst) {
-  const size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x;
-  if (i < n) dst[i] = src[idx[i]];
-}
-
-// ord: the instances in key order; head[j] = 1 where the key of sorted position j differs from its predecessor's
-__global__ void __launch_bounds__(THREADS) k_key_heads(size_t n, const uint32_t* __restrict__ lo_w, const uint32_t* __restrict__ hi_w,
-                                                      const uint32_t* __restrict__ ord, uint32_t* __restrict__ head) {
-  const size_t j = (size_t)blockIdx.x * THREADS + threadIdx.x;
-  if (j >= n) return;
-  if (j == 0) { head[0] = 1; return; }
-  const uint32_t a = ord[j], b = ord[j - 1];
-  head[j] = (lo_w[a] != lo_w[b] || hi_w[a] != hi_w[b]) ? 1u : 0u;
-}
-
+// ord: the instances in key order; head / uid: the runs of equal keys along it (gof_key_runs_u32)
 __global__ void __launch_bounds__(THREADS) k_key_emit(size_t n, const uint32_t* __restrict__ lo_w, const uint32_t* __restrict__ hi_w,
                                                      const uint32_t* __restrict__ ord, const uint32_t* __restrict__ head,
                                                      const uint32_t* __restrict__ uid, int64_t* __restrict__ keys) {
@@ -225,7 +186,7 @@ static ActLayout act_layout(size_t nv) {
   ActLayout L; size_t o = 0;
   auto take = [&](size_t b) { size_t r = o; o = gof_align_up(o + b, 256); return r; };
   L.header = take(256); L.pos = take(nv * 8); L.flag = take(nv * 4); L.off = take(nv * 4);
-  L.scan_tmp = take((nv / 2048 + 4) * 4 + 4096);
+  L.scan_tmp = take(gof_scan_scratch_bytes(nv));
   L.bytes = o;
   return L;
 }
@@ -337,7 +298,7 @@ static MeshLayout mesh_layout(size_t n, int B) {
   L.marks = take(n * n3);
   L.vid = take(n * n3 * 4);
   L.bv = take(n * 4); L.bf = take(n * 4); L.bv_off = take(n * 4); L.bf_off = take(n * 4);
-  L.scan_tmp = take((n / 2048 + 4) * 4 + 4096);
+  L.scan_tmp = take(gof_scan_scratch_bytes(n));
   L.bytes = o;
   return L;
 }
@@ -581,27 +542,16 @@ int gof_tsdf_touch_count(const gof_tsdf_params_t* params, const gof_tsdf_camera_
   if (h.err) { gof_set_error("tsdf_touch_count: a pixel touches more blocks per axis than 2 tau / (B s) + 2"); return GOF_E_INVALID; }
   const size_t I = h.n_inst;
   if (I == 0) return GOF_OK;
-  uint32_t *lo_a = (uint32_t*)(S + L.lo_a), *lo_b = (uint32_t*)(S + L.lo_b), *hi_a = (uint32_t*)(S + L.hi_a), *hi_b = (uint32_t*)(S + L.hi_b);
+  uint32_t *lo = (uint32_t*)(S + L.lo), *hi = (uint32_t*)(S + L.hi);
   uint32_t *va = (uint32_t*)(S + L.val_a), *vb = (uint32_t*)(S + L.val_b), *hist = (uint32_t*)(S + L.hist);
   uint32_t *head = (uint32_t*)(S + L.head), *uid = (uint32_t*)(S + L.uid);
-  // the unsorted words stay in (lo_b, hi_b); the sorts run on copies in the *_a / head / uid buffers
-  GOF_LAUNCH("tsdf_touch_emit", st, k_touch_emit<<<gp, THREADS, 0, st>>>(npix, depth, c, p, cnt, off, lo_b, hi_b, va));
+  GOF_LAUNCH("tsdf_touch_emit", st, k_touch_emit<<<gp, THREADS, 0, st>>>(npix, depth, c, p, cnt, off, lo, hi));
   GOF_LAUNCH_CHECK(false, st);
-  const unsigned gi = (unsigned)((I + THREADS - 1) / THREADS);
-  // round 1: stable sort of the instance ids by the low word
-  GOF_CUDA_OK(cudaMemcpyAsync(lo_a, lo_b, I * 4, cudaMemcpyDeviceToDevice, st));
-  int in_b = 0;
-  if ((rc = gof_sort_pairs_u32(lo_a, head, va, vb, hist, I, 32, false, st, &in_b)) != GOF_OK) return rc;
-  if (in_b) GOF_CUDA_OK(cudaMemcpyAsync(va, vb, I * 4, cudaMemcpyDeviceToDevice, st));
-  // round 2: stable sort of that order by the high word (keys < 2^63) -> ascending 63-bit keys
-  GOF_LAUNCH("tsdf_touch_gather", st, k_gather_u32<<<gi, THREADS, 0, st>>>(I, hi_b, va, hi_a));
-  GOF_LAUNCH_CHECK(false, st);
-  if ((rc = gof_sort_pairs_u32(hi_a, head, va, vb, hist, I, 31, false, st, &in_b)) != GOF_OK) return rc;
-  uint32_t* ord = in_b ? vb : va;
-  if (ord != lo_a) GOF_CUDA_OK(cudaMemcpyAsync(lo_a, ord, I * 4, cudaMemcpyDeviceToDevice, st));   // final order lives in lo_a
-  GOF_LAUNCH("tsdf_touch_heads", st, k_key_heads<<<gi, THREADS, 0, st>>>(I, lo_b, hi_b, lo_a, head));
-  GOF_LAUNCH_CHECK(false, st);
-  if ((rc = gof_exclusive_scan_u32(head, uid, tmp, &hd->n_unique, I, false, st)) != GOF_OK) return rc;
+  // ascending 63-bit keys (the high word has 31 bits); head / uid are written only after the sort, so they are its key
+  // buffers; the order lands in val_a
+  const GofKeyWords key{{lo, hi, nullptr}, {32, 31, 0}, 2};
+  if ((rc = gof_sort_words_u32(key, I, GofSortBufs{head, uid, va, vb, hist}, va, false, st)) != GOF_OK) return rc;
+  if ((rc = gof_key_runs_u32(key, va, I, head, uid, tmp, &hd->n_unique, false, st)) != GOF_OK) return rc;
   if ((rc = gof_read_back(&h, hd, sizeof(h), st)) != GOF_OK) return rc;
   *num_blocks_out = (int64_t)h.n_unique;
   return GOF_OK;
@@ -622,7 +572,7 @@ int gof_tsdf_touch_emit(const gof_tsdf_params_t* params, const gof_tsdf_camera_t
   if ((int64_t)h.n_unique != num_blocks) { gof_set_error("tsdf_touch_emit: size does not match the count phase"); return GOF_E_INVALID; }
   const size_t I = h.n_inst;
   GOF_LAUNCH("tsdf_touch_keys", st, k_key_emit<<<(unsigned)((I + THREADS - 1) / THREADS), THREADS, 0, st>>>(
-      I, (const uint32_t*)(S + L.lo_b), (const uint32_t*)(S + L.hi_b), (const uint32_t*)(S + L.lo_a), (const uint32_t*)(S + L.head),
+      I, (const uint32_t*)(S + L.lo), (const uint32_t*)(S + L.hi), (const uint32_t*)(S + L.val_a), (const uint32_t*)(S + L.head),
       (const uint32_t*)(S + L.uid), keys_out));
   GOF_LAUNCH_CHECK(false, st);
   return GOF_OK;
