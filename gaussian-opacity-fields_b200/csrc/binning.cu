@@ -29,36 +29,56 @@ constexpr int WARPS = THREADS / 32;
 constexpr uint32_t LB_AGG = 1u << 30;                // status word = flag (2 bits) | count (30 bits): written and read as ONE word
 constexpr uint32_t LB_INC = 2u << 30;
 constexpr uint32_t LB_VAL = (1u << 30) - 1u;
+// The radix passes and the scan + emit kernel count at most n items per status word: their sizes stay below 2^30.
+constexpr size_t LB_MAX_ITEMS = (size_t)1 << 30;
 
 __device__ __forceinline__ uint32_t ld_volatile(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
 __device__ __forceinline__ void st_volatile(uint32_t* p, uint32_t v) { *reinterpret_cast<volatile uint32_t*>(p) = v; }
+__device__ __forceinline__ uint64_t ld_volatile(const uint64_t* p) { return *reinterpret_cast<const volatile uint64_t*>(p); }
+__device__ __forceinline__ void st_volatile(uint64_t* p, uint64_t v) { *reinterpret_cast<volatile uint64_t*>(p) = v; }
+
+// Look-back status words.  u32: flag in bits 30-31, a 30-bit count (the radix passes and the scan + emit kernel, whose
+// counts stay below 2^30).  u64: flag in the high half, the full u32 running total in the low half (the general scan, whose
+// totals may reach 2^32 - 1); 8-byte aligned, so one load or store moves flag and value together.
+template <typename W> struct LbWord;
+template <> struct LbWord<uint32_t> {
+  static constexpr int SHIFT = 30;
+  static constexpr uint32_t VAL = LB_VAL;
+};
+template <> struct LbWord<uint64_t> {
+  static constexpr int SHIFT = 32;
+  static constexpr uint64_t VAL = 0xffffffffull;
+};
 
 // Decoupled look-back: a chunk publishes its aggregate in a status word (flag | count, written and read as ONE word), walks
 // back over its predecessors' words until one carries an inclusive prefix, then publishes its own inclusive prefix.
 // Warp-wide variant for the scans (one running quantity per chunk, thousands of chunks in flight): the 32 lanes of a warp
 // fetch 32 consecutive predecessors in one coalesced request, so a walk over k predecessors costs k/32 dependent round
 // trips.  Called by ALL lanes of one warp; every lane returns the exclusive prefix.
-__device__ __forceinline__ uint32_t lookback_warp(uint32_t* status, uint32_t chunk, uint32_t aggregate) {
+template <typename W>
+__device__ __forceinline__ uint32_t lookback_warp(W* status, uint32_t chunk, uint32_t aggregate) {
+  constexpr int S = LbWord<W>::SHIFT;
+  constexpr W AGG = (W)1 << S, INC = (W)2 << S;
   const int lane = threadIdx.x & 31;
-  if (lane == 0) st_volatile(status + chunk, (chunk == 0 ? LB_INC : LB_AGG) | aggregate);
+  if (lane == 0) st_volatile(status + chunk, (chunk == 0 ? INC : AGG) | (W)aggregate);
   uint32_t excl = 0u;
   int64_t pos = (int64_t)chunk;   // entries [0, pos) still to be examined; lane 0 takes the nearest
   while (pos > 0) {
     const int64_t idx = pos - 1 - lane;
-    uint32_t w;
+    W w;
     do {
-      w = idx >= 0 ? ld_volatile(status + idx) : LB_INC;   // in front of chunk 0: an inclusive prefix of zero
-    } while (__any_sync(0xffffffffu, (w >> 30) == 0u));
-    const uint32_t inc = __ballot_sync(0xffffffffu, (w >> 30) == 2u);
+      w = idx >= 0 ? ld_volatile(status + idx) : INC;   // in front of chunk 0: an inclusive prefix of zero
+    } while (__any_sync(0xffffffffu, (w >> S) == 0u));
+    const uint32_t inc = __ballot_sync(0xffffffffu, (w >> S) == 2u);
     const int first = inc ? __ffs(inc) - 1 : 31;       // nearest predecessor carrying an inclusive prefix
-    uint32_t v = lane <= first ? (w & LB_VAL) : 0u;
+    uint32_t v = lane <= first ? (uint32_t)(w & LbWord<W>::VAL) : 0u;
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
     excl += v;
     if (inc) break;
     pos -= 32;
   }
-  if (lane == 0 && chunk != 0) st_volatile(status + chunk, LB_INC | (excl + aggregate));
+  if (lane == 0 && chunk != 0) st_volatile(status + chunk, INC | (W)(excl + aggregate));
   return excl;
 }
 
@@ -279,6 +299,7 @@ int sort_pairs(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, uint32_t* scratch
                int* result_in_b) {
   *result_in_b = 0;
   if (n == 0 || nbits <= 0) return GOF_OK;
+  if (n >= LB_MAX_ITEMS) { gof_set_error("radix sort of %zu items: fewer than 2^30 supported", n); return GOF_E_INVALID; }
   Digits dg;
   split_digits(nbits, &dg);
   const SortScratch sc = carve_sort_scratch(scratch, n);
@@ -293,9 +314,10 @@ int sort_pairs(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, uint32_t* scratch
 }
 
 // ------------------------------------------------------------------------------------------------
-// single-launch exclusive scan of u32 (decoupled look-back); chunk = GOF_SCAN_CHUNK values per CTA
+// single-launch exclusive scan of u32 (decoupled look-back over 64-bit status words: running totals up to 2^32 - 1 are exact,
+// larger ones wrap like any u32 sum); chunk = GOF_SCAN_CHUNK values per CTA
 __global__ void __launch_bounds__(THREADS) k_scan_excl(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, size_t n,
-                                                      uint32_t* __restrict__ status, uint32_t* __restrict__ ticket,
+                                                      uint64_t* __restrict__ status, uint32_t* __restrict__ ticket,
                                                       uint32_t* __restrict__ total_out, uint32_t nchunks) {
   __shared__ uint32_t s_chunk, s_prefix;
   if (threadIdx.x == 0) s_chunk = atomicAdd(ticket, 1u);
@@ -412,6 +434,7 @@ __global__ void __launch_bounds__(256) k_tile_ranges(size_t L, const KeyT* __res
 template <typename KeyT>
 int bin_tiles_t(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin, const GofBinLayout& BL, char* img,
                 const GofImageLayout& IL, bool debug, cudaStream_t st) {
+  if (R >= LB_MAX_ITEMS) { gof_set_error("binning: %zu (tile, Gaussian) instances, fewer than 2^30 supported", R); return GOF_E_INVALID; }
   uint2* ranges = reinterpret_cast<uint2*>(img + IL.ranges);
   GOF_CUDA_OK(cudaMemsetAsync(ranges, 0, (size_t)v.tiles * sizeof(uint2), st));
   if (R == 0) return GOF_OK;
@@ -514,9 +537,12 @@ int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uin
     if (total) GOF_CUDA_OK(cudaMemsetAsync(total, 0, 4, st));
     return GOF_OK;
   }
+  if (reinterpret_cast<uintptr_t>(tmp) % 8u) { gof_set_error("exclusive_scan: tmp must be 8-byte aligned"); return GOF_E_INVALID; }
+  // tmp: nchunks u64 status words, then the chunk ticket
   const uint32_t nchunks = (uint32_t)((n + GOF_SCAN_CHUNK - 1) / GOF_SCAN_CHUNK);
-  GOF_CUDA_OK(cudaMemsetAsync(tmp, 0, ((size_t)nchunks + 2) * 4, st));
-  GOF_LAUNCH("scan", st, k_scan_excl<<<nchunks, THREADS, 0, st>>>(in, out, n, tmp, tmp + nchunks + 1, total, nchunks));
+  GOF_CUDA_OK(cudaMemsetAsync(tmp, 0, ((size_t)nchunks * 2 + 1) * 4, st));
+  GOF_LAUNCH("scan", st, k_scan_excl<<<nchunks, THREADS, 0, st>>>(in, out, n, reinterpret_cast<uint64_t*>(tmp), tmp + (size_t)nchunks * 2,
+                                                                  total, nchunks));
   GOF_LAUNCH_CHECK(debug, st);
   return GOF_OK;
 }
@@ -529,6 +555,7 @@ int gof_sort_words_u32(const GofKeyWords& key, size_t n, const GofSortBufs& b, u
     passes += (key.bits[k] + 7) / 8;
   }
   if (n == 0) return GOF_OK;
+  if (n >= LB_MAX_ITEMS) { gof_set_error("sort_words: %zu items, the radix sort takes fewer than 2^30", n); return GOF_E_INVALID; }
   // every radix pass moves the values to the other buffer: start in the one from which the last pass ends in ord
   uint32_t* vals = passes % 2 == 0 ? ord : (ord == b.va ? b.vb : b.va);
   uint32_t* spare = vals == b.va ? b.vb : b.va;
@@ -550,6 +577,7 @@ int gof_sort_words_u32(const GofKeyWords& key, size_t n, const GofSortBufs& b, u
 
 int gof_key_runs_u32(const GofKeyWords& key, const uint32_t* ord, size_t n, uint32_t* head, uint32_t* run, uint32_t* scan_tmp,
                      uint32_t* num_runs, bool debug, cudaStream_t st) {
+  if (key.nw < 1 || key.nw > 3) { gof_set_error("key_runs: 1-3 words"); return GOF_E_INVALID; }
   if (n > 0) {
     GOF_LAUNCH("run_heads", st, k_run_heads<<<(unsigned)((n + THREADS - 1) / THREADS), THREADS, 0, st>>>(n, key, ord, head));
     GOF_LAUNCH_CHECK(debug, st);
@@ -561,4 +589,39 @@ int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLa
                   char* img, const GofImageLayout& IL, bool debug, cudaStream_t st) {
   if (BL.key_bytes == 2) return bin_tiles_t<uint16_t>(P, R, v, geom, GL, bin, BL, img, IL, debug, st);
   return bin_tiles_t<uint32_t>(P, R, v, geom, GL, bin, BL, img, IL, debug, st);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Test entry points (tests/test_gpu_sort_primitives.py, tools/sanitize_run.py): the sort, run and scan primitives above over
+// plain pointers, so that they can be checked against an exact reference on their own.  Not part of the public header.
+// All pointers are device pointers except `words` and `bits` (host arrays of nw entries).
+namespace {
+GofKeyWords probe_key(int nw, const uint32_t* const* words, const int* bits) {
+  GofKeyWords key{};
+  key.nw = nw;
+  for (int k = 0; k < nw && k < 3; ++k) { key.w[k] = words[k]; key.bits[k] = bits[k]; }
+  return key;
+}
+}  // namespace
+
+extern "C" GOF_API int gof_probe_sort_words_u32(int nw, const uint32_t* const* words, const int* bits, size_t n, uint32_t* ka,
+                                                uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist, int ord_is_vb, void* stream) {
+  return gof_sort_words_u32(probe_key(nw, words, bits), n, GofSortBufs{ka, kb, va, vb, hist}, ord_is_vb ? vb : va, false,
+                            (cudaStream_t)stream);
+}
+
+extern "C" GOF_API int gof_probe_key_runs_u32(int nw, const uint32_t* const* words, const int* bits, const uint32_t* ord, size_t n,
+                                              uint32_t* head, uint32_t* run, uint32_t* scan_tmp, uint32_t* num_runs, void* stream) {
+  return gof_key_runs_u32(probe_key(nw, words, bits), ord, n, head, run, scan_tmp, num_runs, false, (cudaStream_t)stream);
+}
+
+extern "C" GOF_API int gof_probe_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n,
+                                                    void* stream) {
+  return gof_exclusive_scan_u32(in, out, tmp, total, n, false, (cudaStream_t)stream);
+}
+
+// which = 0: the `hist` scratch of a sort of n items (gof_sort_scratch_bytes); 1: the `tmp` of a scan of n values
+// (gof_scan_scratch_bytes)
+extern "C" GOF_API size_t gof_probe_scratch_bytes(int which, size_t n) {
+  return which == 0 ? gof_sort_scratch_bytes(n) : which == 1 ? gof_scan_scratch_bytes(n) : 0;
 }

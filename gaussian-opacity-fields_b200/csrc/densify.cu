@@ -148,7 +148,12 @@ __global__ void __launch_bounds__(256) k_gather_rows(const float* __restrict__ s
 }  // namespace
 
 // Step 1: the four keep-flags of every Gaussian and their exclusive scans.  flags / offsets: [4][P] u32 (device), totals: [4] u32
-// (device; read them back to size the outputs), scan_tmp: gof_scan_scratch_bytes(P).
+// (device; read them back to size the outputs), scan_tmp: gof_densify_scratch_bytes(P).
+extern "C" GOF_API size_t gof_densify_scratch_bytes(int P) {
+  if (P <= 0) return 0;
+  return gof_scan_scratch_bytes((size_t)P);
+}
+
 extern "C" GOF_API int gof_densify_plan(int P, const float* accum, const float* accum_abs, const float* denom, const float* scaling_raw,
                                         const float* opacity_raw, float max_grad, float abs_threshold, float dense_extent,
                                         float min_opacity, float prune_scale, uint32_t* flags, uint32_t* offsets, uint32_t* totals,

@@ -212,9 +212,9 @@ static constexpr inline size_t gof_sort_scratch_bytes(size_t n) {
 #define GOF_SCAN_ITEMS 8                               // values per thread of the single-launch exclusive scan
 #define GOF_SCAN_CHUNK (GOF_BLOCK_SIZE * GOF_SCAN_ITEMS) // values per block of that scan
 
-// Scratch (`tmp`) of gof_exclusive_scan_u32 over n values: one look-back status word per chunk of GOF_SCAN_CHUNK values and a
-// ticket word, with slack.
-static constexpr inline size_t gof_scan_scratch_bytes(size_t n) { return (n / GOF_SCAN_CHUNK + 4) * 4 + 4096; }
+// Scratch (`tmp`, 8-byte aligned) of gof_exclusive_scan_u32 over n values: one 8-byte look-back status word per chunk of
+// GOF_SCAN_CHUNK values and a ticket word, with slack.
+static constexpr inline size_t gof_scan_scratch_bytes(size_t n) { return (n / GOF_SCAN_CHUNK + 4) * 8 + 4096; }
 
 struct GofGeomLayout {      // "geomBuffer": everything sized by P
   size_t splat, splat_bwd, rect, tiles, clamped, depth;
@@ -360,13 +360,17 @@ struct GofKeyWords {
 // The sort never writes the key words, except w[0] when the caller made it ka; no other word may be one of these buffers.
 struct GofSortBufs { uint32_t *ka, *kb, *va, *vb, *hist; };
 // Stable sort of the items 0..n-1 by `key`: leaves ord[j] = the item at sorted position j in `ord`, which is va or vb.
+// n < 2^30 (the radix passes count items in 30-bit fields); a larger n fails with GOF_E_INVALID before any work is enqueued.
 int gof_sort_words_u32(const GofKeyWords& key, size_t n, const GofSortBufs& b, uint32_t* ord, bool debug, cudaStream_t st);
 // Runs of equal keys along ord: head[j] = 1 where the key of ord[j] differs from that of ord[j - 1] (head[0] = 1), run[j] = the
 // exclusive scan of head, *num_runs (device) = the number of runs.  scan_tmp: gof_scan_scratch_bytes(n).
 int gof_key_runs_u32(const GofKeyWords& key, const uint32_t* ord, size_t n, uint32_t* head, uint32_t* run, uint32_t* scan_tmp,
                      uint32_t* num_runs, bool debug, cudaStream_t st);
-// exclusive scan of n u32 (in != out allowed); total (if non-NULL, device) receives the sum; tmp: gof_scan_scratch_bytes(n)
+// exclusive scan of n u32 (in != out allowed); total (if non-NULL, device) receives the sum; tmp: gof_scan_scratch_bytes(n),
+// 8-byte aligned.  Offsets and total are exact while the sum stays below 2^32 and wrap mod 2^32 beyond.
 int gof_exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t* tmp, uint32_t* total, size_t n, bool debug, cudaStream_t st);
+// The depth sort, the tile binning (R = the number of (tile, Gaussian) instances) and the point sort share the radix passes'
+// limit: P, R and n below 2^30, or GOF_E_INVALID.
 int gof_depth_sort(int P, char* geom, const GofGeomLayout& L, bool debug, cudaStream_t st);
 int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin,
                   const GofBinLayout& BL, char* img, const GofImageLayout& IL, bool debug, cudaStream_t st);

@@ -22,6 +22,8 @@ from diff_gaussian_rasterization import _C
 
 _lib = _C._lib
 _v = ctypes.c_void_p
+_lib.gof_densify_scratch_bytes.restype = ctypes.c_size_t
+_lib.gof_densify_scratch_bytes.argtypes = [ctypes.c_int]
 _lib.gof_densify_plan.restype = ctypes.c_int
 _lib.gof_densify_plan.argtypes = [ctypes.c_int] + [_v] * 5 + [ctypes.c_float] * 5 + [_v] * 5
 _lib.gof_densify_emit.restype = ctypes.c_int
@@ -64,7 +66,7 @@ def densify_and_prune(params, exp_avg, exp_avg_sq, xyz_gradient_accum, xyz_gradi
     flags = torch.empty(4 * max(P, 1), dtype=torch.int32, device=dev)
     offsets = torch.empty_like(flags)
     totals = torch.zeros(4, dtype=torch.int32, device=dev)
-    tmp = torch.empty(P // 2048 + 8 + 1024, dtype=torch.int32, device=dev)
+    tmp = torch.empty(max(int(_lib.gof_densify_scratch_bytes(P)), 1), dtype=torch.uint8, device=dev)
     st = _C._stream()
     with torch.cuda.device(dev):
         _C._check(_lib.gof_densify_plan(P, acc.data_ptr(), acc_abs.data_ptr(), den.data_ptr(), p["scaling"].data_ptr(), p["opacity"].data_ptr(),

@@ -324,11 +324,13 @@ GOF_API int gof_compute_3d_filter(int P, const float* xyz, int n_cams, const flo
                                   void* scratch4, void* stream);
 /* GaussianModel.densify_and_prune (scene/gaussian_model.py:631-707) in three steps (csrc/densify.cu; SURVEY.md 8(f) rank 4):
  * plan   -- the four keep-flags of every Gaussian (kept original | clone | split child 1 | split child 2) from the accumulated
- *           statistics and their exclusive scans; flags / offsets [4][P] u32, totals [4] u32 on the device;
+ *           statistics and their exclusive scans; flags / offsets [4][P] u32, totals [4] u32 on the device, scan_tmp
+ *           gof_densify_scratch_bytes(P) device bytes, 8-byte aligned, contents irrelevant;
  * emit   -- per output row (blocks in that order, ascending source index) its source Gaussian and kind, the re-sampled
  *           positions and the raw scalings; totals_host = the four block sizes read back; noise = optional [3][P][3] standard
  *           normal samples, otherwise Philox(seed);
  * gather -- dst[o,:] = src[src_index[o],:] for one parameter / optimizer-state tensor (zero_new: rows of new Gaussians are 0). */
+GOF_API size_t gof_densify_scratch_bytes(int P);
 GOF_API int gof_densify_plan(int P, const float* accum, const float* accum_abs, const float* denom, const float* scaling_raw,
                              const float* opacity_raw, float max_grad, float abs_threshold, float dense_extent, float min_opacity,
                              float prune_scale, uint32_t* flags, uint32_t* offsets, uint32_t* totals, uint32_t* scan_tmp, void* stream);
@@ -356,8 +358,8 @@ GOF_API int gof_adam_step(size_t n, float* param, float* exp_avg, float* exp_avg
  * pruning is exact, so its output does not depend on its search order; this library searches a Morton-ordered 32-ary box
  * tree instead of testing every 1024-point box (simple_knn.cu:168-181).  Scratch: gof_knn_scratch_bytes(P) device bytes,
  * 256-byte aligned, contents irrelevant.  No allocation and no host synchronisation (the call can be captured in a CUDA
- * graph); kernels run on `stream`.  P = 0 launches nothing; P < 0 fails with GOF_E_INVALID (the reference's int P bounds
- * P below 2^31). */
+ * graph); kernels run on `stream`.  P = 0 launches nothing; P < 0 and P >= 2^30 (the limit of the library's radix sort) fail
+ * with GOF_E_INVALID. */
 GOF_API size_t gof_knn_scratch_bytes(int P);
 GOF_API int gof_knn_mean_dist(int P, const float* points /*[P,3]*/, float* mean_dists /*[P]*/, void* scratch, size_t scratch_bytes,
                               void* stream);

@@ -115,7 +115,7 @@ def test_exclusive_scan_through_densify_plan(P):
     flags = torch.empty(4 * P, dtype=torch.int32, device=dev)
     offsets = torch.empty_like(flags)
     totals = torch.empty(4, dtype=torch.int32, device=dev)
-    tmp = torch.empty(P // 2048 + 8, dtype=torch.int32, device=dev)
+    tmp = torch.empty(int(gof_densify._lib.gof_densify_scratch_bytes(P)), dtype=torch.uint8, device=dev)
     _C._check(gof_densify._lib.gof_densify_plan(P, acc.data_ptr(), acc_abs.data_ptr(), den.data_ptr(), scaling.data_ptr(),
                                                 opacity.data_ptr(), 2e-4, 4e-4, 0.017, 0.05, 0.035, flags.data_ptr(),
                                                 offsets.data_ptr(), totals.data_ptr(), tmp.data_ptr(), _C._stream()))

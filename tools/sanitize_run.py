@@ -5,7 +5,8 @@
 
 parts: render (forward + backward, SH and precomputed-colour paths, multi-batch tile lists), integrate, tetmesh, loss,
 params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), knn (distCUDA2 on clouds of
-1-4097 points, coincident and non-finite rows included).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
+1-4097 points, coincident and non-finite rows included), sort (the multi-word sort, key runs and scan at n = 1 and 4097, three
+words).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
 import os
 import sys
 
@@ -118,8 +119,30 @@ def knn(dev):
         print("knn", kind, P, "finite", int(torch.isfinite(out).sum()), flush=True)
 
 
+def sort(dev):
+    # the sort, run and scan primitives through their test entry points: one item, a chunk and a key, three words (w[0] == ka)
+    from test_gpu_sort_primitives import _bind, _words_arg
+    lib = _bind(_C._lib)
+    st = _C._stream()
+    g = torch.Generator().manual_seed(7)
+    for n in (1, 4097):
+        bits = (32, 31, 9)
+        words = [torch.randint(-2**31, 2**31, (n,), dtype=torch.int32, generator=g).to(dev) for _ in bits]
+        kb, va, vb, head, run = (torch.empty(n, dtype=torch.int32, device=dev) for _ in range(5))
+        ka = words[0]
+        hist = torch.empty(int(lib.gof_probe_scratch_bytes(0, n)), dtype=torch.uint8, device=dev)
+        tmp = torch.empty(int(lib.gof_probe_scratch_bytes(1, n)), dtype=torch.uint8, device=dev)
+        total = torch.empty(1, dtype=torch.int32, device=dev)
+        wp, bp = _words_arg([w.data_ptr() for w in words], bits)
+        _C._check(lib.gof_probe_sort_words_u32(3, wp, bp, n, ka.data_ptr(), kb.data_ptr(), va.data_ptr(), vb.data_ptr(), hist.data_ptr(), 1, st))
+        _C._check(lib.gof_probe_key_runs_u32(3, wp, bp, vb.data_ptr(), n, head.data_ptr(), run.data_ptr(), tmp.data_ptr(), total.data_ptr(), st))
+        _C._check(lib.gof_probe_exclusive_scan_u32(run.data_ptr(), head.data_ptr(), tmp.data_ptr(), total.data_ptr(), n, st))
+        torch.cuda.synchronize()
+        print("sort n =", n, "scan total", int(total.item()) & 0xFFFFFFFF, flush=True)
+
+
 PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf,
-         "knn": knn}
+         "knn": knn, "sort": sort}
 
 if __name__ == "__main__":
     dev = torch.device("cuda")
