@@ -1,7 +1,8 @@
 // param_ops.cuh -- the parameter prologue / epilogue around the rasterizer (SURVEY.md 8(f) rank 2; reference:
 // scene/gaussian_model.py:152-194 activations with the 3D filter, :360 torch.optim.Adam(eps=1e-15)).
-// STAGED COMPONENT, a caller of the rasterizer.  Per-Gaussian functions are host/device so that tests/hostmath can run this
-// very source on the CPU against golden vectors generated from the reference's own Python.
+// A caller of the rasterizer.  Per-Gaussian functions are host/device so that tests/hostmath can run this very source on the
+// CPU against golden vectors generated from the reference's own Python; tests/test_gpu_train_step.py checks the CUDA kernels
+// against fp64 restatements of the formulas below.
 //
 //   activate:           raw (log-scale[3], quaternion[4], opacity logit, filter_3D, f_dc[3], f_rest[15*3])
 //                       -> scales = sqrt(exp(s)^2 + f^2), rotations = q / max(|q|, 1e-12),

@@ -1,7 +1,8 @@
 """Parameter prologue / epilogue around the rasterizer (SURVEY.md section 8(f) rank 2; reference:
 scene/gaussian_model.py:152-194 and :360) through the C ABI (`gof_activate_params*`, `gof_adam_step`, csrc/param_ops.cu).
-STAGED: the arithmetic is verified on the CPU against goldens generated from the reference's Python
-(tests/test_param_ops_host.py); the CUDA wrappers are exercised by tests/test_gpu_param_ops.py.
+The arithmetic is verified on the CPU against goldens generated from the reference's Python (tests/test_param_ops_host.py);
+the CUDA kernels against those goldens (tests/test_gpu_param_ops.py) and against fp64 restatements at up to 10^6 Gaussians
+(tests/test_gpu_train_step.py).
 
     scales, rotations, opacities, shs = activate(_scaling, _rotation, _opacity, filter_3D, _features_dc, _features_rest)
         == (pc.get_scaling_with_3D_filter, pc.get_rotation, pc.get_opacity_with_3D_filter, pc.get_features), differentiable
@@ -27,7 +28,12 @@ _lib.gof_adam_step.argtypes = [ctypes.c_size_t, _v, _v, _v, _v, ctypes.c_double,
 def _f32(t):
     if not t.is_cuda or t.dtype != torch.float32:
         raise RuntimeError("gof_b200 params: CUDA float32 tensors required (no CPU path)")
-    return t.contiguous()
+    # the kernels move rotations as float4: a contiguous view at an odd storage offset (a parameter sliced out of a flat
+    # buffer) is copied to a fresh, aligned allocation, as the rasterizer binding does (_C._c)
+    t = t.contiguous()
+    if t.numel() and (t.data_ptr() & 15):
+        t = t.clone(memory_format=torch.contiguous_format)
+    return t
 
 
 class _Activate(torch.autograd.Function):

@@ -307,7 +307,8 @@ GOF_API int gof_view_loss(int W, int H, const float* render, const float* gt, co
 /* Parameter prologue / epilogue around the rasterizer (SURVEY.md 8(f) rank 2; callers of the rasterizer, staged):
  * activations with the 3D filter (scene/gaussian_model.py:152-194: scales = sqrt(exp(s)^2 + f^2), rotations = normalize(q),
  * opacity = sigmoid(o) * sqrt(prod exp(s)^2 / prod(exp(s)^2 + f^2)), shs = cat(f_dc, f_rest)), their backward (raw-parameter
- * gradients from the rasterizer's output gradients), and one torch.optim.Adam step (:360, eps 1e-15).  Device pointers, fp32. */
+ * gradients from the rasterizer's output gradients), and one torch.optim.Adam step (:360, eps 1e-15).  Device pointers, fp32.
+ * Rotation arrays (input, output and their gradients) must be 16-byte aligned; otherwise the call returns GOF_E_INVALID. */
 GOF_API int gof_activate_params(int P, int M_rest, const float* scaling_raw, const float* rotation_raw, const float* opacity_raw,
                                 const float* filter_3D, const float* features_dc, const float* features_rest, float* scales,
                                 float* rotations, float* opacities, float* shs, void* stream);

@@ -6,7 +6,7 @@
 parts: render (forward + backward, SH and precomputed-colour paths, multi-batch tile lists), integrate, tetmesh, loss,
 params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), knn (distCUDA2 on clouds of
 1-4097 points, coincident and non-finite rows included), sort (the multi-word sort, key runs and scan at n = 1 and 4097, three
-words).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
+words), appearance (the weight-gradient kernel of the appearance network, several tiles per CTA).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
 import os
 import sys
 
@@ -141,8 +141,24 @@ def sort(dev):
         print("sort n =", n, "scan total", int(total.item()) & 0xFFFFFFFF, flush=True)
 
 
+def appearance(dev):
+    # the appearance network's weight gradient (conv_wgrad.cu) for every channel pair: W % 4 == 0 (cp.async double buffer) with
+    # 1 024+ tiles, i.e. at least 3 per CTA of the persistent grid on an H100, so that the prefetch, the buffer swap and the refill
+    # barrier run; the scalar fill (odd W); and an image smaller than one tile
+    import gof_appearance
+    lib = gof_appearance._wgrad_lib()
+    g = torch.Generator().manual_seed(3)
+    for (co, ci), (H, W) in (((16, 16), (264, 1024)), ((3, 16), (264, 1024)), ((16, 8), (264, 1024)), ((16, 16), (257, 1021)), ((3, 16), (5, 20))):
+        x = torch.randn(ci, H, W, generator=g).to(dev)
+        gy = torch.randn(co, H, W, generator=g).to(dev)
+        dW, db = torch.zeros(co, ci, 3, 3, device=dev), torch.zeros(co, device=dev)
+        _C._check(lib.gof_conv3x3_wgrad(co, ci, H, W, x.data_ptr(), gy.data_ptr(), dW.data_ptr(), db.data_ptr(), _C._stream()))
+        torch.cuda.synchronize()
+        print("appearance", (co, ci), (H, W), "|dW|max", float(dW.abs().max()), flush=True)
+
+
 PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf,
-         "knn": knn, "sort": sort}
+         "knn": knn, "sort": sort, "appearance": appearance}
 
 if __name__ == "__main__":
     dev = torch.device("cuda")
