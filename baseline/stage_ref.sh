@@ -1,7 +1,7 @@
 #!/usr/bin/env bash
 # TEST / BASELINE INFRASTRUCTURE ONLY.  Stages the UNMODIFIED Python sources of the reference that sit either side of the
 # rasterizer (its autograd wrapper, gaussian_renderer.render/integrate, the loss / depth / SH helpers, the appearance network,
-# utils/tetmesh.py, train.py and extract_mesh.py as text) into baseline/_ref/gof_ref_py/ -- git-ignored, but shipped to the
+# utils/tetmesh.py, train.py, extract_mesh.py and dtu_eval/eval.py as text) into baseline/_ref/gof_ref_py/ -- git-ignored, but shipped to the
 # GPU box -- so that tests and `bench.py --impl reference` can run the reference's OWN code there (/root/reference does not
 # exist on the GPU box).  Nothing under gaussian-opacity-fields_b200/ reads this directory.
 set -euo pipefail
@@ -22,4 +22,5 @@ cp "$REF/train.py" "$OUT/text/train.py"
 cp "$REF/extract_mesh.py" "$OUT/text/extract_mesh.py"
 cp "$REF/scene/gaussian_model.py" "$OUT/text/gaussian_model.py"
 cp "$REF/scene/cameras.py" "$OUT/text/cameras.py"
+cp "$REF/dtu_eval/eval.py" "$OUT/text/dtu_eval.py"
 echo "[stage_ref] staged reference Python into $OUT"

@@ -365,6 +365,35 @@ GOF_API size_t gof_knn_scratch_bytes(int P);
 GOF_API int gof_knn_mean_dist(int P, const float* points /*[P,3]*/, float* mean_dists /*[P]*/, void* scratch, size_t scratch_bytes,
                               void* stream);
 
+/* The DTU mesh evaluation of dtu_eval/eval.py (DESIGN section 4.6).  Points are device double [n,3]; every step is a
+ * sequence of single IEEE double operations in the order written in DESIGN, so oracle/dtu_eval_oracle.py reproduces it bit for
+ * bit.  Coordinates must be finite (the Python layer refuses others); any point count of 2^30 or more is refused.
+ *
+ * Mesh sampling (eval.py:48-71) at `density` = r: out [num_vertices + num_samples, 3] = the vertices in order, then per face
+ * with area2 > 0, per row i, per column j, the samples of the face.  Count first, with scratch of
+ * gof_mesh_sample_scratch_bytes(num_faces) bytes (256-byte aligned) and a second, row-sized scratch taken through row_alloc;
+ * then emit with both.  A face index outside [0, num_vertices) fails with GOF_E_INVALID. */
+GOF_API size_t gof_mesh_sample_scratch_bytes(int64_t num_faces);
+GOF_API int gof_mesh_sample_count(int64_t num_vertices, const double* vertices, int64_t num_faces, const int64_t* faces /*[F,3]*/,
+                                  double density, void* scratch, size_t scratch_bytes, gof_alloc_fn row_alloc, void* row_user,
+                                  int64_t* num_samples_out, void* stream);
+GOF_API int gof_mesh_sample_emit(int64_t num_vertices, const double* vertices, int64_t num_faces, const int64_t* faces, double density,
+                                 const void* scratch, const void* row_scratch, int64_t num_samples, double* out, void* stream);
+/* Greedy downsample (eval.py:86-94) in the order perm (a permutation of 0..n-1, else GOF_E_INVALID): position k holds point
+ * perm[k]; kept[k] = 1 iff no kept position k' < k has ((dx*dx + dy*dy) + dz*dz) <= radius*radius.  Scratch of
+ * gof_ordered_downsample_scratch_bytes(n) bytes; the neighbour list (4 bytes per pair) through pair_alloc.  More than
+ * 2^32 - 1 pairs fail with GOF_E_INVALID.  *num_rounds_out: the rounds the parallel decision took. */
+GOF_API size_t gof_ordered_downsample_scratch_bytes(int64_t n);
+GOF_API int gof_ordered_downsample(int64_t n, const double* points, const uint32_t* perm, double radius, uint8_t* kept,
+                                   int64_t* num_rounds_out, int64_t* num_pairs_out, void* scratch, size_t scratch_bytes,
+                                   gof_alloc_fn pair_alloc, void* pair_user, void* stream);
+/* out[i] = min over the n_ref reference points of ((dx*dx + dy*dy) + dz*dz) to query i, or its sqrt if take_sqrt (eval.py:119-133).
+ * n_ref = 0 with queries fails with GOF_E_INVALID.  Scratch of gof_nn_dist_scratch_bytes(n_ref, n_query) bytes; no allocation
+ * and no host synchronisation. */
+GOF_API size_t gof_nn_dist_scratch_bytes(int64_t n_ref, int64_t n_query);
+GOF_API int gof_nn_dist(int64_t n_ref, const double* ref, int64_t n_query, const double* query, double* out, int take_sqrt,
+                        void* scratch, size_t scratch_bytes, void* stream);
+
 GOF_API const char* gof_last_error(void);
 GOF_API int gof_version(void);
 

@@ -4,7 +4,7 @@
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python tools/sanitize_run.py [parts...]
 
 parts: render (forward + backward, SH and precomputed-colour paths, multi-batch tile lists), integrate, tetmesh, loss,
-params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), knn (distCUDA2 on clouds of
+params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), dtu (mesh sampling, downsample, 1-NN of the DTU evaluation), knn (distCUDA2 on clouds of
 1-4097 points, coincident and non-finite rows included), sort (the multi-word sort, key runs and scan at n = 1 and 4097, three
 words), appearance (the weight-gradient kernel of the appearance network, several tiles per CTA).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
 import os
@@ -119,6 +119,20 @@ def knn(dev):
         print("knn", kind, P, "finite", int(torch.isfinite(out).sum()), flush=True)
 
 
+def dtu(dev):
+    # the DTU evaluation (dtu_eval.cu): a mesh with a degenerate face, the downsample with a pair list, 1-NN with queries outside
+    # the reference box
+    import gof_dtu_eval
+    rng = np.random.default_rng(4)
+    V = torch.from_numpy(rng.uniform(-2, 2, (40, 3))).to(dev)
+    F = torch.from_numpy(np.concatenate([rng.integers(0, 40, (30, 3)), [[1, 1, 2]]])).to(dev)
+    pts = gof_dtu_eval.sample_mesh(V, F, 0.1)
+    kept, rounds = gof_dtu_eval.ordered_downsample(pts, torch.randperm(pts.shape[0], device=dev), 0.1)
+    d = gof_dtu_eval.nn_dist(pts[kept][:33], pts * 1.5)
+    torch.cuda.synchronize()
+    print("dtu samples", pts.shape[0], "kept", int(kept.sum()), "rounds", rounds, "max dist", float(d.max()), flush=True)
+
+
 def sort(dev):
     # the sort, run and scan primitives through their test entry points: one item, a chunk and a key, three words (w[0] == ka)
     from test_gpu_sort_primitives import _bind, _words_arg
@@ -158,7 +172,7 @@ def appearance(dev):
 
 
 PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf,
-         "knn": knn, "sort": sort, "appearance": appearance}
+         "knn": knn, "dtu": dtu, "sort": sort, "appearance": appearance}
 
 if __name__ == "__main__":
     dev = torch.device("cuda")
