@@ -349,12 +349,18 @@ DownLayout down_layout(int n) {
 // ---- nearest-neighbour distances --------------------------------------------------------------------------------
 
 // One warp per 32 Morton-sorted queries (sorted slot s -> query order[s]); best = the smallest squared distance to any point of
-// the reference tree.
+// the reference tree.  INDEXED: the search starts from best = r2 and accepts a point only below it, ids[slot] is the original
+// index of the tree point at a slot, and among points at the same smallest distance the lowest original index wins; nodes and
+// children are entered while their bound is <= best (not <), so a tied point is never pruned.  out = best (INFINITY when no
+// point lies below r2) and out_idx = its index or -1.
+template <bool INDEXED>
 __global__ void __launch_bounds__(SEARCH_WARPS * 32) k_nn_search(int nq, gof_tree::Tree tree, const double* __restrict__ xs,
                                                                  const double* __restrict__ ys, const double* __restrict__ zs,
                                                                  const double4* __restrict__ boxes, const double* __restrict__ qxs,
                                                                  const double* __restrict__ qys, const double* __restrict__ qzs,
-                                                                 const uint32_t* __restrict__ qorder, int take_sqrt, double* __restrict__ out) {
+                                                                 const uint32_t* __restrict__ qorder, int take_sqrt, double* __restrict__ out,
+                                                                 int n_ref, const uint32_t* __restrict__ ids, double r2,
+                                                                 int32_t* __restrict__ out_idx) {
   __shared__ uint32_t s_stack[SEARCH_WARPS][STACK];
   __shared__ int s_count[MAX_LEVELS];
   __shared__ long long s_offset[MAX_LEVELS];
@@ -370,7 +376,8 @@ __global__ void __launch_bounds__(SEARCH_WARPS * 32) k_nn_search(int nq, gof_tre
   const int self = group * LEAF + lane;
   const double qx = qxs[self], qy = qys[self], qz = qzs[self];
   const bool valid = self < nq && finite3(qx, qy, qz);
-  double best = INFINITY;
+  double best = INDEXED ? r2 : INFINITY;
+  int bi = -1;
   const double inf = INFINITY;
   const double qlx = warp_vmin(valid ? qx : inf), qly = warp_vmin(valid ? qy : inf), qlz = warp_vmin(valid ? qz : inf);
   const double qhx = warp_vmax(valid ? qx : -inf), qhy = warp_vmax(valid ? qy : -inf), qhz = warp_vmax(valid ? qz : -inf);
@@ -382,16 +389,23 @@ __global__ void __launch_bounds__(SEARCH_WARPS * 32) k_nn_search(int nq, gof_tre
     const int lvl = (int)(e >> LEVEL_SHIFT), node = (int)(e & ((1u << LEVEL_SHIFT) - 1));
     const double4* nb = boxes + 2 * (s_offset[lvl] + node);
     const double4 lo = nb[0], hi = nb[1];
-    const bool need = valid && sq3(gap(qx, qx, lo.x, hi.x), gap(qy, qy, lo.y, hi.y), gap(qz, qz, lo.z, hi.z)) < best;
+    const double bound = sq3(gap(qx, qx, lo.x, hi.x), gap(qy, qy, lo.y, hi.y), gap(qz, qz, lo.z, hi.z));
+    const bool need = valid && (INDEXED ? bound <= best : bound < best);
     if (!__any_sync(0xffffffffu, need)) continue;
     if (lvl == 0) {
       const size_t ps = (size_t)node * LEAF + lane;
       const double cx = xs[ps], cy = ys[ps], cz = zs[ps];
+      const int ci = INDEXED && (long long)ps < n_ref ? (int)ids[ps] : 0;
 #pragma unroll 4
       for (int k = 0; k < LEAF; ++k) {
         const double px = __shfl_sync(0xffffffffu, cx, k), py = __shfl_sync(0xffffffffu, cy, k), pz = __shfl_sync(0xffffffffu, cz, k);
         const double d = sq3(__dsub_rn(px, qx), __dsub_rn(py, qy), __dsub_rn(pz, qz));
-        if (d < best) best = d;                // NaN padding never enters
+        if (INDEXED) {
+          const int pi = __shfl_sync(0xffffffffu, ci, k);
+          if (d < best || (d == best && bi >= 0 && pi < bi)) { best = d; bi = pi; }   // NaN padding never enters
+        } else if (d < best) {
+          best = d;                            // NaN padding never enters
+        }
       }
       continue;
     }
@@ -399,12 +413,14 @@ __global__ void __launch_bounds__(SEARCH_WARPS * 32) k_nn_search(int nq, gof_tre
     const double thr = warp_vmax(valid ? best : 0.0);
     const int c = node * LEAF + lane;
     double cb = INFINITY;
-    if (c < s_count[lvl - 1]) {
+    const bool exists = c < s_count[lvl - 1];
+    if (exists) {
       const double4* cbx = boxes + 2 * (s_offset[lvl - 1] + c);
       const double4 clo = cbx[0], chi = cbx[1];
       cb = sq3(gap(qlx, qhx, clo.x, chi.x), gap(qly, qhy, clo.y, chi.y), gap(qlz, qhz, clo.z, chi.z));
     }
-    const bool push = cb < thr;
+    // INDEXED with r2 = inf: thr may be inf, so a missing child (cb = inf) must be excluded explicitly
+    const bool push = INDEXED ? exists && cb <= thr : cb < thr;
     const uint32_t mask = __ballot_sync(0xffffffffu, push);
     int rank = 0;
 #pragma unroll 8
@@ -418,21 +434,85 @@ __global__ void __launch_bounds__(SEARCH_WARPS * 32) k_nn_search(int nq, gof_tre
     sp += n;
     __syncwarp();
   }
-  if (self < nq) out[qorder[self]] = take_sqrt ? __dsqrt_rn(best) : best;
+  if (self < nq) {
+    if (INDEXED) {
+      out[qorder[self]] = bi >= 0 ? best : INFINITY;
+      out_idx[qorder[self]] = bi;
+    } else {
+      out[qorder[self]] = take_sqrt ? __dsqrt_rn(best) : best;
+    }
+  }
 }
 
-struct NnLayout { gof_tree::Layout t; size_t qhi1, qhi2, qka, qkb, qva, qvb, qhist, qxs, qys, qzs, bytes; };
-NnLayout nn_layout(int n_ref, int n_query) {
-  NnLayout L; size_t o = 0;
-  auto take = layout_taker(o);
-  L.t = gof_tree::tree_layout<double>(n_ref, take);
+// The queries' half of a 1-NN search: keys, sort buffers and the gathered planes padded to whole groups of 32
+struct QueryLayout { size_t qhi1, qhi2, qka, qkb, qva, qvb, qhist, qxs, qys, qzs; };
+template <class Take>
+QueryLayout query_layout(int n_query, Take&& take) {
+  QueryLayout L;
   const size_t q = (size_t)n_query, padded = (q + LEAF - 1) / LEAF * LEAF;
   L.qhi1 = take(q * 4); L.qhi2 = take(q * 4);
   L.qka = take(q * 4); L.qkb = take(q * 4); L.qva = take(q * 4); L.qvb = take(q * 4);
   L.qhist = take(gof_sort_scratch_bytes(q));
   L.qxs = take(padded * 8); L.qys = take(padded * 8); L.qzs = take(padded * 8);
+  return L;
+}
+
+struct NnLayout { gof_tree::Layout t; QueryLayout q; size_t bytes; };
+NnLayout nn_layout(int n_ref, int n_query) {
+  NnLayout L; size_t o = 0;
+  auto take = layout_taker(o);
+  L.t = gof_tree::tree_layout<double>(n_ref, take);
+  L.q = query_layout(n_query, take);
   L.bytes = o;
   return L;
+}
+
+// A query scratch of gof_nn_query is stamped after its queries are sorted, so that a later call may reuse the order; the stamp
+// names the query count, and an order is only a permutation of 0 .. nq-1 when the stamp says nq.
+__host__ __device__ constexpr unsigned long long order_stamp(int nq) { return 0x6e6e5f6f72646572ull ^ (unsigned long long)nq; }
+
+__global__ void k_order_stamp(unsigned long long* stamp, int nq) { *stamp = order_stamp(nq); }
+
+// Before an order is reused: if the scratch holds no order for nq queries (fresh, or sorted for another count), the identity
+// order is used instead.  The order changes the speed of the search only, never its results.
+__global__ void __launch_bounds__(THREADS) k_order_guard(int nq, const unsigned long long* __restrict__ stamp, uint32_t* __restrict__ va) {
+  const int s = blockIdx.x * THREADS + threadIdx.x;
+  if (s < nq && *stamp != order_stamp(nq)) va[s] = (uint32_t)s;
+}
+
+// The queries against a built tree: keyed against the tree's box (clamped), sorted unless `sort` is false (then the order left
+// in the query scratch by an earlier call with the same n_query is reused, checked against `stamp`), gathered and searched.
+// stamp: NULL (gof_nn_dist, always sorting) or the query scratch's stamp word.  No host synchronisation.
+template <bool INDEXED>
+int nn_query(int n_ref, const gof_tree::Bufs<double>& b, int nq, const double* query, char* S, const QueryLayout& L, bool sort,
+             unsigned long long* stamp, int take_sqrt, double* out, double r2, int32_t* out_idx, cudaStream_t st) {
+  int rc;
+  const gof_tree::Tree tree = gof_tree::make_tree(n_ref);
+  const int padded = (nq + LEAF - 1) / LEAF * LEAF;
+  uint32_t *hi1 = (uint32_t*)(S + L.qhi1), *hi2 = (uint32_t*)(S + L.qhi2), *ka = (uint32_t*)(S + L.qka), *kb = (uint32_t*)(S + L.qkb);
+  uint32_t *va = (uint32_t*)(S + L.qva), *vb = (uint32_t*)(S + L.qvb), *hist = (uint32_t*)(S + L.qhist);
+  double *qxs = (double*)(S + L.qxs), *qys = (double*)(S + L.qys), *qzs = (double*)(S + L.qzs);
+  if (sort) {
+    GOF_LAUNCH("dtu_query_keys", st, gof_tree::k_tree_keys<double><<<blocks_for((size_t)nq, THREADS), THREADS, 0, st>>>(nq, query, b.bbox,
+                                                                                                                       ka, hi1, hi2));
+    GOF_LAUNCH_CHECK(false, st);
+    const GofKeyWords key{{ka, hi1, hi2}, {32, 32, 32}, 3};
+    if ((rc = gof_sort_words_u32(key, (size_t)nq, GofSortBufs{ka, kb, va, vb, hist}, va, false, st)) != GOF_OK) return rc;
+    if (stamp) {
+      GOF_LAUNCH("dtu_order_stamp", st, k_order_stamp<<<1, 1, 0, st>>>(stamp, nq));
+      GOF_LAUNCH_CHECK(false, st);
+    }
+  } else {
+    GOF_LAUNCH("dtu_order_guard", st, k_order_guard<<<blocks_for((size_t)nq, THREADS), THREADS, 0, st>>>(nq, stamp, va));
+    GOF_LAUNCH_CHECK(false, st);
+  }
+  GOF_LAUNCH("dtu_query_gather", st, gof_tree::k_tree_gather<double><<<blocks_for((size_t)padded, THREADS), THREADS, 0, st>>>(
+                                         nq, padded, query, va, qxs, qys, qzs));
+  GOF_LAUNCH_CHECK(false, st);
+  GOF_LAUNCH("dtu_nn_search", st, k_nn_search<INDEXED><<<blocks_for((size_t)padded / LEAF, SEARCH_WARPS), SEARCH_WARPS * 32, 0, st>>>(
+                                      nq, tree, b.xs, b.ys, b.zs, b.boxes, qxs, qys, qzs, va, take_sqrt, out, n_ref, b.va, r2, out_idx));
+  GOF_LAUNCH_CHECK(false, st);
+  return GOF_OK;
 }
 
 int check_count(int64_t n, const char* what, const char* fn) {
@@ -644,21 +724,84 @@ extern "C" GOF_API int gof_nn_dist(int64_t n_ref, const double* ref, int64_t n_q
   const gof_tree::Bufs<double> b = gof_tree::carve<double>(S, L.t);
   const gof_tree::Tree tree = gof_tree::make_tree((int)n_ref);
   if ((rc = gof_tree::build_tree<double>((int)n_ref, ref, b, tree, st)) != GOF_OK) return rc;
-  // queries: keyed against the reference box (clamped), sorted, gathered into planes padded to whole groups of 32
-  const int nq = (int)n_query, padded = (nq + LEAF - 1) / LEAF * LEAF;
-  uint32_t *hi1 = (uint32_t*)(S + L.qhi1), *hi2 = (uint32_t*)(S + L.qhi2), *ka = (uint32_t*)(S + L.qka), *kb = (uint32_t*)(S + L.qkb);
-  uint32_t *va = (uint32_t*)(S + L.qva), *vb = (uint32_t*)(S + L.qvb), *hist = (uint32_t*)(S + L.qhist);
-  double *qxs = (double*)(S + L.qxs), *qys = (double*)(S + L.qys), *qzs = (double*)(S + L.qzs);
-  GOF_LAUNCH("dtu_query_keys", st, gof_tree::k_tree_keys<double><<<blocks_for((size_t)nq, THREADS), THREADS, 0, st>>>(nq, query, b.bbox,
-                                                                                                                     ka, hi1, hi2));
-  GOF_LAUNCH_CHECK(false, st);
-  const GofKeyWords key{{ka, hi1, hi2}, {32, 32, 32}, 3};
-  if ((rc = gof_sort_words_u32(key, (size_t)nq, GofSortBufs{ka, kb, va, vb, hist}, va, false, st)) != GOF_OK) return rc;
-  GOF_LAUNCH("dtu_query_gather", st, gof_tree::k_tree_gather<double><<<blocks_for((size_t)padded, THREADS), THREADS, 0, st>>>(
-                                         nq, padded, query, va, qxs, qys, qzs));
-  GOF_LAUNCH_CHECK(false, st);
-  GOF_LAUNCH("dtu_nn_search", st, k_nn_search<<<blocks_for((size_t)padded / LEAF, SEARCH_WARPS), SEARCH_WARPS * 32, 0, st>>>(
-                                      nq, tree, b.xs, b.ys, b.zs, b.boxes, qxs, qys, qzs, va, take_sqrt, out));
-  GOF_LAUNCH_CHECK(false, st);
-  return GOF_OK;
+  return nn_query<false>((int)n_ref, b, (int)n_query, query, S, L.q, true, nullptr, take_sqrt, out, 0.0, nullptr, st);
+}
+
+// ---- the same search split into a persistent tree and repeated queries (Tanks and Temples ICP, DESIGN section 4.7) ----------
+
+namespace {
+gof_tree::Layout tree_only_layout(int n_ref, size_t* bytes) {
+  size_t o = 0;
+  auto take = layout_taker(o);
+  const gof_tree::Layout L = gof_tree::tree_layout<double>(n_ref, take);
+  *bytes = o;
+  return L;
+}
+// gof_nn_query's scratch: the order stamp, then the queries' buffers
+QueryLayout query_only_layout(int n_query, size_t* stamp, size_t* bytes) {
+  size_t o = 0;
+  auto take = layout_taker(o);
+  *stamp = take(8);
+  const QueryLayout L = query_layout(n_query, take);
+  *bytes = o;
+  return L;
+}
+}  // namespace
+
+extern "C" GOF_API size_t gof_nn_tree_scratch_bytes(int64_t n_ref) {
+  if (n_ref <= 0 || (uint64_t)n_ref >= SORT_LIMIT) return 0;
+  size_t bytes;
+  tree_only_layout((int)n_ref, &bytes);
+  return bytes;
+}
+
+extern "C" GOF_API int gof_nn_tree_build(int64_t n_ref, const double* ref, void* tree_scratch, size_t scratch_bytes, void* stream) {
+  int rc;
+  if ((rc = check_count(n_ref, "reference points", "nn_tree_build")) != GOF_OK) return rc;
+  if (n_ref == 0) { gof_set_error("nn_tree_build: no reference points"); return GOF_E_INVALID; }
+  if (!ref || !tree_scratch) { gof_set_error("nn_tree_build: NULL argument"); return GOF_E_INVALID; }
+  size_t need;
+  const gof_tree::Layout L = tree_only_layout((int)n_ref, &need);
+  if (scratch_bytes < need) {
+    gof_set_error("nn_tree_build: scratch of %zu bytes, %zu needed (gof_nn_tree_scratch_bytes)", scratch_bytes, need);
+    return GOF_E_INVALID;
+  }
+  const gof_tree::Bufs<double> b = gof_tree::carve<double>(static_cast<char*>(tree_scratch), L);
+  return gof_tree::build_tree<double>((int)n_ref, ref, b, gof_tree::make_tree((int)n_ref), (cudaStream_t)stream);
+}
+
+extern "C" GOF_API size_t gof_nn_query_scratch_bytes(int64_t n_query) {
+  if (n_query <= 0 || (uint64_t)n_query >= SORT_LIMIT) return 0;
+  size_t stamp, bytes;
+  query_only_layout((int)n_query, &stamp, &bytes);
+  return bytes;
+}
+
+extern "C" GOF_API int gof_nn_query(int64_t n_ref, void* tree_scratch, size_t tree_scratch_bytes, int64_t n_query, const double* query,
+                                    double r2, int reuse_order, int32_t* out_index, double* out_d2, void* query_scratch,
+                                    size_t scratch_bytes, void* stream) {
+  int rc;
+  if ((rc = check_count(n_ref, "reference points", "nn_query")) != GOF_OK) return rc;
+  if ((rc = check_count(n_query, "query points", "nn_query")) != GOF_OK) return rc;
+  if (!(r2 >= 0.0)) { gof_set_error("nn_query: r2 = %g must be >= 0", r2); return GOF_E_INVALID; }
+  if (n_query == 0) return GOF_OK;
+  if (n_ref == 0) { gof_set_error("nn_query: no reference points for %lld queries", (long long)n_query); return GOF_E_INVALID; }
+  if (!tree_scratch || !query || !out_index || !out_d2 || !query_scratch) { gof_set_error("nn_query: NULL argument"); return GOF_E_INVALID; }
+  size_t tree_need;
+  const gof_tree::Layout TL = tree_only_layout((int)n_ref, &tree_need);
+  if (tree_scratch_bytes < tree_need) {
+    gof_set_error("nn_query: tree scratch of %zu bytes, %zu needed for %lld reference points (gof_nn_tree_scratch_bytes)",
+                  tree_scratch_bytes, tree_need, (long long)n_ref);
+    return GOF_E_INVALID;
+  }
+  size_t stamp, need;
+  const QueryLayout L = query_only_layout((int)n_query, &stamp, &need);
+  if (scratch_bytes < need) {
+    gof_set_error("nn_query: scratch of %zu bytes, %zu needed (gof_nn_query_scratch_bytes)", scratch_bytes, need);
+    return GOF_E_INVALID;
+  }
+  char* QS = static_cast<char*>(query_scratch);
+  const gof_tree::Bufs<double> b = gof_tree::carve<double>(static_cast<char*>(tree_scratch), TL);
+  return nn_query<true>((int)n_ref, b, (int)n_query, query, QS, L, reuse_order == 0, (unsigned long long*)(QS + stamp), 0, out_d2, r2,
+                        out_index, (cudaStream_t)stream);
 }

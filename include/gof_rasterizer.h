@@ -394,6 +394,48 @@ GOF_API size_t gof_nn_dist_scratch_bytes(int64_t n_ref, int64_t n_query);
 GOF_API int gof_nn_dist(int64_t n_ref, const double* ref, int64_t n_query, const double* query, double* out, int take_sqrt,
                         void* scratch, size_t scratch_bytes, void* stream);
 
+/* The same 1-NN search split in two, for repeated queries against one cloud (the Tanks and Temples ICP, DESIGN section 4.7):
+ * gof_nn_tree_build keeps the tree over ref in tree_scratch (gof_nn_tree_scratch_bytes(n_ref) bytes, kept intact between
+ * queries); gof_nn_query writes, for every query, out_index = the reference point with the smallest ((dx*dx + dy*dy) + dz*dz)
+ * strictly below r2, the lowest index among equals, or -1, and out_d2 = that value (INFINITY for -1).  Query scratch of
+ * gof_nn_query_scratch_bytes(n_query) bytes.  tree_scratch_bytes is the size of tree_scratch, checked against n_ref.
+ * reuse_order != 0 skips the Morton sort of the queries and reuses the order that an earlier call with this query scratch and
+ * the same n_query stamped into it; a scratch without such a stamp (fresh, or sorted for another count) is searched in input
+ * order instead.  Results never depend on the order.  No allocation and no host synchronisation. */
+GOF_API size_t gof_nn_tree_scratch_bytes(int64_t n_ref);
+GOF_API int gof_nn_tree_build(int64_t n_ref, const double* ref, void* tree_scratch, size_t scratch_bytes, void* stream);
+GOF_API size_t gof_nn_query_scratch_bytes(int64_t n_query);
+GOF_API int gof_nn_query(int64_t n_ref, void* tree_scratch, size_t tree_scratch_bytes, int64_t n_query, const double* query, double r2,
+                         int reuse_order, int32_t* out_index, double* out_d2, void* query_scratch, size_t scratch_bytes, void* stream);
+
+/* The Tanks and Temples evaluation of eval_tnt/run.py (DESIGN section 4.7).  Points are device double [n,3], finite; any count
+ * of 2^30 or more is refused with GOF_E_INVALID.  A transformation is a host double[16], row-major; a point maps to
+ * (((m00*x + m01*y) + m02*z) + m03) / w per row, w the fourth row's value.
+ *
+ * Polygon-volume crop (SelectionPolygonVolume.crop_point_cloud), optionally after `transform` (NULL: none): axis = the
+ * orthogonal axis (0, 1, 2), polygon_uv = host [num_vertices, 2] of the polygon's two other coordinates in ascending axis order,
+ * 3 <= num_vertices <= 3072.  out [*num_out, 3] = the kept points in input order (capacity n), out_index (or NULL) their
+ * input indices.  Scratch of gof_crop_scratch_bytes(n) bytes; reads back the kept count. */
+GOF_API size_t gof_crop_scratch_bytes(int64_t n);
+GOF_API int gof_crop_polygon(int64_t n, const double* points, const double* transform, int axis, double axis_min, double axis_max,
+                             int num_vertices, const double* polygon_uv, double* out, uint32_t* out_index, int64_t* num_out,
+                             void* scratch, size_t scratch_bytes, void* stream);
+/* Voxel down-sample (PointCloud.voxel_down_sample): out [*num_out, 3] (capacity n) = per occupied voxel the mean of its points,
+ * summed in input order, in ascending (x, y, z) voxel index order.  voxel * INT_MAX below the extent of the box grown by
+ * voxel / 2 fails with GOF_E_INVALID ("voxel_size is too small"), and so does a point with a non-finite coordinate.  Scratch of gof_voxel_down_sample_scratch_bytes(n) bytes. */
+GOF_API size_t gof_voxel_down_sample_scratch_bytes(int64_t n);
+GOF_API int gof_voxel_down_sample(int64_t n, const double* points, double voxel, double* out, int64_t* num_out, void* scratch,
+                                  size_t scratch_bytes, void* stream);
+/* Point-to-point ICP moments over the pairs (i, index[i]), index[i] >= 0, with d2[i] their squared distances.  Host
+ * moments[18] = count, sum d2, mean src[3], mean tgt[3] (sum * (1 / count)), sum (t - mt)(s - ms)^T [3][3] row-major by target
+ * axis, sum |s - ms|^2.  Fixed summation order, independent of the launch: two runs are bit-identical.  Scratch of
+ * gof_icp_moments_scratch_bytes(n) bytes; one read-back. */
+GOF_API size_t gof_icp_moments_scratch_bytes(int64_t n);
+GOF_API int gof_icp_moments(int64_t n, const double* src, const double* tgt, const int32_t* index, const double* d2, double* moments,
+                            void* scratch, size_t scratch_bytes, void* stream);
+/* points <- transform(points), in place. */
+GOF_API int gof_transform_points(int64_t n, double* points, const double* transform, void* stream);
+
 GOF_API const char* gof_last_error(void);
 GOF_API int gof_version(void);
 

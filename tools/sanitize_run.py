@@ -4,7 +4,8 @@
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python tools/sanitize_run.py [parts...]
 
 parts: render (forward + backward, SH and precomputed-colour paths, multi-batch tile lists), integrate, tetmesh, loss,
-params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), dtu (mesh sampling, downsample, 1-NN of the DTU evaluation), knn (distCUDA2 on clouds of
+params, filter, tsdf (touch / activate with pool growth / integrate / marching cubes), dtu (mesh sampling, downsample, 1-NN of the DTU evaluation), tnt (crop, voxel
+down-sample, ICP and distances of the Tanks and Temples evaluation), knn (distCUDA2 on clouds of
 1-4097 points, coincident and non-finite rows included), sort (the multi-word sort, key runs and scan at n = 1 and 4097, three
 words), appearance (the weight-gradient kernel of the appearance network, several tiles per CTA).  Sizes are tiny on purpose (the tools slow kernels down 100-1000x).  Exit code 0 = every call returned."""
 import os
@@ -133,6 +134,23 @@ def dtu(dev):
     print("dtu samples", pts.shape[0], "kept", int(kept.sum()), "rounds", rounds, "max dist", float(d.max()), flush=True)
 
 
+def tnt(dev):
+    # the Tanks and Temples evaluation (tnt_eval.cu and the indexed 1-NN of dtu_eval.cu): a transformed crop with a concave
+    # polygon, the voxel down-sample, an ICP run with an empty-target check, and the two distance passes
+    import gof_tnt_eval
+    rng = np.random.default_rng(5)
+    pts = torch.from_numpy(rng.uniform(-1, 1, (3000, 3))).to(dev)
+    vol = gof_tnt_eval.crop_volume("z", -0.5, 0.5, [[-0.8, -0.8, 0], [0.8, -0.8, 0], [0, 0, 0], [0.8, 0.8, 0], [-0.8, 0.8, 0]])
+    T = np.eye(4)
+    T[:3, :3] *= 1.1
+    s = gof_tnt_eval.voxel_down_sample(gof_tnt_eval.crop(pts, vol, T), 0.05)
+    t = gof_tnt_eval.voxel_down_sample(gof_tnt_eval.crop(pts, vol), 0.05)
+    r = gof_tnt_eval.registration_icp(s, t, 0.2, max_iteration=5)
+    d1, d2 = gof_tnt_eval.distances(s, t), gof_tnt_eval.distances(t, s)
+    torch.cuda.synchronize()
+    print("tnt", s.shape[0], t.shape[0], "icp iterations", r["iterations"], "max d", float(d1.max()), float(d2.max()), flush=True)
+
+
 def sort(dev):
     # the sort, run and scan primitives through their test entry points: one item, a chunk and a key, three words (w[0] == ka)
     from test_gpu_sort_primitives import _bind, _words_arg
@@ -172,7 +190,7 @@ def appearance(dev):
 
 
 PARTS = {"render": render, "integrate": integrate, "tetmesh": tetmesh, "loss": loss, "params": params, "filter": filt, "tsdf": tsdf,
-         "knn": knn, "dtu": dtu, "sort": sort, "appearance": appearance}
+         "knn": knn, "dtu": dtu, "tnt": tnt, "sort": sort, "appearance": appearance}
 
 if __name__ == "__main__":
     dev = torch.device("cuda")
