@@ -12,7 +12,12 @@ reference's extract_mesh.py, restated with view sharding over the GPUs of one bo
 * CachedIntegrator  -- the same, with the Gaussian side of every view prepared once and reused by all passes (SURVEY 8(f) rank 3).
 * marching_tetrahedra_sharded / merge_tet_shards -- utils/tetmesh.py's chunk loop (:55-95) spread over ranks (SURVEY 8(e)).
 * extract_level_set -- marching_tetrahedra_with_binary_search (extract_mesh.py:37-120) up to the mesh arrays.
+* get_tetra_points  == GaussianModel.get_tetra_points (scene/gaussian_model.py:433-463), get_frustum_mask == its module-level
+                       get_frustum_mask (:31-72): one CUDA pass (csrc/tetra_points.cu, DESIGN §4.8) in memory linear in the
+                       points, where the reference builds ~40 bytes per (view, point).
 """
+import ctypes
+
 import torch
 import torch.distributed as dist
 
@@ -248,3 +253,68 @@ def extract_level_set(points, points_scale, tets, views, integrate_fn, n_binary_
         _a, colors = evaluate_alpha(verts, views, integrate_fn, return_color=True, group=group)
         tick("evaluate_alpha_colors_s", t0)
     return {"vertices": verts, "faces": faces, "mask": distance <= scale, "colors": colors}
+
+
+# ---- the tetrahedra points and their multi-view frustum mask (csrc/tetra_points.cu) ---------------------------------------
+def _tetra_lib():
+    from diff_gaussian_rasterization import _C
+    lib, v = _C._lib, ctypes.c_void_p
+    lib.gof_tetra_points.restype = ctypes.c_int
+    lib.gof_tetra_points.argtypes = [ctypes.c_int, v, v, v, ctypes.c_int, v, ctypes.c_float, ctypes.c_float, v, v, v, v]
+    lib.gof_frustum_mask.restype = ctypes.c_int
+    lib.gof_frustum_mask.argtypes = [ctypes.c_int64, v, ctypes.c_int, v, ctypes.c_float, ctypes.c_float, v, v]
+    return _C, lib
+
+
+def pack_views(views, device):
+    """[n,20] float32 table of gof_tetra_points / gof_frustum_mask from objects with the reference Camera's attributes
+    (world_view_transform, focal_x, focal_y, image_width, image_height; scene/cameras.py).  The scalars are rounded to float32
+    as the reference's `torch.Tensor([...])` rounds them."""
+    views = list(views)
+    if not views:
+        raise ValueError("at least one view is needed (the reference reads views[0])")
+    wvt = torch.stack([torch.as_tensor(v.world_view_transform).detach().to(device=device, dtype=torch.float32).reshape(16) for v in views])
+    extra = torch.tensor([[v.focal_x, v.focal_y, v.image_width, v.image_height] for v in views], dtype=torch.float32)
+    return torch.cat([wvt, extra.to(device)], dim=1).contiguous()
+
+
+@torch.no_grad()
+def get_tetra_points(xyz, scales_with_filter, rotation, views, near=0.02, far=1e6):
+    """== GaussianModel.get_tetra_points (scene/gaussian_model.py:433-463) with xyz = gaussians.get_xyz,
+    scales_with_filter = gaussians.get_scaling_with_3D_filter and rotation = gaussians._rotation (the raw quaternions;
+    they are normalised here as build_rotation does).  Returns (points [M,3], points_scale [M,1]): the 8 corners of every
+    Gaussian's 3-sigma box, then the centres, kept where some view's frustum holds them.  Width and height come from views[0]
+    for every view, as in the reference."""
+    from gof_params import _f32
+    _C, lib = _tetra_lib()
+    x, s, q = _f32(xyz), _f32(scales_with_filter), _f32(rotation)
+    P = int(x.shape[0])
+    if tuple(x.shape) != (P, 3) or tuple(s.shape) != (P, 3) or tuple(q.shape) != (P, 4):
+        raise ValueError(f"get_tetra_points: expected xyz [P,3], scales [P,3], rotation [P,4]; got {tuple(x.shape)}, "
+                         f"{tuple(s.shape)}, {tuple(q.shape)}")
+    table = pack_views(views, x.device)
+    pts = torch.empty((9 * P, 3), dtype=torch.float32, device=x.device)
+    sc = torch.empty((9 * P, 1), dtype=torch.float32, device=x.device)
+    mask = torch.empty(9 * P, dtype=torch.bool, device=x.device)
+    with torch.cuda.device(x.device):
+        _C._check(lib.gof_tetra_points(P, x.data_ptr(), s.data_ptr(), q.data_ptr(), int(table.shape[0]), table.data_ptr(), float(near),
+                                       float(far), pts.data_ptr(), sc.data_ptr(), mask.data_ptr(), _C._stream()))
+    return pts[mask], sc[mask]
+
+
+@torch.no_grad()
+def get_frustum_mask(points, cameras, near=0.02, far=1e6):
+    """== get_frustum_mask (scene/gaussian_model.py:31-72): bool [N], True where the frustum of some camera holds the point
+    (near <= depth <= far, 0 <= u <= W-1, 0 <= v <= H-1, with W and H of cameras[0])."""
+    from gof_params import _f32
+    _C, lib = _tetra_lib()
+    p = _f32(points)
+    N = int(p.shape[0])
+    if tuple(p.shape) != (N, 3):
+        raise ValueError(f"get_frustum_mask: expected points [N,3], got {tuple(p.shape)}")
+    table = pack_views(cameras, p.device)
+    mask = torch.empty(N, dtype=torch.bool, device=p.device)
+    with torch.cuda.device(p.device):
+        _C._check(lib.gof_frustum_mask(N, p.data_ptr(), int(table.shape[0]), table.data_ptr(), float(near), float(far), mask.data_ptr(),
+                                       _C._stream()))
+    return mask

@@ -323,6 +323,20 @@ GOF_API int gof_activate_params_backward(int P, int M_rest, const float* scaling
  * T, focal_x, focal_y, width, height.  scratch4: 4 device bytes. */
 GOF_API int gof_compute_3d_filter(int P, const float* xyz, int n_cams, const float* cams, float max_focal, float* filter_3D,
                                   void* scratch4, void* stream);
+/* GaussianModel.get_tetra_points (scene/gaussian_model.py:433-463) before its compaction, and get_frustum_mask (:31-72)
+ * (csrc/tetra_points.cu, DESIGN §4.8).  views [n_views,20] float32 = world_view_transform (16, row-major as the reference
+ * stores it), focal_x, focal_y, width, height; width and height are read from views[0] only, for every view, as the
+ * reference does.  near / far are the reference's Python scalars rounded to float32.
+ * gof_tetra_points: xyz, scales (get_scaling_with_3D_filter) [P,3], rotations [P,4] the RAW quaternions (_rotation, 16-byte
+ *   aligned) -> out_points [9P,3] (corner k of Gaussian g at 8g + k, sz fastest in the signs (sx, sy, sz); the centres at
+ *   8P + g), out_scale [9P] (max of 3 * scales, NaN-propagating), out_mask [9P] bytes 0/1 (inside the frustum of a view).
+ * gof_frustum_mask: points [N,3] -> out_mask [N] bytes 0/1.
+ * No allocation, no host synchronisation.  GOF_E_INVALID when P < 0, 9P > 2^32 - 1, N < 0, n_views < 1, or the rotations
+ * are misaligned. */
+GOF_API int gof_tetra_points(int P, const float* xyz, const float* scales, const float* rotations, int n_views, const float* views,
+                             float near, float far, float* out_points, float* out_scale, unsigned char* out_mask, void* stream);
+GOF_API int gof_frustum_mask(int64_t N, const float* points, int n_views, const float* views, float near, float far,
+                             unsigned char* out_mask, void* stream);
 /* GaussianModel.densify_and_prune (scene/gaussian_model.py:631-707) in three steps (csrc/densify.cu; SURVEY.md 8(f) rank 4):
  * plan   -- the four keep-flags of every Gaussian (kept original | clone | split child 1 | split child 2) from the accumulated
  *           statistics and their exclusive scans; flags / offsets [4][P] u32, totals [4] u32 on the device, scan_tmp
