@@ -175,11 +175,12 @@ static int finish_async_read_u32(SideCopy* sc, uint32_t* out) {
   return GOF_OK;
 }
 
-// Preprocess + depth sort + num_rendered, shared by forward and integrate.
+// Preprocess + depth sort + num_rendered, shared by forward and integrate.  box_margin (gof_cull_bbox) is 0 for the
+// forward and 0.5 for integrate, whose corner rays reach half a pixel beyond the centre ray.
 static int preprocess_sort_count(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& GL, int* radii,
-                                 cudaStream_t st, uint32_t* R) {
+                                 float box_margin, cudaStream_t st, uint32_t* R) {
   int rc;
-  if ((rc = gof_launch_preprocess(s, v, geom, GL, radii, st)) != GOF_OK) return rc;
+  if ((rc = gof_launch_preprocess(s, v, geom, GL, radii, box_margin, st)) != GOF_OK) return rc;
   SideCopy* sc = s->debug ? nullptr : begin_async_read_u32(geom + GL.total, st);
   if ((rc = gof_depth_sort(s->P, geom, GL, s->debug != 0, st)) != GOF_OK) return rc;
   if (sc) return finish_async_read_u32(sc, R);
@@ -276,7 +277,7 @@ extern "C" int gof_rasterize_forward(const gof_scene_t* s, gof_alloc_fn geom_all
 
   // rasterizer_impl.cu:334-340: the instance count sizes the binning buffer (read while the depth sort runs)
   uint32_t R = 0;
-  if ((rc = preprocess_sort_count(s, v, geom, GL, radii, st, &R)) != GOF_OK) return rc;
+  if ((rc = preprocess_sort_count(s, v, geom, GL, radii, 0.0f, st, &R)) != GOF_OK) return rc;
   *num_rendered = (int)R;
   tr.mark("pre+sort, num_rendered");
 
@@ -455,7 +456,7 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
   char* img = (char*)image_alloc(image_user, IL.bytes);
   if (!geom || !img) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
   uint32_t R = 0;
-  if ((rc = preprocess_sort_count(s, v, geom, GL, radii, st, &R)) != GOF_OK) return rc;
+  if ((rc = preprocess_sort_count(s, v, geom, GL, radii, 0.5f, st, &R)) != GOF_OK) return rc;
   *num_rendered = (int)R;
   const GofBinLayout BL = gof_bin_layout((size_t)R, s->width, s->height, /*with_masks=*/false);
   char* bin = (char*)binning_alloc(binning_user, BL.bytes);
@@ -521,7 +522,7 @@ extern "C" int gof_integrate_prepare(const gof_scene_t* s, gof_alloc_fn geom_all
     geom = (char*)geom_alloc(geom_user, GL.bytes);
     img = (char*)image_alloc(image_user, IL.bytes);
     if (!geom || !img) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
-    if ((rc = preprocess_sort_count(s, v, geom, GL, radii, st, &R)) != GOF_OK) return rc;
+    if ((rc = preprocess_sort_count(s, v, geom, GL, radii, 0.5f, st, &R)) != GOF_OK) return rc;
   }
   *num_rendered = (int)R;
   const GofIntCacheLayout CL = gof_int_cache_layout((size_t)s->P, s->width, s->height, (size_t)R);

@@ -252,7 +252,7 @@ static inline GofGeomLayout gof_geom_layout(size_t P) {
 
 struct GofImageLayout {     // "imgBuffer": per pixel + per tile
   size_t accum;      // float[4][tiles*256]  tile-major: T, dist1, dist2, raw distortion
-  size_t ncontrib;   // u32  [2][tiles*256]  tile-major: last contributor, median contributor
+  size_t ncontrib;   // u32  [2][tiles*256]  tile-major: last contributor, median contributor (integrate: contributors recorded)
   size_t ranges;     // uint2[tiles]
   size_t bytes;
 };
@@ -338,8 +338,9 @@ static inline GofView gof_make_view(const gof_scene_t* s) {
 }
 
 // preprocess.cu
+// box_margin: see gof_cull_bbox (0 when the records feed the blend kernels, 0.5 when they feed k_integrate)
 int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& L,
-                          int* radii, cudaStream_t st);
+                          int* radii, float box_margin, cudaStream_t st);
 int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const char* geom,
                                    const GofGeomLayout& L, const int* radii, float* dL_dmean2D, float* dL_dopacity,
                                    float* dL_dcolor, float* dL_dv2g, float* dL_dmean3D, float* dL_dsh, float* dL_dscale,

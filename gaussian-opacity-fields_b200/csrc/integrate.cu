@@ -5,7 +5,8 @@
 //    influence any output, SURVEY.md A.6), no second host round-trip for the point count;
 //  * pass 1 (per pixel, five sub-pixel rays, records which Gaussians contribute) keeps the reference's arithmetic --
 //    including the different FMA fusion nvcc gave each of the five unrolled rays -- but only visits Gaussians whose
-//    alpha-support box can touch the warp's pixels (box widened by 2 px for the corner rays);
+//    alpha-support box holds one of the warp's pixels (preprocess builds that box for all five rays, gof_cull_bbox with
+//    margin 0.5);
 //  * pass 2 is POINT-parallel: one thread per query point walks the contributor list of the pixel the point falls in
 //    and gathers the records directly, instead of every pixel thread rescanning all points of the tile and keeping
 //    8 KB of per-thread arrays (forward.cu:879,1015-1017,1104-1105);
@@ -75,7 +76,7 @@ struct IntArgs {
   const float* bg;
   uint16_t* ids;        // [gridDim][256][1024]
   float* final_T;       // tile-major plane 0 of the image state
-  uint32_t* ncontrib;   // tile-major plane 0
+  uint32_t* ncontrib;   // tile-major planes 0 (last contributor) and 1 (contributors recorded, for export_state)
   float* out_color;     // [9][H][W]
   float* out_alpha;     // [PN]
   float* out_color_int; // [PN][3]
@@ -196,8 +197,10 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
         if (k * 32 >= nb) break;
         const int idx = k * 32 + lane;
         const float4 qb = s_rec[idx][3];
-        // corner rays reach half a pixel beyond the warp's block; the box is additionally widened by 1.5 px
-        uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0 - 2, wy0 - 2, wx0 + 9, wy0 + 5));
+        // The box holds every pixel at which one of the five rays can pass the alpha test (the half pixel of the corner
+        // rays is inside it, added before the rounding to integers), so it is tested against the warp's 8x4 pixels as they
+        // are: a Gaussian skipped here would be rejected by all five ray_step calls of all 32 lanes.
+        uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
         while (m) {
           const int j = k * 32 + __ffs(m) - 1;
           m &= m - 1;
@@ -236,6 +239,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
     const size_t slot = (size_t)tile * 256 + threadIdx.x;
     a.final_T[slot] = T0;
     a.ncontrib[slot] = last_contributor;
+    a.ncontrib[(size_t)a.tiles * 256 + slot] = n_local;
     const float col0 = F_FMA(T0, a.bg[0], C0), col1 = F_FMA(T0, a.bg[1], C1), col2 = F_FMA(T0, a.bg[2], C2);
     s_cnt[threadIdx.x] = n_local;
     s_col[threadIdx.x][0] = col0; s_col[threadIdx.x][1] = col1; s_col[threadIdx.x][2] = col2;

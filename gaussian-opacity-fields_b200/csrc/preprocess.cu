@@ -38,6 +38,7 @@ struct PreArgs {
   uint32_t* total;      // sum of tiles_touched = num_rendered (zeroed by the launcher)
   float* reject_k;      // see GofGeomLayout::reject_k
   int cull;             // 1: store the conservative alpha-support box, 0: store the whole plane
+  float box_margin;     // pixels the box reaches beyond the centre rays (gof_cull_bbox): 0 blend, 0.5 opacity-field query
 };
 
 __global__ void __launch_bounds__(256) k_preprocess(const PreArgs a) {
@@ -160,7 +161,8 @@ __global__ void __launch_bounds__(256) k_preprocess(const PreArgs a) {
 #pragma unroll
       for (int k = 0; k < 10; ++k) rec.v2g[k] = a.v2g_precomp[10 * idx + k];
     }
-    const GofBox box = a.cull ? gof_cull_bbox(rec.v2g, rec.opacity, lambda_min, a.W, a.H, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy)
+    const GofBox box = a.cull ? gof_cull_bbox(rec.v2g, rec.opacity, lambda_min, a.W, a.H, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy,
+                                                a.box_margin)
                               : gof_full_box();
     rec.box_lo = ((uint32_t)box.x0 & 0xffffu) | ((uint32_t)box.y0 << 16);
     rec.box_hi = ((uint32_t)box.x1 & 0xffffu) | ((uint32_t)box.y1 << 16);
@@ -597,7 +599,7 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
 }  // namespace
 
 int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& L,
-                          int* radii, cudaStream_t st) {
+                          int* radii, float box_margin, cudaStream_t st) {
   PreArgs a{};
   a.P = s->P; a.D = s->D; a.M = s->M; a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.grid_y = v.grid_y;
   a.tan_fovx = s->tan_fovx; a.tan_fovy = s->tan_fovy; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
@@ -619,9 +621,12 @@ int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, co
   a.reject_k = reinterpret_cast<float*>(geom + L.reject_k);
   GOF_CUDA_OK(cudaMemsetAsync(a.total, 0, 4, st));
   {
-    static int cull = -1;   // GOF_CULL=0 disables the alpha-support boxes (A/B testing; results are identical)
+    // GOF_CULL=0 stores the whole plane instead of the alpha-support boxes (A/B testing).  Results are identical as long as
+    // the box covers every ray its consumer casts: the centre ray for the blend, centre and corner rays for the query.
+    static int cull = -1;
     if (cull < 0) { const char* e = getenv("GOF_CULL"); cull = (e && e[0] == '0') ? 0 : 1; }
     a.cull = cull;
+    a.box_margin = box_margin;
   }
   GOF_LAUNCH("preprocess_fwd", st, k_preprocess<<<(s->P + 255) / 256, 256, 0, st>>>(a));
   GOF_LAUNCH_CHECK(s->debug, st);

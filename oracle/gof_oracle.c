@@ -900,6 +900,15 @@ static int point_project(const float* p, const float* vm, int W, int H, float fo
   return 1;
 }
 
+/* Test helper: point_project for PN points.  ok[i] = 1 when point i projects inside the image; xy / depth are written for
+ * those only. */
+void oracle_project_points(int W, int H, float tan_fovx, float tan_fovy, const float* viewmatrix, int PN, const float* points3D,
+                           float* xy, float* depth, unsigned char* ok) {
+  const float focal_y = H / (2.0f * tan_fovy), focal_x = W / (2.0f * tan_fovx);
+  for (int i = 0; i < PN; ++i)
+    ok[i] = (unsigned char)point_project(points3D + 3 * (size_t)i, viewmatrix, W, H, focal_x, focal_y, xy + 2 * (size_t)i, depth + i);
+}
+
 /* the five rays of forward.cu:919-930 with the reference's per-ray fusion (k = 0: centre, 1..4: corners) */
 static void pair_geom_k(int k, const float* v, float rx, float ry, float* n, float* AA, float* BB) {
   float n0, n1, n2, bh;
@@ -921,13 +930,66 @@ static void pair_geom_k(int k, const float* v, float rx, float ry, float* n, flo
 
 #define MAX_CONTRIB 1024 /* MAX_NUM_CONTRIBUTORS * 4, forward.cu:879,986 */
 
+/* 1 when x lies within `ulps` units in the last place of the threshold: a decision `x < thr` taken here may come out
+ * the other way in an implementation whose expf differs from this host's in the last bits */
+static int near_threshold(float x, float thr, float ulps) { return fabsf(x - thr) <= ulps * 1.1920929e-7f * fabsf(thr); }
+
+/* One ray of pass 1 against one Gaussian, forward.cu:931-958: 1 when the ray passes the near-plane and alpha tests
+ * (the caller applies the transmittance test).  *marginal is set when one of the two decisions is within 8 ulp. */
+static int ray_accepts(int k, const float* v, float opac, float rx, float ry, float* t_out, float* alpha_out, int* marginal) {
+  float nrm[3], AA, BB;
+  pair_geom_k(k, v, rx, ry, nrm, &AA, &BB);
+  const float CC = v[9];
+  const float t = -BB / (2 * AA);
+  if (near_threshold(t, 0.2f, 8.f)) *marginal = 1;
+  if (t <= NEAR_PLANE) return 0;
+  const double min_value = fma((double)(-BB / AA), (double)BB / 4., (double)CC);
+  float power = (float)(-0.5 * min_value);
+  if (power > 0.0f) power = 0.0f;
+  const float alpha = fminf(0.99f, opac * expf(power));
+  if (near_threshold(alpha, 1.0f / 255.0f, 8.f)) *marginal = 1;
+  if (alpha < 1.0f / 255.0f) return 0;
+  *t_out = t; *alpha_out = alpha;
+  return 1;
+}
+
+static const float RAY_OFFX[5] = {0.0f, -0.5f, 0.5f, -0.5f, 0.5f};
+static const float RAY_OFFY[5] = {0.0f, -0.5f, -0.5f, 0.5f, 0.5f};
+
+/* Test helper, the five-ray counterpart of oracle_alpha_map: out[py][px] is a bit mask of the rays of pixel (px, py)
+ * (bit 0 centre, bits 1-4 corners) on which ONE Gaussian passes the near-plane and alpha tests of pass 1.  A pixel
+ * with a non-zero mask is one at which the query can record the Gaussian as a contributor. */
+void oracle_ray_mask_map(int W, int H, float tan_fovx, float tan_fovy, const float* v2g, float opacity, unsigned char* out) {
+  const float focal_y = H / (2.0f * tan_fovy), focal_x = W / (2.0f * tan_fovx);
+  for (int py = 0; py < H; ++py)
+    for (int px = 0; px < W; ++px) {
+      const float pixfx = (float)px + 0.5f, pixfy = (float)py + 0.5f;
+      unsigned char m = 0;
+      for (int k = 0; k < 5; ++k) {
+        const float rx = (float)((pixfx + RAY_OFFX[k] - W / 2.) / focal_x), ry = (float)((pixfy + RAY_OFFY[k] - H / 2.) / focal_y);
+        float t, alpha;
+        int marg = 0;
+        if (ray_accepts(k, v2g, opacity, rx, ry, &t, &alpha, &marg)) m |= (unsigned char)(1u << k);
+      }
+      out[(size_t)py * W + px] = m;
+    }
+}
+
 /* Whole integrate for one view.  Inputs: Gaussian state + tile lists from oracle_preprocess / oracle_bin.
  * out_color [9,H,W] (channels 0-2, 6, 7, 8 written), final_T [H,W], n_contrib [H,W],
- * out_alpha_integrated [PN] (caller-initialised to 1), out_color_integrated [PN,3] (caller-initialised to 0). */
-void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float* viewmatrix, int PN, const float* points3D,
+ * out_alpha_integrated [PN] (caller-initialised to 1), out_color_integrated [PN,3] (caller-initialised to 0).
+ * Optional (NULL to skip): n_recorded [H,W] contributors recorded per pixel (<= 1024); marginal_pix [H,W] and
+ * marginal_pt [PN] (caller-zeroed) are 1 where a decision the result depends on lies so close to its threshold that
+ * an expf differing in the last bits can take it the other way -- alpha against 1/255 and t against 0.2 within 8 ulp,
+ * T' against 1e-4 within twice the relative error a ray's transmittance can have picked up, sum over its blended
+ * Gaussians of (8 alpha / (1 - alpha) + 2) 2^-24 (alpha is within 8 * 2^-24 relative, each product rounds once on
+ * either side) -- as `marginal` of oracle_render_backward; a point inherits the flag of its pixel.  pt_clamp [PN,2] counts, per point, the contributors
+ * of pass 2 whose depth was clamped to the point's depth and those whose depth was not. */
+void oracle_integrate_checked(int W, int H, float tan_fovx, float tan_fovy, const float* viewmatrix, int PN, const float* points3D,
                       const uint32_t* ranges, const uint32_t* point_list, const float* features, const float* view2gaussian,
                       const float* conic_opacity, const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
-                      float* out_alpha_integrated, float* out_color_integrated) {
+                      float* out_alpha_integrated, float* out_color_integrated, uint32_t* n_recorded,
+                      unsigned char* marginal_pix, unsigned char* marginal_pt, uint32_t* pt_clamp) {
   const float focal_y = H / (2.0f * tan_fovy), focal_x = W / (2.0f * tan_fovx);
   const int gx = (W + BLOCK_X - 1) / BLOCK_X;
   const size_t HW = (size_t)H * W;
@@ -951,8 +1013,6 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
   for (int i = 0; i < PN; ++i)
     if (ppix[i] >= 0) order[cur[ppix[i]]++] = (uint32_t)i;
 
-  static const float offx[5] = {0.0f, -0.5f, 0.5f, -0.5f, 0.5f};
-  static const float offy[5] = {0.0f, -0.5f, -0.5f, 0.5f, 0.5f};
 #pragma omp parallel for schedule(dynamic, 4)
   for (int py = 0; py < H; ++py) {
     uint16_t* ids = (uint16_t*)malloc(MAX_CONTRIB * sizeof(uint16_t));
@@ -962,12 +1022,14 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
       const uint32_t* range = ranges + 2 * ((py / BLOCK_Y) * gx + (px / BLOCK_X));
       float rxk[5], ryk[5];
       for (int k = 0; k < 5; ++k) {
-        rxk[k] = (float)((pixfx + offx[k] - W / 2.) / focal_x);
-        ryk[k] = (float)((pixfy + offy[k] - H / 2.) / focal_y);
+        rxk[k] = (float)((pixfx + RAY_OFFX[k] - W / 2.) / focal_x);
+        ryk[k] = (float)((pixfy + RAY_OFFY[k] - H / 2.) / focal_y);
       }
       float Ts[5] = {1, 1, 1, 1, 1};
+      float Terr[5] = {0, 0, 0, 0, 0}; /* relative error bound of Ts[k], for `marginal` only */
       float C[8] = {0};
       uint32_t contributor = 0, last_contributor = 0, n_local = 0;
+      int marg = 0;
       /* pass 1, forward.cu:886-993 */
       for (uint32_t kk = range[0]; kk < range[1]; ++kk) {
         contributor++;
@@ -976,18 +1038,13 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
         const float opac = conic_opacity[4 * (size_t)gid + 3];
         int used = 0;
         for (int k = 0; k < 5; ++k) {
-          float nrm[3], AA, BB;
-          pair_geom_k(k, v, rxk[k], ryk[k], nrm, &AA, &BB);
-          const float CC = v[9];
-          const float t = -BB / (2 * AA);
-          if (t <= NEAR_PLANE) continue;
-          const double min_value = fma((double)(-BB / AA), (double)BB / 4., (double)CC);
-          float power = (float)(-0.5 * min_value);
-          if (power > 0.0f) power = 0.0f;
-          const float alpha = fminf(0.99f, opac * expf(power));
-          if (alpha < 1.0f / 255.0f) continue;
+          float t, alpha;
+          if (!ray_accepts(k, v, opac, rxk[k], ryk[k], &t, &alpha, &marg)) continue;
           const float test_T = Ts[k] * (1 - alpha);
+          const float terr = Terr[k] + (8.f * alpha / (1 - alpha) + 2.f) * 5.9604645e-8f;
+          if (fabsf(test_T - 0.0001f) <= 2.f * terr * 0.0001f) marg = 1;
           if (test_T < 0.0001f) continue;
+          Terr[k] = terr;
           if (k == 0)
             for (int ch = 0; ch < 3; ++ch) C[ch] = fmaf(Ts[0], alpha * features[3 * (size_t)gid + ch], C[ch]);
           if (t > C[6]) C[6] = t;
@@ -1003,6 +1060,8 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
       }
       final_T[pix_id] = Ts[0];
       n_contrib[pix_id] = last_contributor;
+      if (n_recorded) n_recorded[pix_id] = n_local;
+      if (marginal_pix) marginal_pix[pix_id] = (unsigned char)marg;
       float col[3];
       for (int ch = 0; ch < 3; ++ch) { col[ch] = fmaf(Ts[0], bg[ch], C[ch]); out_color[ch * HW + pix_id] = col[ch]; }
       out_color[6 * HW + pix_id] = C[6];
@@ -1015,7 +1074,8 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
         const float ry = (float)(((double)pxy[2 * (size_t)id + 1] - H / 2.) / focal_y);
         const float ray_depth = pdepth[id];
         float point_alpha = 0.f, point_T = 1.f;
-        uint32_t num_iterated = 0, second = 0;
+        uint32_t num_iterated = 0, second = 0, n_clamped = 0, n_free = 0;
+        int pmarg = marg;
         for (uint32_t kk = range[0]; kk < range[1]; ++kk) {
           num_iterated++;
           if (num_iterated > last_contributor) break;
@@ -1025,14 +1085,17 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
           const float* v = view2gaussian + 10 * (size_t)gid;
           const pair_t p = pair_geom(v, rx, ry);
           float t = -p.BB / (2 * p.AA);
-          if (t > ray_depth) t = ray_depth;
+          if (t > ray_depth) { t = ray_depth; n_clamped++; } else n_free++;
           const float power = -0.5f * (v[9] + fmaf(p.BB, t, (p.AA * t) * t));
           const float alpha = fminf(0.99f, conic_opacity[4 * (size_t)gid + 3] * expf(power));
+          if (near_threshold(alpha, 1.0f / 255.0f, 8.f)) pmarg = 1;
           if (alpha < 1.0f / 255.0f) continue;
           point_alpha = fmaf(alpha, point_T, point_alpha);
           point_T = point_T * (1 - alpha);
         }
         out_alpha_integrated[id] = point_alpha;
+        if (marginal_pt) marginal_pt[id] = (unsigned char)pmarg;
+        if (pt_clamp) { pt_clamp[2 * (size_t)id] = n_clamped; pt_clamp[2 * (size_t)id + 1] = n_free; }
         for (int ch = 0; ch < 3; ++ch) out_color_integrated[3 * (size_t)id + ch] = col[ch];
       }
       out_color[8 * HW + pix_id] = (float)(p1 - p0);
@@ -1040,4 +1103,14 @@ void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float*
     free(ids);
   }
   free(pxy); free(pdepth); free(ppix); free(cnt); free(order); free(cur);
+}
+
+/* oracle_integrate_checked without the optional outputs */
+void oracle_integrate(int W, int H, float tan_fovx, float tan_fovy, const float* viewmatrix, int PN, const float* points3D,
+                      const uint32_t* ranges, const uint32_t* point_list, const float* features, const float* view2gaussian,
+                      const float* conic_opacity, const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
+                      float* out_alpha_integrated, float* out_color_integrated) {
+  oracle_integrate_checked(W, H, tan_fovx, tan_fovy, viewmatrix, PN, points3D, ranges, point_list, features, view2gaussian,
+                           conic_opacity, bg, out_color, final_T, n_contrib, out_alpha_integrated, out_color_integrated, NULL, NULL,
+                           NULL, NULL);
 }

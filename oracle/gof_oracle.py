@@ -206,9 +206,29 @@ def alpha_map(W, H, tan_fovx, tan_fovy, v2g, opacity):
     return out
 
 
+def ray_mask_map(W, H, tan_fovx, tan_fovy, v2g, opacity):
+    """[H,W] uint8: bit k set where ray k of the opacity-field query (0 centre, 1-4 corners) accepts the Gaussian."""
+    out = np.zeros((H, W), np.uint8)
+    v = np.ascontiguousarray(v2g, np.float32)
+    _lib.oracle_ray_mask_map(int(W), int(H), ctypes.c_float(tan_fovx), ctypes.c_float(tan_fovy), _p(v), ctypes.c_float(float(opacity)), _p(out))
+    return out
+
+
+def project_points(scene, points3D):
+    """The query's projection of points3D [PN,3]: (xy [PN,2], depth [PN], ok [PN] bool); xy / depth are NaN where the point
+    does not project into the image."""
+    pts = _np(points3D)
+    PN = int(pts.shape[0])
+    xy, depth, ok = np.full((PN, 2), np.nan, np.float32), np.full(PN, np.nan, np.float32), np.zeros(PN, np.uint8)
+    _lib.oracle_project_points(scene.W, scene.H, ctypes.c_float(scene.tan_fovx), ctypes.c_float(scene.tan_fovy),
+                               _p(scene.arr["viewmatrix"]), PN, _p(pts), _p(xy), _p(depth), _p(ok))
+    return xy, depth, ok.astype(bool)
+
+
 def integrate(scene, points3D):
     """Opacity-field query of `points3D` [PN,3] for one view: (out_color[9,H,W], alpha_integrated[PN],
-    color_integrated[PN,3], radii[P], state) -- the 4 tensors GaussianRasterizer.integrate returns, plus state."""
+    color_integrated[PN,3], radii[P], state) -- the 4 tensors GaussianRasterizer.integrate returns, plus state.  The state
+    also holds n_recorded [H,W], marginal_pix [H,W], marginal_pt [PN] and pt_clamp [PN,2] (see oracle_integrate)."""
     g = preprocess(scene)
     R, point_list, ranges = bin_tiles(scene.W, scene.H, g["radii"], g["means2D"], g["depths"], g["tiles_touched"])
     pts = _np(points3D)
@@ -219,12 +239,18 @@ def integrate(scene, points3D):
     n_contrib = np.zeros((H, W), np.uint32)
     alpha_int = np.ones(PN, np.float32)
     color_int = np.zeros((PN, 3), np.float32)
+    n_recorded = np.zeros((H, W), np.uint32)
+    marginal_pix, marginal_pt = np.zeros((H, W), np.uint8), np.zeros(PN, np.uint8)
+    pt_clamp = np.zeros((PN, 2), np.uint32)
     if scene.P and PN:
-        _lib.oracle_integrate(W, H, ctypes.c_float(scene.tan_fovx), ctypes.c_float(scene.tan_fovy), _p(scene.arr["viewmatrix"]),
-                              PN, _p(pts), _p(np.ascontiguousarray(ranges, np.uint32)), _p(np.ascontiguousarray(point_list, np.uint32)),
-                              _p(np.ascontiguousarray(g["rgb"], np.float32)), _p(np.ascontiguousarray(g["view2gaussian"], np.float32)),
-                              _p(np.ascontiguousarray(g["conic_opacity"], np.float32)), _p(scene.arr["background"]), _p(out),
-                              _p(final_T), _p(n_contrib), _p(alpha_int), _p(color_int))
+        _lib.oracle_integrate_checked(W, H, ctypes.c_float(scene.tan_fovx), ctypes.c_float(scene.tan_fovy), _p(scene.arr["viewmatrix"]),
+                                      PN, _p(pts), _p(np.ascontiguousarray(ranges, np.uint32)), _p(np.ascontiguousarray(point_list, np.uint32)),
+                                      _p(np.ascontiguousarray(g["rgb"], np.float32)), _p(np.ascontiguousarray(g["view2gaussian"], np.float32)),
+                                      _p(np.ascontiguousarray(g["conic_opacity"], np.float32)), _p(scene.arr["background"]), _p(out),
+                                      _p(final_T), _p(n_contrib), _p(alpha_int), _p(color_int), _p(n_recorded), _p(marginal_pix),
+                                      _p(marginal_pt), _p(pt_clamp))
     st = dict(g)
-    st.update(num_rendered=R, point_list=point_list, ranges=ranges, final_T=final_T, n_contrib=n_contrib)
+    st.update(num_rendered=R, point_list=point_list, ranges=ranges, final_T=final_T, n_contrib=n_contrib,
+              n_recorded=n_recorded, marginal_pix=marginal_pix.astype(bool), marginal_pt=marginal_pt.astype(bool),
+              pt_clamp=pt_clamp)
     return out, alpha_int, color_int, g["radii"], st

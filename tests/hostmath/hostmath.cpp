@@ -56,16 +56,23 @@ void hm_pair(const float* v2g, unsigned pix_x, unsigned pix_y, int W, int H, flo
   out[4] = gof_mapped_t(out[2]); out[5] = gof_normal_length(p); out[6] = p.n0; out[7] = p.n1; out[8] = p.n2;
 }
 
-// conservative cull box of one Gaussian (gof_cull_bbox); scale may be NULL (then no box: full plane)
-void hm_bbox(const float* v2g, float opacity, const float* scale, int W, int H, float tan_fovx, float tan_fovy, int* out) {
+// conservative cull box of one Gaussian (gof_cull_bbox); scale may be NULL (then no box: full plane); margin_px is 0 for
+// the blend's centre rays and 0.5 for the five rays of the opacity-field query
+void hm_bbox_margin(const float* v2g, float opacity, const float* scale, int W, int H, float tan_fovx, float tan_fovy,
+                    float margin_px, int* out) {
   const float focal_y = H / (2.0f * tan_fovy), focal_x = W / (2.0f * tan_fovx);
   double lam = 0.0;
   if (scale) {
     lam = 1e300;
     for (int k = 0; k < 3; ++k) { const double si = 1.0 / ((double)scale[k] * scale[k] + 1e-7); lam = si < lam ? si : lam; }
   }
-  const GofBox b = gof_cull_bbox(v2g, opacity, lam, W, H, focal_x, focal_y, tan_fovx, tan_fovy);
+  const GofBox b = gof_cull_bbox(v2g, opacity, lam, W, H, focal_x, focal_y, tan_fovx, tan_fovy, margin_px);
   out[0] = b.x0; out[1] = b.y0; out[2] = b.x1; out[3] = b.y1;
+}
+
+// the blend's box (margin 0)
+void hm_bbox(const float* v2g, float opacity, const float* scale, int W, int H, float tan_fovx, float tan_fovy, int* out) {
+  hm_bbox_margin(v2g, opacity, scale, W, H, tan_fovx, tan_fovy, 0.0f, out);
 }
 
 void hm_sh(int deg, const float* mean, const float* campos, const float* sh, float* rgb, unsigned char* clamped) {

@@ -1,6 +1,8 @@
 """GPU: the alpha-support boxes only skip work.  Rendering with GOF_CULL=0 (every staged Gaussian visited by every
 warp, like the reference) and GOF_CULL=1 must give BIT-identical images and per-pixel counters, and gradients that
-differ only by float summation order -- on ordinary, needle-shaped and sub-pixel Gaussians."""
+differ only by float summation order -- on ordinary, needle-shaped and sub-pixel Gaussians.  The same holds bit for bit for the
+opacity-field query (image, per-point alpha and colour, last contributor and contributor count), also on Gaussians thinner
+than a pixel that only its corner rays meet."""
 import os
 import subprocess
 import sys
@@ -28,7 +30,7 @@ def test_culling_never_changes_results():
         a = _run("0", inputs, os.path.join(d, "a.npz"))
         b = _run("1", inputs, os.path.join(d, "b.npz"))
         for k in a.files:
-            if k.endswith(("_color", "_ncontrib", "_accum")):
+            if k.endswith(("_color", "_ncontrib", "_accum", "_int_alpha", "_int_colint")):
                 np.testing.assert_array_equal(a[k].view(np.int32), b[k].view(np.int32), err_msg=k)
             else:
                 den = max(np.abs(a[k]).max(), 1e-30)
@@ -39,3 +41,4 @@ def test_culling_never_changes_results():
                     assert np.quantile(diff, 0.99) < 1e-2, f"{k}: q99 {np.quantile(diff, 0.99)}"
                 else:
                     assert diff.max() < 1e-5, f"{k}: {diff.max()}"
+        assert sum(k.endswith("_int_alpha") for k in a.files) == 4 and (a["n_int_alpha"] < 1).sum() > 1000
