@@ -420,6 +420,8 @@ extern "C" int gof_export_state(int P, int width, int height, int num_rendered, 
                                 cudaMemcpyDeviceToDevice, st));
   if (out->ranges)
     GOF_CUDA_OK(cudaMemcpyAsync(out->ranges, img + IL.ranges, (size_t)grid_x * grid_y * 8, cudaMemcpyDeviceToDevice, st));
+  if (out->blend_masks && num_rendered > 0)
+    GOF_CUDA_OK(cudaMemcpyAsync(out->blend_masks, bin + BL.vmask, BL.vmask_stride * 8 * 4, cudaMemcpyDeviceToDevice, st));
   if (out->accum_alpha || out->n_contrib) {
     dim3 b(16, 16), g((width + 15) / 16, (height + 15) / 16);
     k_export_image<<<g, b, 0, st>>>(width, height, grid_x, (size_t)grid_x * grid_y * 256,

@@ -44,7 +44,7 @@ class _Scene(ctypes.Structure):
 class _StateView(ctypes.Structure):
     _fields_ = [(n, _fp) for n in (
         "depths", "means2D", "conic_opacity", "rgb", "view2gaussian", "clamped", "tiles_touched",
-        "point_list", "ranges", "accum_alpha", "n_contrib")]
+        "point_list", "ranges", "accum_alpha", "n_contrib", "blend_masks")]
 
 
 _lib.gof_last_error.restype = ctypes.c_char_p
@@ -455,8 +455,10 @@ def integrate_points_cached(cache, background, points3D, viewmatrix, tan_fovx, t
     return out_color, alpha_int, color_int
 
 
-def export_state(P, W, H, num_rendered, geomBuffer, binningBuffer, imgBuffer, radii):
-    """Parity-test helper (gof_export_state): this library's scratch buffers in the reference's field layout."""
+def export_state(P, W, H, num_rendered, geomBuffer, binningBuffer, imgBuffer, radii, masks=False):
+    """Parity-test helper (gof_export_state): this library's scratch buffers in the reference's field layout.  masks=True
+    (buffers of a forward only) adds "blend_masks", int32 [8, num_rendered + 32 * tiles]: the masks the forward leaves for the
+    backward, laid out as GofBinLayout::vmask (csrc/gof_common.cuh); opt-in, as they take 32 bytes per rendered pair."""
     dev = radii.device
     tiles = ((W + 15) // 16) * ((H + 15) // 16)
     out = {
@@ -470,6 +472,8 @@ def export_state(P, W, H, num_rendered, geomBuffer, binningBuffer, imgBuffer, ra
         "accum_alpha": torch.zeros(4, H, W, device=dev),
         "n_contrib": torch.zeros(2, H, W, dtype=torch.int32, device=dev),
     }
+    if masks:
+        out["blend_masks"] = torch.zeros(8, num_rendered + 32 * tiles, dtype=torch.int32, device=dev)
     sv = _StateView()
     for k, t in out.items():
         setattr(sv, k, t.data_ptr())

@@ -183,6 +183,10 @@ typedef struct gof_state_view {
   uint32_t* ranges;         /* [tiles,2] ImageState::ranges */
   float* accum_alpha;       /* [4,H,W] ImageState::accum_alpha (T, dist1, dist2, raw distortion) */
   uint32_t* n_contrib;      /* [2,H,W] ImageState::n_contrib (last, median) */
+  uint32_t* blend_masks;    /* [8, R + 32*tiles] a raw copy of the blend masks the forward leaves for the backward; word
+                               layout: GofBinLayout::vmask in csrc/gof_common.cuh.  Only the words of group g of (tile, warp)
+                               with 32 g < the largest n_contrib[0] of the warp's 32 pixels are defined.  No reference
+                               counterpart; binning buffers of gof_integrate carry no masks. */
 } gof_state_view_t;
 
 GOF_API int gof_export_state(int P, int width, int height, int num_rendered,

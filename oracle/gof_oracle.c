@@ -384,14 +384,38 @@ static pair_t pair_geom(const float* v, float rx, float ry) {
   return p;
 }
 
-/* forward.cu:409-612 renderCUDA.  out_color [9,H,W], final_T [4,H,W], n_contrib [2,H,W]. */
-void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const uint32_t* ranges,
-                           const uint32_t* point_list, const float* features, const float* view2gaussian,
-                           const float* conic_opacity, const float* bg, float* out_color, float* final_T,
-                           uint32_t* n_contrib) {
+static int near_threshold(float x, float thr, float ulps);
+
+/* forward.cu:409-612 renderCUDA.  out_color [9,H,W], final_T [4,H,W], n_contrib [2,H,W].
+ * Optional outputs (NULL to skip; they do not change the others):
+ *   marginal_pix [H,W]  1 where a decision of the pixel lies so close to its threshold that an expf differing in the last
+ *                       bits can take it the other way: an alpha within 8 ulp of 1/255; a T' within twice its error bound
+ *                       of 1e-4; a T within twice its error bound of 0.5 at the median test.  t (against 0.2) involves no
+ *                       expf and is computed the same way everywhere, so it raises no flag.
+ *   n_blended [H,W]     the number of pairs the pixel blended.
+ *   blended [H,W,nwords] bit p of word p/32: the pixel blended entry p (0-based) of its tile list (nwords >= the longest
+ *                       list / 32, rounded up; every word of the pixel is written).
+ *   accum_err [4,H,W]   absolute bounds on how far final_T[0..3] (T, dist1, dist2, raw distortion) of any implementation
+ *                       that runs this float sequence with an alpha within 8 u = 8 * 2^-24 relative of this one (expf within
+ *                       3 ulp over both sides, op * exp rounded once on each), and a mapped depth m within 2 u m, can lie
+ *                       from this one, both sides rounding every operation.  Running first-order bounds, in double:
+ *                         T      relative eT:  eT += 8u a / (1 - a) + 4u per blended pair (1 - a and the product each round
+ *                                on both sides);
+ *                         dist1  E1 += (eT + 12u) T a m + 2u |dist1'|     (a, m, a*m, the fma),
+ *                         dist2  E2 += (eT + 16u) T a m^2 + 2u |dist2'|   (m^2 moves by 6u),
+ *                         raw distortion, with e = (1-T) m^2 + dist2 - 2 dist1 m and mag = |(1-T) m^2| + |dist2| + 2|dist1 m|:
+ *                                de = (eT T + u) m^2 + E2 + 2 m E1 + 12u mag   (inputs, then the fma / add roundings),
+ *                                Ed += (eT + 10u) T a |e| + T a de + 2u D',  D' = sum T a |e| so far.
+ *                       The eT of the marginal tests above is this one. */
+void oracle_render_forward_checked(int W, int H, float tan_fovx, float tan_fovy, const uint32_t* ranges,
+                                   const uint32_t* point_list, const float* features, const float* view2gaussian,
+                                   const float* conic_opacity, const float* bg, float* out_color, float* final_T,
+                                   uint32_t* n_contrib, unsigned char* marginal_pix, uint32_t* n_blended, uint32_t* blended,
+                                   int nwords, double* accum_err) {
   const float focal_y = H / (2.0f * tan_fovy), focal_x = W / (2.0f * tan_fovx);
   const int gx = (W + BLOCK_X - 1) / BLOCK_X;
   const size_t HW = (size_t)H * W;
+  const double u = 5.9604644775390625e-8; /* 2^-24 */
 #pragma omp parallel for schedule(dynamic, 8)
   for (int py = 0; py < H; ++py) {
     for (int px = 0; px < W; ++px) {
@@ -403,6 +427,11 @@ void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const u
       uint32_t contributor = 0, last_contributor = 0, max_contributor = (uint32_t)-1;
       float C[8] = {0};
       float dist1 = 0, dist2 = 0, distortion = 0;
+      uint32_t* bits = blended ? blended + pix_id * (size_t)nwords : NULL;
+      if (bits) memset(bits, 0, (size_t)nwords * sizeof(uint32_t));
+      uint32_t nb = 0;
+      int marg = 0;
+      double eT = 0, E1 = 0, E2 = 0, Ed = 0, Dabs = 0;
       for (uint32_t k = range[0]; k < range[1]; ++k) {
         contributor++;
         const uint32_t gid = point_list[k];
@@ -417,8 +446,11 @@ void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const u
         float power = (float)(-0.5 * min_value);
         if (power > 0.0f) power = 0.0f;
         const float alpha = fminf(0.99f, opac * expf(power));
+        if (near_threshold(alpha, 1.0f / 255.0f, 8.f)) marg = 1;
         if (alpha < 1.0f / 255.0f) continue;
         const float test_T = T * (1 - alpha);
+        const double eT1 = eT + 8 * u * alpha / (1 - alpha) + 4 * u;
+        if (fabs((double)test_T - 0.0001) <= 2 * eT1 * 0.0001) marg = 1;
         if (test_T < 0.0001f) break; /* done = true */
         const float max_t = t;
         const float mapped_max_t = (float)((FAR_PLANE * max_t - FAR_PLANE * NEAR_PLANE) / ((FAR_PLANE - NEAR_PLANE) * max_t));
@@ -428,15 +460,30 @@ void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const u
         /* forward.cu:552-565 in the fused form of the reference's SASS (fma accumulation onto T) */
         const float m2 = mapped_max_t * mapped_max_t;
         const float error = fmaf(-dist1, mapped_max_t + mapped_max_t, fmaf(A, m2, dist2));
+        if (accum_err) {
+          const double m = mapped_max_t, mm = m2, Ta = (double)T * alpha;
+          const double mag = fabs((double)A * mm) + fabs((double)dist2) + 2 * fabs((double)dist1 * m);
+          const double de = (eT * T + u) * mm + E2 + 2 * fabs(m) * E1 + 12 * u * mag;
+          Dabs += Ta * fabs((double)error);
+          Ed += (eT + 10 * u) * Ta * fabs((double)error) + Ta * de + 2 * u * Dabs;
+        }
         distortion = fmaf(T, error * alpha, distortion);
         dist1 = fmaf(T, alpha * mapped_max_t, dist1);
         dist2 = fmaf(T, m2 * alpha, dist2);
+        if (accum_err) {
+          E1 += (eT + 12 * u) * (double)T * alpha * fabs((double)mapped_max_t) + 2 * u * fabs((double)dist1);
+          E2 += (eT + 16 * u) * (double)T * alpha * m2 + 2 * u * fabs((double)dist2);
+        }
         for (int ch = 0; ch < 3; ++ch) C[ch] = fmaf(T, alpha * features[3 * (size_t)gid + ch], C[ch]);
         for (int ch = 0; ch < 3; ++ch) C[3 + ch] = fmaf(T, alpha * nn[ch], C[3 + ch]);
+        if (fabs((double)T - 0.5) <= 2 * eT * T) marg = 1;
         if (T > 0.5) { C[6] = t; max_contributor = contributor; }
         C[7] = fmaf(T, alpha, C[7]);
         T = test_T;
+        eT = eT1;
         last_contributor = contributor;
+        nb++;
+        if (bits) bits[(k - range[0]) >> 5] |= 1u << ((k - range[0]) & 31);
       }
       const float dbn = distortion;
       distortion = (float)(distortion / ((double)((1 - T) * (1 - T)) + 1e-7));
@@ -447,8 +494,22 @@ void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const u
       out_color[6 * HW + pix_id] = C[6];
       out_color[7 * HW + pix_id] = C[7];
       out_color[8 * HW + pix_id] = distortion;
+      if (marginal_pix) marginal_pix[pix_id] = (unsigned char)marg;
+      if (n_blended) n_blended[pix_id] = nb;
+      if (accum_err) {
+        accum_err[pix_id] = eT * T; accum_err[pix_id + HW] = E1; accum_err[pix_id + 2 * HW] = E2; accum_err[pix_id + 3 * HW] = Ed;
+      }
     }
   }
+}
+
+/* oracle_render_forward_checked without the optional outputs */
+void oracle_render_forward(int W, int H, float tan_fovx, float tan_fovy, const uint32_t* ranges,
+                           const uint32_t* point_list, const float* features, const float* view2gaussian,
+                           const float* conic_opacity, const float* bg, float* out_color, float* final_T,
+                           uint32_t* n_contrib) {
+  oracle_render_forward_checked(W, H, tan_fovx, tan_fovy, ranges, point_list, features, view2gaussian, conic_opacity, bg,
+                                out_color, final_T, n_contrib, NULL, NULL, NULL, 0, NULL);
 }
 
 /* |x - ref| within n float ulp of ref */

@@ -127,17 +127,28 @@ def bin_tiles(W, H, radii, means2D, depths, tiles_touched):
     return R, point_list[:R], ranges
 
 
-def render_forward(scene, g, point_list, ranges):
+def render_forward(scene, g, point_list, ranges, checked=False):
+    """Blend forward: (out_color [9,H,W], final_T [4,H,W], n_contrib [2,H,W]).  checked=True appends a dict of the optional
+    outputs of oracle_render_forward_checked: marginal_pix [H,W] bool, n_blended [H,W], blended [H,W,nwords] u32 (bit p:
+    entry p of the pixel's tile list was blended) and accum_err [4,H,W] float64; the three arrays above are the same."""
     W, H = scene.W, scene.H
     out = np.zeros((9, H, W), np.float32)
     final_T = np.zeros((4, H, W), np.float32)
     n_contrib = np.zeros((2, H, W), np.uint32)
-    _lib.oracle_render_forward(W, H, ctypes.c_float(scene.tan_fovx), ctypes.c_float(scene.tan_fovy),
-                               _p(np.ascontiguousarray(ranges, np.uint32)), _p(np.ascontiguousarray(point_list, np.uint32)),
-                               _p(np.ascontiguousarray(g["rgb"], np.float32)), _p(np.ascontiguousarray(g["view2gaussian"], np.float32)),
-                               _p(np.ascontiguousarray(g["conic_opacity"], np.float32)), _p(scene.arr["background"]),
-                               _p(out), _p(final_T), _p(n_contrib))
-    return out, final_T, n_contrib
+    args = (W, H, ctypes.c_float(scene.tan_fovx), ctypes.c_float(scene.tan_fovy),
+            _p(np.ascontiguousarray(ranges, np.uint32)), _p(np.ascontiguousarray(point_list, np.uint32)),
+            _p(np.ascontiguousarray(g["rgb"], np.float32)), _p(np.ascontiguousarray(g["view2gaussian"], np.float32)),
+            _p(np.ascontiguousarray(g["conic_opacity"], np.float32)), _p(scene.arr["background"]), _p(out), _p(final_T), _p(n_contrib))
+    if not checked:
+        _lib.oracle_render_forward(*args)
+        return out, final_T, n_contrib
+    r = np.asarray(ranges, np.int64).reshape(-1, 2)
+    nwords = max(1, int(((r[:, 1] - r[:, 0]).max(initial=0) + 31) // 32))
+    ex = dict(marginal_pix=np.zeros((H, W), np.uint8), n_blended=np.zeros((H, W), np.uint32),
+              blended=np.zeros((H, W, nwords), np.uint32), accum_err=np.zeros((4, H, W), np.float64))
+    _lib.oracle_render_forward_checked(*args, _p(ex["marginal_pix"]), _p(ex["n_blended"]), _p(ex["blended"]), nwords, _p(ex["accum_err"]))
+    ex["marginal_pix"] = ex["marginal_pix"].astype(bool)
+    return out, final_T, n_contrib, ex
 
 
 BOUND_COMPONENTS = 17   # columns of `mag` / `marginal`: dL_dcolors 0-2 | dL_dmean2D 3-5 | dL_dopacity 6 | dL_dv2g 7-16
@@ -174,13 +185,17 @@ def preprocess_backward(scene, radii, clamped, dL_dcolor, dL_dv2g):
     return d
 
 
-def forward(scene):
-    """Full forward: (out_color, radii, state dict with every intermediate)."""
+def forward(scene, checked=False):
+    """Full forward: (out_color, radii, state dict with every intermediate).  checked=True adds the optional outputs of
+    render_forward(checked=True) to the state."""
     g = preprocess(scene)
     R, point_list, ranges = bin_tiles(scene.W, scene.H, g["radii"], g["means2D"], g["depths"], g["tiles_touched"])
-    out, final_T, n_contrib = render_forward(scene, g, point_list, ranges)
+    res = render_forward(scene, g, point_list, ranges, checked=checked)
+    out, final_T, n_contrib = res[:3]
     st = dict(g)
     st.update(num_rendered=R, point_list=point_list, ranges=ranges, accum_alpha=final_T, n_contrib=n_contrib)
+    if checked:
+        st.update(res[3])
     return out, g["radii"], st
 
 

@@ -16,6 +16,12 @@ KEYS = ("means3D", "scales", "rotations", "opacities", "shs")
 NEEDLES = "n"   # _integrate_scenes.needle_scene: Gaussians that only the corner rays of the opacity-field query meet
 
 
+def _built_scenes():
+    """Scenes of the forward's edge tests: pixels saturating at batch and group boundaries, and alphas on and just above
+    1/255 (the pre-reject's margin)."""
+    return [("s", *_integrate_scenes.saturation_scene()), ("t", *_integrate_scenes.threshold_scene())]
+
+
 def make_inputs(path):
     out = {}
     for tag, cfg, view, sigma, aniso, radius in CASES:
@@ -29,6 +35,9 @@ def make_inputs(path):
     cam, gs = _integrate_scenes.needle_scene()
     for k in KEYS:
         out[f"{NEEDLES}_{k}"] = gs[k].numpy()
+    for tag, cam, gs in _built_scenes():
+        for k in KEYS:
+            out[f"{tag}_{k}"] = gs[k].numpy()
     np.savez(path, **out)
 
 
@@ -38,10 +47,12 @@ def main(in_path, out_path):
     res = {}
     views = [(tag, gof_synth.make_camera(cfg["width"], cfg["height"], view=view, radius=radius), cfg["P"]) for tag, cfg, view, _, _, radius in CASES]
     views.append((NEEDLES, _integrate_scenes.needle_scene()[0], _integrate_scenes.NEEDLE_CASE["P"]))
+    views += [(tag, cam, int(gs["means3D"].shape[0])) for tag, cam, gs in _built_scenes()]
+    degree = {tag: gs["sh_degree"] for tag, _, gs in _built_scenes()}
     for tag, cam, P in views:
         cfg = dict(P=P, width=cam.image_width, height=cam.image_height)
         gs = {k: torch.from_numpy(inp[f"{tag}_{k}"]) for k in KEYS}
-        gs["sh_degree"] = 3
+        gs["sh_degree"] = degree.get(tag, 3)
         fa = _util.fwd_args(cam, gs, dev)
         # the opacity-field query of points around every Gaussian: its boxes must cover the corner rays as well
         g = torch.Generator().manual_seed(7)

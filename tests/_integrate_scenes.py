@@ -130,6 +130,53 @@ def u16_scene():
     return cam, gs, pts, dict(first_wrapped=(10, 10), wrapped_after=(3, 3), id_zero=(21, 5))
 
 
+def tile_stack(cam, tx, ty, n, seed, opacity=(0.005, 0.015), sigma=0.5, depth=(2.0, 6.0), spread=2.5, at=(8.0, 8.0)):
+    """n Gaussians whose tile rectangle is tile (tx, ty) alone: centres within `spread` px of the tile position `at`,
+    `sigma` px wide (the rectangle reaches radius ~ 3 sigma px beyond the centre)."""
+    rng = np.random.default_rng(seed)
+    xy = np.stack([16 * tx + at[0] + rng.uniform(-spread, spread, n), 16 * ty + at[1] + rng.uniform(-spread, spread, n)], 1)
+    return blobs(cam, xy, rng.uniform(*depth, n), sigma, rng.uniform(*opacity, n), seed=seed)
+
+
+SAT_AT = [3, 32, 33, 256, 257]
+
+
+def saturation_scene():
+    """One row of tiles; tile k saturates its centre pixel at list position SAT_AT[k]: faint fillers in a tile corner, then
+    opaque layers on the centre, then more fillers; the centre pixel's last contributor is the entry before."""
+    cam = gof_synth.make_camera(16 * len(SAT_AT), 16, view=6)
+    parts = []
+    for t, s in enumerate(SAT_AT):
+        if s > 3:
+            parts.append(tile_stack(cam, t, 0, s - 3, seed=200 + t, depth=(1.5, 2.0), spread=1.0, at=(4.5, 4.5)))
+        layers = blobs(cam, np.tile([[16 * t + 8.5, 8.5]], (5, 1)), 2.5 + 0.05 * np.arange(5), 2.0, 0.97, seed=210 + t)
+        parts += [layers, tile_stack(cam, t, 0, 60, seed=220 + t, depth=(3.0, 4.0), spread=1.0, at=(11.5, 11.5))]
+    return cam, concat(parts)
+
+
+def threshold_scene():
+    """96x64 pixels under opacities on and around the blend's alpha thresholds: in 1/255 (1 + [1e-5, 2e-3]) (the window the
+    pre-reject's 2e-3 margin must keep), exactly float(1/255) and a few ulp either side of it, in [0.00392, 1/255), 0, and
+    0.99, 0.995 and 1.0 (the clamp); over wide faint Gaussians, a thin ring of each of which lies in that window, and under
+    which no pixel saturates."""
+    cam = gof_synth.make_camera(96, 64, view=12)
+    rng = np.random.default_rng(13)
+    xy = lambda n: np.stack([rng.uniform(-4, 100, n), rng.uniform(-4, 68, n)], 1)   # noqa: E731
+    a = np.float64(np.float32(1.0 / 255.0))
+    ulps = np.nextafter(np.float32(a), np.float32(1)) - np.float32(a)
+    groups = [
+        (300, a * (1 + rng.uniform(1e-5, 2e-3, 300)), rng.uniform(2.0, 8.0, 300)),
+        # the stored opacity is op * coef, coef = sqrt(det0 / (det1 + 1e-6) + 1e-6) a few 1e-7 above 1: a spread of ulps below
+        (200, a + ulps * rng.integers(-16, 2, 200), rng.uniform(1.0, 6.0, 200)),
+        (30, rng.uniform(0.00392, a, 30), rng.uniform(1.0, 6.0, 30)),
+        (30, np.zeros(30), rng.uniform(1.0, 6.0, 30)),
+        (90, np.repeat([0.99, 0.995, 1.0], 30), rng.uniform(0.5, 2.0, 90)),
+        (300, rng.uniform(0.01, 0.05, 300), rng.uniform(12.0, 25.0, 300)),
+    ]
+    parts = [blobs(cam, xy(n), rng.uniform(2.0, 6.0, n), s, np.asarray(op, np.float32), seed=40 + i) for i, (n, op, s) in enumerate(groups)]
+    return cam, concat(parts)
+
+
 def _quat(R):
     """(w, x, y, z) of a proper rotation matrix."""
     w = math.sqrt(max(0.0, 1.0 + R[0, 0] + R[1, 1] + R[2, 2])) / 2.0

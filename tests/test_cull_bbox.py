@@ -42,19 +42,29 @@ CASES = [
 ]
 
 
-@pytest.mark.parametrize("case", CASES, ids=[f"case{i}" for i in range(len(CASES))])
+@pytest.mark.parametrize("case", CASES + ["needles", "placed", "thresholds"],
+                         ids=[f"case{i}" for i in range(len(CASES))] + ["needles", "placed", "thresholds"])
 def test_box_contains_every_accepted_pixel(hm, case):
-    cam = gof_synth.make_camera(case["W"], case["H"], view=case["seed"] * 7, radius=case["radius"])
-    gs = gof_synth.make_gaussians(case["P"], case["seed"], cam.focal_x, sigma_px=case["sigma_px"])
-    lo, hi = case["aniso"]
-    g = torch.Generator().manual_seed(case["seed"] + 99)
-    an = torch.exp(torch.rand(case["P"], 3, generator=g) * np.log(hi / lo) + np.log(lo))
-    gs["scales"] = (gs["scales"].max(dim=1, keepdim=True).values * an).contiguous()
+    """The blend's box (margin 0, centre rays), also for sub-pixel needles, Gaussians centred on pixel corners, edges and
+    borders, and opacities on and around 1/255 (_integrate_scenes.threshold_scene)."""
+    if case == "needles":
+        cam, gs = scenes.needle_scene()
+    elif case == "placed":
+        cam, gs = _placed_scene()
+    elif case == "thresholds":
+        cam, gs = scenes.threshold_scene()
+    else:
+        cam = gof_synth.make_camera(case["W"], case["H"], view=case["seed"] * 7, radius=case["radius"])
+        gs = gof_synth.make_gaussians(case["P"], case["seed"], cam.focal_x, sigma_px=case["sigma_px"])
+        lo, hi = case["aniso"]
+        g = torch.Generator().manual_seed(case["seed"] + 99)
+        an = torch.exp(torch.rand(case["P"], 3, generator=g) * np.log(hi / lo) + np.log(lo))
+        gs["scales"] = (gs["scales"].max(dim=1, keepdim=True).values * an).contiguous()
     sc = gof_oracle.scene_from_synth(cam, gs)
     st = gof_oracle.preprocess(sc)
     vis = np.nonzero(st["radii"] > 0)[0]
     assert len(vis) > 50
-    W, H = case["W"], case["H"]
+    W, H = sc.W, sc.H
     tight = nonempty = 0
     box = np.zeros(4, np.int32)
     for gid in vis:
@@ -72,7 +82,7 @@ def test_box_contains_every_accepted_pixel(hm, case):
         if box[0] > -30000:
             tight += 1
     assert nonempty > 20
-    if case["radius"] >= 4.0:
+    if isinstance(case, str) or case["radius"] >= 4.0:
         assert tight > 0.5 * nonempty, "the box should be finite for most Gaussians in front of the camera"
 
 

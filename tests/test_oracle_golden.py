@@ -47,6 +47,47 @@ def test_forward_matches_reference(path):
         assert _golden.relerr(st["accum_alpha"][k], fx["accum_alpha"][k])[0] < 1e-5
 
 
+def _bits_popcount(b):
+    return np.unpackbits(np.ascontiguousarray(b).view(np.uint8), axis=-1).sum(-1, dtype=np.int64)
+
+
+def _highest_bit_plus_one(b):
+    """[..., nwords] u32 bitsets -> 1 + the index of the highest set bit, 0 where none is set."""
+    bits = np.unpackbits(np.ascontiguousarray(b).view(np.uint8), axis=-1, bitorder="little")
+    has = bits.any(-1)
+    return np.where(has, bits.shape[-1] - np.argmax(bits[..., ::-1], axis=-1), 0)
+
+
+@pytest.mark.parametrize("path", FIX, ids=[p.split("/")[-1] for p in FIX])
+def test_checked_forward_is_the_plain_forward(path):
+    """oracle_render_forward_checked computes the plain oracle's outputs bit for bit; its blend bitset agrees with its own
+    counters; and its accumulator error bounds hold against the reference extension's outputs (CUDA expf, a double mapped depth)
+    at every pixel it does not flag marginal."""
+    fx = _golden.load(path)
+    sc = _golden.oracle_scene(fx)
+    out, radii, st = gof_oracle.forward(sc)
+    cout, cradii, cst = gof_oracle.forward(sc, checked=True)
+    np.testing.assert_array_equal(cout.view(np.int32), out.view(np.int32))
+    np.testing.assert_array_equal(cst["accum_alpha"].view(np.int32), st["accum_alpha"].view(np.int32))
+    np.testing.assert_array_equal(cst["n_contrib"], st["n_contrib"])
+    bits, last, med = cst["blended"], cst["n_contrib"][0], cst["n_contrib"][1]
+    assert bits.shape[-1] * 32 >= int((st["ranges"][:, 1] - st["ranges"][:, 0]).max())
+    np.testing.assert_array_equal(_bits_popcount(bits), cst["n_blended"])
+    np.testing.assert_array_equal(_highest_bit_plus_one(bits), last)
+    has = med != 0xFFFFFFFF
+    ys, xs = np.nonzero(has)
+    p = med[has].astype(np.int64) - 1
+    assert ((bits[ys, xs, p >> 5] >> (p & 31).astype(np.uint32)) & 1).all(), "the median contributor is not in the bitset"
+    assert (cst["n_blended"] > 0).mean() > 0.5 and cst["n_blended"].max() > 8
+    good = ~cst["marginal_pix"]
+    assert good.mean() > 0.99
+    np.testing.assert_array_equal(last[good], fx["n_contrib"][0].view(np.uint32)[good])
+    np.testing.assert_array_equal(med[good], fx["n_contrib"][1].view(np.uint32)[good])
+    for k in range(4):
+        d = np.abs(fx["accum_alpha"][k].astype(np.float64) - cst["accum_alpha"][k])
+        assert (d[good] <= cst["accum_err"][k][good]).all(), f"accum_alpha[{k}]: {float((d / cst['accum_err'][k])[good].max())} x the bound"
+
+
 @pytest.mark.parametrize("path", FIX, ids=[p.split("/")[-1] for p in FIX])
 def test_backward_matches_reference(path):
     fx = _golden.load(path)

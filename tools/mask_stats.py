@@ -19,23 +19,6 @@ import gof_synth  # noqa: E402
 from diff_gaussian_rasterization import _C as ours  # noqa: E402
 
 
-def align(o, a=256):
-    return (o + a - 1) // a * a
-
-
-def bin_layout(R, tiles):
-    """gof_bin_layout (csrc/gof_common.cuh) for u16 keys"""
-    nb = (R + 4095) // 4096
-    o = 0
-    offs = {}
-    for name, nbytes in (("key_a", R * 2), ("key_b", R * 2), ("val_a", R * 4), ("val_b", R * 4), ("hist", 4352 + 4 * (nb + 1) * 1024)):
-        offs[name] = o
-        o = align(o + nbytes)
-    offs["vmask"] = o
-    offs["vstride"] = R + 32 * tiles
-    return offs
-
-
 def popc(x):
     x = x.to(torch.int64) & 0xFFFFFFFF
     x = x - ((x >> 1) & 0x55555555)
@@ -53,10 +36,9 @@ def main():
     P, W, H = gs["means3D"].shape[0], cam.image_width, cam.image_height
     R, color, radii, geom, binning, img = ours.rasterize_gaussians(*fa)
     torch.cuda.synchronize()
-    st = ours.export_state(P, W, H, R, geom, binning, img, radii)
+    st = ours.export_state(P, W, H, R, geom, binning, img, radii, masks=True)
     gx, gy = (W + 15) // 16, (H + 15) // 16
     tiles = gx * gy
-    L = bin_layout(R, tiles)
     ranges = st["ranges"].to(torch.int64)                       # [tiles,2]
     lens = ranges[:, 1] - ranges[:, 0]
     ngroups = (lens + 31) // 32
@@ -65,7 +47,7 @@ def main():
     first_group = torch.cumsum(ngroups, 0) - ngroups
     g_in_tile = torch.arange(G, device=dev) - first_group[tile_of_group]
     gstart = ranges[tile_of_group, 0] + 32 * tile_of_group + 32 * g_in_tile      # word offset of lane 0
-    vm = binning[L["vmask"]:L["vmask"] + 8 * L["vstride"] * 4].view(torch.int32).view(8, L["vstride"])
+    vm = st["blend_masks"]                                                       # [8, R + 32*tiles]
     idx = gstart[:, None] + torch.arange(32, device=dev)[None, :]                # [G,32]
     words = vm[:, idx]                                                          # [8,G,32]
     # validity: group g of (tile, warp) was written iff 32*g < warp_last (max last_contributor of the warp's 32 pixels)
