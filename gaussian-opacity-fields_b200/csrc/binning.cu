@@ -287,12 +287,6 @@ int onesweep_passes(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, size_t n, co
   return GOF_OK;
 }
 
-int sm_count() {
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
-  return sms;
-}
-
 // complete sort of n (key, value) pairs on the low nbits of the key: memset of the scratch, digit histograms, passes
 template <typename KeyT>
 int sort_pairs(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, uint32_t* scratch, size_t n, int nbits, bool debug, cudaStream_t st,
@@ -305,7 +299,7 @@ int sort_pairs(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, uint32_t* scratch
   const SortScratch sc = carve_sort_scratch(scratch, n);
   GOF_CUDA_OK(cudaMemsetAsync(scratch, 0, GOF_SORT_HEAD_BYTES + (size_t)dg.passes * sc.pass_words * 4, st));
   const size_t want = (n + (size_t)THREADS * 8 - 1) / ((size_t)THREADS * 8);
-  const unsigned grid = (unsigned)(want < (size_t)sm_count() * 4 ? want : (size_t)sm_count() * 4);
+  const unsigned grid = (unsigned)(want < (size_t)gof_sm_count() * 4 ? want : (size_t)gof_sm_count() * 4);
   GOF_LAUNCH("radix_hist", st, k_digit_hist<KeyT><<<grid, THREADS, 0, st>>>(ka, n, dg, sc.ghist));
   GOF_LAUNCH_CHECK(debug, st);
   const int rc = onesweep_passes<KeyT>(ka, kb, va, vb, n, dg, sc, debug, st);

@@ -181,17 +181,15 @@ int launch_v(const float* x, const float* gy, int H, int W, float* dW, float* db
   constexpr int THREADS = (CO / COPT) * CI * RG;
   constexpr int SMEM = 4 * TileLayout<CO, CI, PIPE>::FLOATS * (PIPE ? 2 : 1);
   const int tiles_x = (W + TW - 1) / TW, tiles_y = (H + TH - 1) / TH, tiles = tiles_x * tiles_y;
-  static int sms = 0, per_sm = 0;   // resident CTAs per SM of this instantiation: the persistent grid is exactly one wave
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
+  int per_sm = 1;   // resident CTAs per SM of this instantiation: the persistent grid is exactly one wave
+  const int rc = gof_device_once((const void*)k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE>, [](int, int* v) -> int {
     GOF_CUDA_OK(cudaFuncSetAttribute(k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE>, THREADS, SMEM) != cudaSuccess || per_sm < 1)
-      per_sm = 1;
-  }
-  const int grid = tiles < sms * per_sm ? tiles : sms * per_sm;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(v, k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE>, THREADS, SMEM) != cudaSuccess || *v < 1)
+      *v = 1;
+    return GOF_OK;
+  }, &per_sm);
+  if (rc != GOF_OK) return rc;
+  const int grid = tiles < gof_sm_count() * per_sm ? tiles : gof_sm_count() * per_sm;
   GOF_LAUNCH("conv3x3_wgrad", st, (k_conv3x3_wgrad<CO, CI, COPT, RG, PIPE><<<grid, THREADS, SMEM, st>>>(x, gy, H, W, tiles_x, tiles, dW, db)));
   GOF_LAUNCH_CHECK(false, st);
   return GOF_OK;

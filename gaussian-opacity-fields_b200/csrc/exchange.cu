@@ -194,10 +194,8 @@ extern "C" GOF_API int gof_p2p_allreduce_sum_f32(float* const* peers, int world,
 }
 
 static unsigned exchange_grid(size_t items) {
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
   const size_t want = (items + 511) / 512;
-  return (unsigned)(want < (size_t)sms * 4 ? want : (size_t)sms * 4);
+  return (unsigned)(want < (size_t)gof_sm_count() * 4 ? want : (size_t)gof_sm_count() * 4);
 }
 
 // mc: multicast address of the bucket (valid in THIS process); n floats, the first n_sum summed, the rest max-reduced as

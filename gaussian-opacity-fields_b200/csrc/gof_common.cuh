@@ -53,7 +53,14 @@ void gof_prof_end(cudaStream_t st);
 void* gof_pinned_slot();   // 64 bytes
 int gof_read_back(void* dst, const void* src_dev, size_t bytes, cudaStream_t st);   // copy + stream sync; GOF_OK / GOF_E_CUDA
 
-// GOF_STATS=1: device counters of the backward blend (pairs visited / evaluated / contributing); nullptr otherwise
+// ---- per-device launch state (api.cu; safe to call from several host threads) ----------------------------------------
+// SM count of the current device (132 if the query fails).
+int gof_sm_count();
+// Runs setup(device, &value) once per (current device, key) -- e.g. key = a kernel whose function attributes it sets -- and
+// returns the value it left in *value (may be NULL).  A setup that does not return GOF_OK runs again on the next call.
+// setup runs under the state's mutex and must not call these functions itself.
+int gof_device_once(const void* key, int (*setup)(int dev, int* value), int* value);
+// GOF_STATS=1: the current device's counters of the backward blend (pairs visited / evaluated / contributing); nullptr otherwise
 unsigned long long* gof_stats_buffer();
 
 // ---- shared-memory access with an explicit base register ----------------------------------------------

@@ -331,13 +331,13 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
 
 template <bool STATS>
 int launch_backward(const BwdArgs& a, int tiles, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
+  const int rc = gof_device_once((const void*)k_render_backward<STATS>, [](int, int*) -> int {
     const int need = (STATS ? 3 : 4) * (SMEM_BYTES + 1024);   // only what the resident CTAs need: the rest stays L1
     GOF_CUDA_OK(cudaFuncSetAttribute(k_render_backward<STATS>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                      (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
-    attr_set = true;
-  }
+    return GOF_OK;
+  }, nullptr);
+  if (rc != GOF_OK) return rc;
   GOF_LAUNCH("render_bwd", st, k_render_backward<STATS><<<tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
   return GOF_OK;
 }

@@ -245,13 +245,15 @@ int gof_launch_render_forward(const gof_scene_t* s, const GofView& v, const char
   a.plane = (size_t)v.tiles * 256;
   a.vmask = reinterpret_cast<uint32_t*>(bin + BL.vmask);
   a.vstride = BL.vmask_stride;
-  static bool attr_set = false;   // 4 CTAs x (40 KB + 1 KB) per SM: ask for just that much shared memory -- the rest
-  if (!attr_set) {                // stays L1 (local-memory spills and the mask / output traffic go through it)
+  // 4 CTAs x (40 KB + 1 KB) per SM: ask for just that much shared memory -- the rest stays L1 (local-memory spills and the
+  // mask / output traffic go through it)
+  const int rc = gof_device_once((const void*)k_render_forward, [](int, int*) -> int {
     const int need = 4 * (2 * BATCH * 80 + 1024 + 64);
     GOF_CUDA_OK(cudaFuncSetAttribute(k_render_forward, cudaFuncAttributePreferredSharedMemoryCarveout,
                                      (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
-    attr_set = true;
-  }
+    return GOF_OK;
+  }, nullptr);
+  if (rc != GOF_OK) return rc;
   GOF_LAUNCH("render_fwd", st, k_render_forward<<<v.tiles, GOF_BLOCK_SIZE, 0, st>>>(a));
   GOF_LAUNCH_CHECK(s->debug, st);
   return GOF_OK;
