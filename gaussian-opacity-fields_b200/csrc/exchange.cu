@@ -89,75 +89,7 @@ __global__ void __launch_bounds__(512) k_nvls_allreduce(float4* mc, size_t begin
   }
 }
 
-
-// ---- tuning probes (tools/exchange_sweep.py): the SUM exchange with every launch parameter exposed.
-// layout 0: grid-stride lattice (consecutive warps of the whole grid touch consecutive 512 bytes); layout 1: each CTA walks
-// contiguous chunks of threads*U float4.  mode bit 0: reduce (ld_reduce / peer loads), bit 1: broadcast (st / peer stores).
-template <int U>
-__global__ void k_nvls_probe(float4* mc, size_t begin, size_t end, int layout, int mode, float4* sink) {
-  const size_t T = blockDim.x, G = gridDim.x;
-  const size_t inner = layout ? T : G * T;                      // distance between a thread's U elements
-  const size_t outer = G * T * U;                               // distance between a thread's rounds
-  size_t i = begin + (layout ? (size_t)blockIdx.x * T * U + threadIdx.x : (size_t)blockIdx.x * T + threadIdx.x);
-  float4 keep = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (; i < end; i += outer) {
-    float4 v[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const size_t j = i + u * inner;
-      v[u] = (j < end && (mode & 1)) ? mm_ld_add(mc + j) : make_float4(1.f, 1.f, 1.f, 1.f);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const size_t j = i + u * inner;
-      if (j < end) { if (mode & 2) mm_st(mc + j, v[u]); else keep.x += v[u].x + v[u].w; }
-    }
-  }
-  if (!(mode & 2) && keep.x == 123.456f) sink[0] = keep;
-}
-
-template <int W, int U>
-__global__ void k_p2p_probe(const PeerPtrs a, size_t begin, size_t end, int layout) {
-  const size_t T = blockDim.x, G = gridDim.x;
-  const size_t inner = layout ? T : G * T, outer = G * T * U;
-  size_t i = begin + (layout ? (size_t)blockIdx.x * T * U + threadIdx.x : (size_t)blockIdx.x * T + threadIdx.x);
-  for (; i < end; i += outer) {
-    float4 v[U][W];
-#pragma unroll
-    for (int u = 0; u < U; ++u)
-#pragma unroll
-      for (int r = 0; r < W; ++r) { const size_t j = i + u * inner; v[u][r] = j < end ? ld_cg(a.p[r] + j) : make_float4(0.f, 0.f, 0.f, 0.f); }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const size_t j = i + u * inner;
-      float4 s = v[u][0];
-#pragma unroll
-      for (int r = 1; r < W; ++r) s = combine(s, v[u][r], true);
-      if (j < end) {
-#pragma unroll
-        for (int r = 0; r < W; ++r) __stcg(a.p[r] + j, s);
-      }
-    }
-  }
-}
-
 }  // namespace
-
-// Peer access from the current device to `peer_device` (the device index, in THIS process, on which a peer bucket was
-// mapped).  CUDA IPC mappings opened under the exporting device's context are not reachable from kernels of another
-// device until this has been called once.  Idempotent.
-extern "C" GOF_API int gof_enable_peer_access(int peer_device) {
-  int cur = 0;
-  GOF_CUDA_OK(cudaGetDevice(&cur));
-  if (peer_device == cur) return GOF_OK;
-  int can = 0;
-  GOF_CUDA_OK(cudaDeviceCanAccessPeer(&can, cur, peer_device));
-  if (!can) { gof_set_error("device %d cannot access device %d (no NVLink/PCIe peer path)", cur, peer_device); return GOF_E_INVALID; }
-  const cudaError_t e = cudaDeviceEnablePeerAccess(peer_device, 0);
-  if (e == cudaErrorPeerAccessAlreadyEnabled) { (void)cudaGetLastError(); return GOF_OK; }
-  if (e != cudaSuccess) { gof_set_error("cudaDeviceEnablePeerAccess(%d): %s", peer_device, cudaGetErrorString(e)); return GOF_E_CUDA; }
-  return GOF_OK;
-}
 
 // A bucket that other processes can map: plain cudaMalloc (its own allocation, so the IPC handle addresses it at offset
 // 0), zero-filled.  handle64 receives the 64-byte cudaIpcMemHandle_t to send to the peers.
@@ -186,12 +118,6 @@ extern "C" GOF_API int gof_peer_open(const unsigned char* handle64, void** ptr) 
 }
 extern "C" GOF_API int gof_peer_close(void* ptr) { if (ptr) GOF_CUDA_OK(cudaIpcCloseMemHandle(ptr)); return GOF_OK; }
 extern "C" GOF_API int gof_peer_free(void* ptr) { if (ptr) GOF_CUDA_OK(cudaFree(ptr)); return GOF_OK; }
-
-// peers[r] = address (in THIS process) of rank r's bucket, r = 0..world-1; n = floats per bucket (multiple of 4,
-// 16-byte aligned buffers).  Reduces this rank's slice; the caller provides the two cross-rank barriers.
-extern "C" GOF_API int gof_p2p_allreduce_sum_f32(float* const* peers, int world, int rank, size_t n, void* stream) {
-  return gof_p2p_allreduce_f32(peers, world, rank, n, n, stream);
-}
 
 static unsigned exchange_grid(size_t items) {
   const size_t want = (items + 511) / 512;
@@ -238,40 +164,6 @@ extern "C" GOF_API int gof_p2p_allreduce_f32(float* const* peers, int world, int
     case 8: GOF_LAUNCH("p2p_allreduce", st, k_p2p_allreduce<8><<<grid, 512, 0, st>>>(a, begin, end, sum_end)); break;
     default: GOF_LAUNCH("p2p_allreduce", st, k_p2p_allreduce_any<<<grid, 512, 0, st>>>(a, world, begin, end, sum_end)); break;
   }
-  GOF_LAUNCH_CHECK(false, st);
-  return GOF_OK;
-}
-
-// Tuning probes (developer tools only; SUM over [n*rank/world, n*(rank+1)/world) of an n-float bucket).
-extern "C" GOF_API int gof_nvls_probe(float* mc, int world, int rank, size_t n, int grid, int threads, int unroll, int layout, int mode, float* sink,
-                                      void* stream) {
-  if (!mc || world < 1 || (n & 3u) || grid < 1 || threads < 32 || threads > 1024) { gof_set_error("nvls_probe: bad arguments"); return GOF_E_INVALID; }
-  const size_t n4 = n / 4, begin = n4 * (size_t)rank / (size_t)world, end = n4 * (size_t)(rank + 1) / (size_t)world;
-  cudaStream_t st = (cudaStream_t)stream;
-  float4* m = reinterpret_cast<float4*>(mc);
-  float4* sk = reinterpret_cast<float4*>(sink);
-  switch (unroll) {
-    case 1: k_nvls_probe<1><<<grid, threads, 0, st>>>(m, begin, end, layout, mode, sk); break;
-    case 2: k_nvls_probe<2><<<grid, threads, 0, st>>>(m, begin, end, layout, mode, sk); break;
-    case 4: k_nvls_probe<4><<<grid, threads, 0, st>>>(m, begin, end, layout, mode, sk); break;
-    case 8: k_nvls_probe<8><<<grid, threads, 0, st>>>(m, begin, end, layout, mode, sk); break;
-    default: gof_set_error("nvls_probe: unroll 1, 2, 4 or 8"); return GOF_E_INVALID;
-  }
-  GOF_LAUNCH_CHECK(false, st);
-  return GOF_OK;
-}
-extern "C" GOF_API int gof_p2p_probe(float* const* peers, int world, int rank, size_t n, int grid, int threads, int unroll, int layout, void* stream) {
-  if (!peers || (world != 2 && world != 4 && world != 8) || (n & 3u) || grid < 1 || threads < 32 || threads > 1024) {
-    gof_set_error("p2p_probe: bad arguments"); return GOF_E_INVALID; }
-  PeerPtrs a;
-  for (int r = 0; r < GOF_MAX_PEERS; ++r) a.p[r] = reinterpret_cast<float4*>(r < world ? peers[r] : nullptr);
-  const size_t n4 = n / 4, begin = n4 * (size_t)rank / (size_t)world, end = n4 * (size_t)(rank + 1) / (size_t)world;
-  cudaStream_t st = (cudaStream_t)stream;
-#define GOF_P2P_PROBE(W, U) k_p2p_probe<W, U><<<grid, threads, 0, st>>>(a, begin, end, layout)
-  if (world == 2) { if (unroll == 1) GOF_P2P_PROBE(2, 1); else if (unroll == 2) GOF_P2P_PROBE(2, 2); else if (unroll == 4) GOF_P2P_PROBE(2, 4); else GOF_P2P_PROBE(2, 8); }
-  else if (world == 4) { if (unroll == 1) GOF_P2P_PROBE(4, 1); else if (unroll == 2) GOF_P2P_PROBE(4, 2); else GOF_P2P_PROBE(4, 4); }
-  else { if (unroll == 1) GOF_P2P_PROBE(8, 1); else GOF_P2P_PROBE(8, 2); }
-#undef GOF_P2P_PROBE
   GOF_LAUNCH_CHECK(false, st);
   return GOF_OK;
 }

@@ -22,7 +22,6 @@ if not os.path.exists(_LIB_PATH):
     )
 _lib = ctypes.CDLL(_LIB_PATH)
 
-_TRACE = os.environ.get("GOF_TRACE") == "1"
 _ALLOC_FN = ctypes.CFUNCTYPE(ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t)
 _fp = ctypes.c_void_p  # device pointers travel as integers
 
@@ -143,7 +142,6 @@ class _Pool:
 
 
 _POOL = _Pool()
-_USE_POOL = os.environ.get("GOF_POOL", "1") != "0"
 
 
 class _Scratch:
@@ -158,7 +156,7 @@ class _Scratch:
     def __init__(self, device, role="", slack=1.0):
         holder = [torch.empty(0, dtype=torch.uint8, device=device)]
         self._holder = holder
-        pooled = bool(_USE_POOL and role)
+        pooled = bool(role)
 
         def alloc(_user, nbytes):
             try:
@@ -176,13 +174,7 @@ class _Scratch:
                 holder[0] = None                      # drop our reference before asking: the old buffer may be reusable
                 holder[0] = _POOL.take(key, int(nbytes), device, slack)
             else:
-                if _TRACE:
-                    import time
-                    t0 = time.perf_counter()
                 holder[0] = torch.empty(int(nbytes), dtype=torch.uint8, device=device)   # >= 512-byte aligned
-                if _TRACE:
-                    print(f"[gof trace py] alloc {int(nbytes)} bytes took {1e6 * (time.perf_counter() - t0):.1f} us",
-                          file=sys.stderr, flush=True)
             return holder[0].data_ptr()
 
         self.cb = _ALLOC_FN(alloc)

@@ -12,15 +12,11 @@ the embedding broadcast to the 1/32 grid) are built without the `repeat().permut
 `load_flat_grads_` pack the network's and the embedding's gradients into the view-parallel gradient bucket
 (gof_dp.GradBucket(extra_sum=...)) so that they travel in the same exchange as the Gaussian gradients."""
 import ctypes
-import os
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-# A/B switches (developer use): GOF_APP_WGRAD=0 -> cuDNN's weight gradients, GOF_APP_NHWC=1 -> channels-last activations
-_USE_WGRAD = os.environ.get("GOF_APP_WGRAD", "1") != "0"
-_USE_NHWC = os.environ.get("GOF_APP_NHWC", "0") == "1"
 _WGRAD_PAIRS = {(16, 16), (3, 16), (16, 8)}          # (C_out, C_in) pairs csrc/conv_wgrad.cu is instantiated for
 _lib = None
 
@@ -63,7 +59,7 @@ class _Conv3x3(torch.autograd.Function):
 def conv3x3(x, conv):
     """`conv(x)` for an nn.Conv2d(3x3, stride 1, pad 1), through _Conv3x3 when its weight gradient is worth taking over."""
     w = conv.weight
-    if (_USE_WGRAD and x.is_cuda and x.dtype == torch.float32 and x.shape[0] == 1 and (int(w.shape[0]), int(w.shape[1])) in _WGRAD_PAIRS
+    if (x.is_cuda and x.dtype == torch.float32 and x.shape[0] == 1 and (int(w.shape[0]), int(w.shape[1])) in _WGRAD_PAIRS
             and x.shape[2] * x.shape[3] >= 128 * 128 and conv.bias is not None and torch.is_grad_enabled() and w.requires_grad):
         return _Conv3x3.apply(x, w, conv.bias)
     return conv(x)
@@ -94,8 +90,6 @@ class AppearanceNetwork(nn.Module):   # scene/appearance_network.py:18-46
         self.sigmoid = nn.Sigmoid()
 
     def forward(self, x):
-        if x.is_cuda and _USE_NHWC:      # no gain measured (cuDNN converts back and forth around its NCHW engines)
-            x = x.contiguous(memory_format=torch.channels_last)
         x = self.relu(self.conv1(x))
         x = self.up4(self.up3(self.up2(self.up1(x))))
         x = F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True)

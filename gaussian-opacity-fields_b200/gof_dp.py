@@ -26,7 +26,6 @@ gof_rasterize_backward_stats): `dens_sum` (P,3) = (|dL_dmean2D.xy|, |dL_dmean2D.
 (P,2) = (|dL_dmean2D.z|, radius) reduced with MAX -- what GaussianModel.add_densification_stats and train.py:255 accumulate.
 """
 import ctypes
-import os
 
 import torch
 import torch.distributed as dist
@@ -35,7 +34,6 @@ import torch.distributed as dist
 _FIELDS = (("dmeans3D", (3,)), ("dsh", None), ("dopacity", (1,)), ("dscales", (3,)), ("drot", (4,)))
 _STAT_FIELDS = (("dens_sum", (3,)), ("dens_max", (2,)))       # SUM region ends where dens_max starts
 SH_SLOT_HEADER = 64                                           # floats in front of a view record's rgb (include/gof_rasterizer.h)
-_OVERLAP = os.environ.get("GOF_DP_OVERLAP", "0") == "1"       # A/B: record expansion on a side stream, next to the reduction kernel
 
 
 class GradBucket:
@@ -83,7 +81,6 @@ class GradBucket:
         self.flat = torch.zeros(max(self.numel, 64), dtype=dtype, device=device)
         self.views = self._make_views()
         self._symm = None        # torch symmetric-memory handle (NVLS exchange)
-        self._side = None        # side stream of the overlapped record expansion
 
         self._peer_ptrs = None   # addresses (this process) of every rank's bucket, index = rank; own cudaMalloc at [rank]
         self._own_ptr, self._mapped = None, []
@@ -426,24 +423,13 @@ class GradBucket:
             # after the local kernels and completes only when every rank has reached it)
             dist.all_reduce(self._sync, group=group)
             stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-            side = None
-            if expand and _OVERLAP:   # the record expansion and the reduction are independent: run them side by side
-                cur = torch.cuda.current_stream()
-                if self._side is None:
-                    self._side = torch.cuda.Stream(device=self.flat.device)
-                side = self._side
-                side.wait_stream(cur)
-                with torch.cuda.stream(side):
-                    self._expand_sh(self._record_ptrs(), means3D)
             with torch.cuda.device(self.flat.device):
                 if self.exchange == "p2p":
                     self._check(self._lib.gof_p2p_allreduce_f32(self._peer_ptrs, self._world, self._rank, self.n_sum, self.n_reduce, stream))
                 else:
                     self._check(self._lib.gof_nvls_allreduce_f32(ctypes.c_void_p(self._mc), self._world, self._rank, self.n_sum,
                                                                  self.n_reduce, stream))
-            if side is not None:
-                torch.cuda.current_stream().wait_stream(side)
-            elif expand:   # the views' records are read where the ranks left them, over NVLink
+            if expand:   # the views' records are read where the ranks left them, over NVLink
                 self._expand_sh(self._record_ptrs(), means3D)
             # barrier: every slice has been written into every bucket (and every record has been read)
             dist.all_reduce(self._sync, group=group)

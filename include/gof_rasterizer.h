@@ -282,19 +282,15 @@ GOF_API int gof_stats_read(unsigned long long* out);
  * ranks of a flat f32 buffer over NVLink peer memory.  peers[r] = address, valid in THIS process, of rank r's buffer
  * (CUDA IPC mapping; peers[rank] is the local one); n = floats per buffer (multiple of 4, 16-byte aligned).  This
  * rank reduces its 1/world slice from all buffers (rank order 0..world-1: bit-identical results everywhere) and
- * stores it into all of them.  The caller brackets the call with two cross-rank barriers on `stream`. */
-GOF_API int gof_p2p_allreduce_sum_f32(float* const* peers, int world, int rank, size_t n, void* stream);
-/* The same with a MAX tail: floats [0, n_sum) are summed over the ranks, [n_sum, n) max-reduced (the densification statistics
- * max_radii2D / xyz_gradient_accum_abs_max travel in the same bucket); n_sum, n multiples of 4. */
+ * stores it into all of them.  The caller brackets the call with two cross-rank barriers on `stream`.
+ * Floats [0, n_sum) are summed over the ranks, [n_sum, n) max-reduced (the densification statistics
+ * max_radii2D / xyz_gradient_accum_abs_max travel in the same bucket); n_sum a multiple of 4, n_sum == n: plain sum. */
 GOF_API int gof_p2p_allreduce_f32(float* const* peers, int world, int rank, size_t n_sum, size_t n, void* stream);
 /* The same exchange reduced INSIDE the NVSwitch (NVLS): `mc` is the multicast address, valid in this process, of a buffer that
  * every rank has bound to one multicast object at the same offset (e.g. a torch symmetric-memory allocation).  One kernel:
  * multimem.ld_reduce of this rank's 1/world slice (sum, or unsigned max for the non-negative MAX tail) + multimem.st of the
  * result to all ranks.  The caller brackets the call with two cross-rank barriers on `stream`. */
 GOF_API int gof_nvls_allreduce_f32(float* mc, int world, int rank, size_t n_sum, size_t n, void* stream);
-/* Enables peer access from the current device to `peer_device` (needed once per peer before kernels of this device
- * may dereference that peer's IPC-mapped memory).  Idempotent. */
-GOF_API int gof_enable_peer_access(int peer_device);
 /* Buffers for that exchange: gof_peer_alloc = cudaMalloc'ed, zero-filled buffer + its 64-byte CUDA IPC handle;
  * gof_peer_open maps a peer's buffer (handle received from that process) for the CURRENT device. */
 GOF_API int gof_peer_alloc(size_t bytes, void** ptr, unsigned char* handle64);

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Developer timing (GPU box): ms per fwd+bwd step of a config over the 64-view ring (device-resident inputs, CUDA events) and
-the per-kernel split from the library's event brackets.  Environment knobs (GOF_CULL, GOF_POOL) are read by the library
-once per process, so A/B runs are separate invocations:   GOF_CULL=0 python tools/step_time.py C3 30 label"""
+the per-kernel split from the library's event brackets.  The environment knob GOF_CULL is read by the library once per
+process, so A/B runs are separate invocations:   GOF_CULL=0 python tools/step_time.py C3 30 label"""
 import json
 import os
 import sys
