@@ -352,7 +352,9 @@ int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const
                                    const GofGeomLayout& L, const int* radii, float* dL_dmean2D, float* dL_dopacity,
                                    float* dL_dcolor, float* dL_dv2g, float* dL_dmean3D, float* dL_dsh, float* dL_dscale,
                                    float* dL_drot, float* dL_dcov3D, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
-                                   cudaStream_t st);
+                                   float* dL_dviewmatrix, float* dL_dcampos, void* cam_scratch, cudaStream_t st);
+// bytes of cam_scratch: the camera-gradient pass (dL_dviewmatrix non-NULL) leaves one partial row per CTA there
+size_t gof_camera_grad_scratch_bytes(int P);
 int gof_launch_mark_visible(int P, const float* means3D, const float* vm, unsigned char* present,
                             cudaStream_t st);
 

@@ -244,6 +244,9 @@ struct PreBwdArgs {
   float* sh_rgb;            // optional [3][GOF_SH_PLANE(P)] planes: the clamp-masked dL_dRGB the SH gradient is the outer product of
   float* sh_hdr;            //   (view-parallel exchange, csrc/sh_views.cu); sh_hdr[0..3] = camera centre, active degree.  dL_dsh may be NULL.
   size_t sh_plane;
+  // camera gradient (k_preprocess_backward<true> only)
+  double* cam_partial;      // [gridDim.x][K8_CAM_ROW]: the CTA's sum of its Gaussians' camera terms
+  int cam_vm;               // 0: view2gaussian was precomputed, so the view matrix receives no gradient
 };
 
 // m[c][r] column-major helpers mirroring the glm products used by backward.cu:381-587.  The chain rule through
@@ -271,6 +274,9 @@ __device__ __forceinline__ M3 m3_t(const M3& A) {
 
 constexpr int K8_THREADS = 128;
 constexpr int K8_ROW = 49;   // 48 SH-gradient floats per Gaussian + 1 pad: lanes of a warp hit distinct banks
+// Camera terms of one Gaussian (DESIGN.md 4.9): dL_dviewmatrix[4k+i] for k < 4, i < 3 at 3k+i, dL_dcampos at 12..14; a partial
+// row holds them plus one pad double.
+constexpr int K8_CAM_TERMS = 15, K8_CAM_ROW = 16;
 
 // The outputs with rows of 2..10 floats, staged per warp in shared memory: each field holds the warp's 32 rows back to back, i.e.
 // exactly the layout of the warp's block of the global tensor.  Every field starts on a multiple of 32 floats, so the copy-out
@@ -289,6 +295,9 @@ __device__ __forceinline__ void k8_copy_out(float* __restrict__ dst, const float
   for (; i < n; i += 32) dst[i] = src[i];
 }
 
+// CAMERA: also form this Gaussian's camera terms and leave the CTA's fp64 sum of them in a.cam_partial (the instantiation
+// without it is the plain backward, instruction for instruction).
+template <bool CAMERA>
 __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwdArgs a) {
   // Every output leaves through shared memory: a thread produces its Gaussian's row (for dL_dsh one coefficient at a time), the
   // warp then writes its 32 consecutive Gaussians as one contiguous block with 128-bit stores.  Per-thread stores at the rows'
@@ -317,6 +326,11 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
   float dopacity = 0.f, dscale[3] = {0.f, 0.f, 0.f}, dmean[3] = {0.f, 0.f, 0.f}, dens[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
   float4 drot = make_float4(0.f, 0.f, 0.f, 0.f);
   float dRGB[3] = {0.f, 0.f, 0.f};
+  double cam[K8_CAM_TERMS];
+  if constexpr (CAMERA) {
+#pragma unroll
+    for (int k = 0; k < K8_CAM_TERMS; ++k) cam[k] = 0.0;
+  }
 
   if (active) {
   // the blend kernel's accumulator row -> the public gradient tensors (the double sums rounded once to float)
@@ -449,6 +463,19 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
       for (int rr = 0; rr < 3; ++rr)
         dG2W[c][rr] = vm[4 * rr + 0] * dG2V[c][0] + vm[4 * rr + 1] * dG2V[c][1] + vm[4 * rr + 2] * dG2V[c][2];
     dmean[0] = (float)dG2W[3][0]; dmean[1] = (float)dG2W[3][1]; dmean[2] = (float)dG2W[3][2];   // :570-573
+    if constexpr (CAMERA) {
+      // G2V[c][i] = sum_k vm[4k+i] R[k][c] (c < 3) and G2V[3][i] = sum_k vm[4k+i] h_k, h = (mean, 1)
+      if (a.cam_vm) {
+        const double h[3] = {mx, my, mz};
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+          for (int i = 0; i < 3; ++i)
+            cam[3 * k + i] = dG2V[0][i] * R.m[k][0] + dG2V[1][i] * R.m[k][1] + dG2V[2][i] * R.m[k][2] + dG2V[3][i] * h[k];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) cam[9 + i] = dG2V[3][i];
+      }
+    }
 
     // :575-586 quaternion gradient from dL_dMt = dL_dG2W_R
 #define MT(c, r) dG2W[c][r]
@@ -539,6 +566,16 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
     dmean[0] += ((+sum2 - dox * dox) * ddx - doy * dox * ddy - doz * dox * ddz) * invsum32;
     dmean[1] += (-dox * doy * ddx + (sum2 - doy * doy) * ddy - doz * doy * ddz) * invsum32;
     dmean[2] += (-dox * doz * ddx - doy * doz * ddy + (sum2 - doz * doz) * ddz) * invsum32;
+    if constexpr (CAMERA) {
+      // the direction is mean - campos: minus the SH term of dL_dmean3D, evaluated again in double from the same float
+      // ddx, ddy, ddz (the float expressions above keep their own rounding, so dL_dmean3D is the plain backward's)
+      const double ex = dox, ey = doy, ez = doz;
+      const double s2 = ex * ex + ey * ey + ez * ez, inv = 1.0 / (s2 * sqrt(s2));
+      const double gx = ddx, gy = ddy, gz = ddz;
+      cam[12] = -(((s2 - ex * ex) * gx - ey * ex * gy - ez * ex * gz) * inv);
+      cam[13] = -((-ex * ey * gx + (s2 - ey * ey) * gy - ez * ey * gz) * inv);
+      cam[14] = -((-ex * ez * gx - ey * ez * gy + (s2 - ez * ez) * gz) * inv);
+    }
   }
   }   // active
 
@@ -594,9 +631,60 @@ __global__ void __launch_bounds__(K8_THREADS) k_preprocess_backward(const PreBwd
       }
     }
   }
+
+  // ---- the CTA's camera row: a fixed shuffle tree per warp, then the warps in order (no atomics: bit-reproducible) ----
+  if constexpr (CAMERA) {
+    __shared__ double s_cam[K8_THREADS / 32][K8_CAM_TERMS];
+#pragma unroll
+    for (int k = 0; k < K8_CAM_TERMS; ++k) {
+      double t = cam[k];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_down_sync(0xffffffffu, t, o);
+      if (lane == 0) s_cam[warp][k] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x < K8_CAM_ROW) {
+      double t = 0.0;
+      if (threadIdx.x < K8_CAM_TERMS) {
+        t = s_cam[0][threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < K8_THREADS / 32; ++w) t += s_cam[w][threadIdx.x];
+      }
+      a.cam_partial[(size_t)blockIdx.x * K8_CAM_ROW + threadIdx.x] = t;
+    }
+  }
+}
+
+// The camera gradient from the partial rows of k_preprocess_backward<true>: group g of 16 threads sums rows g, g + 64, ... in
+// index order, a fixed tree joins the 64 groups, and the sums are rounded to float once.  dL_dviewmatrix[4k+3] (the
+// coefficients of the view matrix's fourth row, which view2gaussian does not read) are written as zeros.
+constexpr int CAM_SUM_THREADS = 1024, CAM_SUM_GROUPS = CAM_SUM_THREADS / K8_CAM_ROW;
+__global__ void __launch_bounds__(CAM_SUM_THREADS) k_camera_grad_sum(int rows, const double* __restrict__ partial,
+                                                                       float* __restrict__ dL_dviewmatrix, float* __restrict__ dL_dcampos) {
+  __shared__ double s[CAM_SUM_GROUPS][K8_CAM_ROW];
+  const int j = threadIdx.x % K8_CAM_ROW, g = threadIdx.x / K8_CAM_ROW;
+  double t = 0.0;
+#pragma unroll 4
+  for (int r = g; r < rows; r += CAM_SUM_GROUPS) t += partial[(size_t)r * K8_CAM_ROW + j];
+  s[g][j] = t;
+  __syncthreads();
+#pragma unroll
+  for (int n = CAM_SUM_GROUPS / 2; n > 0; n >>= 1) {
+    if (g < n) s[g][j] += s[g + n][j];
+    __syncthreads();
+  }
+  if (threadIdx.x < 16) {
+    const int k = threadIdx.x >> 2, i = threadIdx.x & 3;
+    dL_dviewmatrix[threadIdx.x] = i < 3 ? (float)s[0][3 * k + i] : 0.f;
+  }
+  if (threadIdx.x < 3) dL_dcampos[threadIdx.x] = (float)s[0][12 + threadIdx.x];
 }
 
 }  // namespace
+
+size_t gof_camera_grad_scratch_bytes(int P) {
+  return P > 0 ? (size_t)((P + K8_THREADS - 1) / K8_THREADS) * K8_CAM_ROW * sizeof(double) : 0;
+}
 
 int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& L,
                           int* radii, float box_margin, cudaStream_t st) {
@@ -637,7 +725,7 @@ int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const
                                    const GofGeomLayout& L, const int* radii, float* dL_dmean2D, float* dL_dopacity,
                                    float* dL_dcolor, float* dL_dv2g, float* dL_dmean3D, float* dL_dsh, float* dL_dscale,
                                    float* dL_drot, float* dL_dcov3D, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
-                                   cudaStream_t st) {
+                                   float* dL_dviewmatrix, float* dL_dcampos, void* cam_scratch, cudaStream_t st) {
   (void)v;
   PreBwdArgs a{};
   a.P = s->P; a.D = s->D; a.M = s->M;
@@ -651,7 +739,17 @@ int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const
   a.dL_dscale = dL_dscale; a.dL_drot = dL_drot; a.dL_dcov3D = dL_dcov3D;
   a.dens_sum = (dens_sum && dens_max) ? dens_sum : nullptr; a.dens_max = a.dens_sum ? dens_max : nullptr;
   a.sh_rgb = s->shs ? sh_rgb : nullptr; a.sh_hdr = a.sh_rgb ? sh_hdr : nullptr; a.sh_plane = GOF_SH_PLANE(s->P);
-  GOF_LAUNCH("preprocess_bwd", st, k_preprocess_backward<<<(s->P + K8_THREADS - 1) / K8_THREADS, K8_THREADS, 0, st>>>(a));
+  const int blocks = (s->P + K8_THREADS - 1) / K8_THREADS;
+  if (dL_dviewmatrix == nullptr) {
+    GOF_LAUNCH("preprocess_bwd", st, k_preprocess_backward<false><<<blocks, K8_THREADS, 0, st>>>(a));
+    GOF_LAUNCH_CHECK(s->debug, st);
+    return GOF_OK;
+  }
+  a.cam_partial = static_cast<double*>(cam_scratch);
+  a.cam_vm = s->view2gaussian_precomp == nullptr;
+  GOF_LAUNCH("preprocess_bwd_camera", st, k_preprocess_backward<true><<<blocks, K8_THREADS, 0, st>>>(a));
+  GOF_LAUNCH_CHECK(s->debug, st);
+  GOF_LAUNCH("camera_grad_sum", st, k_camera_grad_sum<<<1, CAM_SUM_THREADS, 0, st>>>(blocks, a.cam_partial, dL_dviewmatrix, dL_dcampos));
   GOF_LAUNCH_CHECK(s->debug, st);
   return GOF_OK;
 }

@@ -57,6 +57,10 @@ _lib.gof_rasterize_backward_stats.restype = ctypes.c_int
 _lib.gof_rasterize_backward_stats.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 17 + [ctypes.c_void_p]
 _lib.gof_rasterize_backward_dp.restype = ctypes.c_int
 _lib.gof_rasterize_backward_dp.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 19 + [ctypes.c_void_p]
+_lib.gof_rasterize_backward_camera_scratch_bytes.restype = ctypes.c_size_t
+_lib.gof_rasterize_backward_camera_scratch_bytes.argtypes = [ctypes.c_int]
+_lib.gof_rasterize_backward_camera.restype = ctypes.c_int
+_lib.gof_rasterize_backward_camera.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 20 + [ctypes.c_size_t, ctypes.c_void_p]
 _lib.gof_sh_grad_from_views.restype = ctypes.c_int
 _lib.gof_sh_grad_from_views.argtypes = [ctypes.c_int] * 3 + [_fp, ctypes.c_void_p, _fp, ctypes.c_void_p]
 _lib.gof_mark_visible.restype = ctypes.c_int
@@ -243,10 +247,11 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
                                  cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                                  kernel_size, subpixel_offset, dL_dout_color, sh, degree, campos, geomBuffer, R,
-                                 binningBuffer, imageBuffer, debug, _out=None):
+                                 binningBuffer, imageBuffer, debug, _out=None, _camera=False):
     """RasterizeGaussiansBackwardCUDA (rasterize_points.cu:124-211).  Returns, in the reference's order
     (:210): (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
-    dL_drotations, dL_dview2gaussian)."""
+    dL_drotations, dL_dview2gaussian).  `_camera=True` (extension, gof_rasterize_backward_camera) appends
+    dL_dviewmatrix and dL_dcampos, shaped like viewmatrix and campos."""
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
     keep = []
@@ -267,6 +272,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     # csrc/sh_views.cu) -- the backward leaves the clamp-masked dL_dRGB and the camera centre instead of dL_dsh, which only exists
     # after the bucket's exchange (the returned dL_dsh is then _out.get("dsh"): the tensor the exchange fills)
     factored = _out is not None and "dsh_rgb" in _out
+    if factored and _camera:
+        raise NotImplementedError("gof_b200: camera gradients are not available with the factored SH gradient (_out['dsh_rgb'])")
     if factored:
         rgb_t, hdr_t = _out["dsh_rgb"], _out.get("sh_hdr")
         if sh is None or sh.numel() == 0:
@@ -316,7 +323,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     dL_dscales = _z("dscales", (P, 3))
     dL_drotations = _z("drot", (P, 4))
     dL_dv2g = _z("dv2g", (P, 10))
-    if P != 0:
+    if _camera:
+        if viewmatrix.numel() != 16 or campos.numel() != 3:
+            raise RuntimeError("gof_b200: camera gradients need a 16-element viewmatrix and a 3-element campos")
+        cam_out = torch.empty(19, dtype=torch.float32, device=means3D.device)
+        dL_dviewmatrix, dL_dcampos = cam_out[:16], cam_out[16:]
+    if P != 0 or _camera:   # with P == 0 the camera entry point writes zeros
         g = dL_dout_color.contiguous()
         rad = radii.contiguous()
         with torch.cuda.device(means3D.device):
@@ -328,17 +340,25 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             if ds is not None and not (ds.is_contiguous() and dm.is_contiguous() and tuple(ds.shape) == (P, 3) and tuple(dm.shape) == (P, 2)
                                        and ds.dtype == torch.float32 and dm.dtype == torch.float32):
                 raise RuntimeError("gof_b200: dens_sum must be a contiguous float32 (P,3) and dens_max (P,2) tensor")
-            _check(_lib.gof_rasterize_backward_dp(
-                ctypes.byref(s), int(R), _ptr(rad, torch.int32), _ptr(geomBuffer, torch.uint8),
-                _ptr(binningBuffer, torch.uint8), _ptr(imageBuffer, torch.uint8), _ptr(g),
-                dL_dmeans2D.data_ptr(), None, dL_dopacity.data_ptr(), dL_dcolors.data_ptr(),
-                dL_dmeans3D.data_ptr(), dL_dcov3D.data_ptr(), (_ptr(full_t) if full_t is not None else None) if factored else _ptr(dL_dsh),
-                dL_dscales.data_ptr(),
-                dL_drotations.data_ptr(), dL_dv2g.data_ptr(), ds.data_ptr() if ds is not None else None,
-                dm.data_ptr() if dm is not None else None, rgb_t.data_ptr() if factored else None,
-                hdr_t.data_ptr() if factored else None, _stream()))
-    return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations,
-            dL_dv2g)
+            common = (ctypes.byref(s), int(R), _ptr(rad, torch.int32), _ptr(geomBuffer, torch.uint8),
+                      _ptr(binningBuffer, torch.uint8), _ptr(imageBuffer, torch.uint8), _ptr(g),
+                      dL_dmeans2D.data_ptr(), None, dL_dopacity.data_ptr(), dL_dcolors.data_ptr(),
+                      dL_dmeans3D.data_ptr(), dL_dcov3D.data_ptr(),
+                      (_ptr(full_t) if full_t is not None else None) if factored else _ptr(dL_dsh),
+                      dL_dscales.data_ptr(), dL_drotations.data_ptr(), dL_dv2g.data_ptr(),
+                      ds.data_ptr() if ds is not None else None, dm.data_ptr() if dm is not None else None)
+            if _camera:
+                nbytes = int(_lib.gof_rasterize_backward_camera_scratch_bytes(P))
+                scratch = torch.empty(nbytes, dtype=torch.uint8, device=means3D.device)
+                _check(_lib.gof_rasterize_backward_camera(*common, dL_dviewmatrix.data_ptr(), dL_dcampos.data_ptr(),
+                                                          scratch.data_ptr(), nbytes, _stream()))
+            else:
+                _check(_lib.gof_rasterize_backward_dp(*common, rgb_t.data_ptr() if factored else None,
+                                                      hdr_t.data_ptr() if factored else None, _stream()))
+    grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations, dL_dv2g)
+    if _camera:
+        grads += (dL_dviewmatrix.view(viewmatrix.shape), dL_dcampos.view(campos.shape))
+    return grads
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):

@@ -62,12 +62,22 @@ def _camera_args(rs):
     return (rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.kernel_size, rs.subpixel_offset)
 
 
+def _camera_inputs(rs):
+    """(viewmatrix, campos) when autograd is to differentiate the render with respect to the camera, otherwise ()."""
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rs.viewmatrix, rs.campos)):
+        return (rs.viewmatrix, rs.campos)
+    return ()
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                view2gaussian_precomp, raster_settings, grad_bucket=None):
+                view2gaussian_precomp, raster_settings, grad_bucket=None, viewmatrix=None, campos=None):
+        """viewmatrix / campos (extension): raster_settings' own camera tensors, passed as inputs only when they are to
+        receive gradients (the render reads them from raster_settings either way)."""
         rs = raster_settings
         ctx.grad_bucket = grad_bucket
+        ctx.camera = viewmatrix is not None
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
                 view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, sh, rs.sh_degree,
                                                              rs.campos, rs.prefiltered, rs.debug)
@@ -89,22 +99,30 @@ class _RasterizeGaussians(torch.autograd.Function):
                 view2gaussian_precomp) + _camera_args(rs) + (grad_out_color, sh, rs.sh_degree, rs.campos, geom,
                                                              ctx.num_rendered, binning, img, rs.debug)
         bucket = ctx.grad_bucket
-        (g_means2D, g_colors, g_opacity, g_means3D, g_cov3D, g_sh, g_scales, g_rot, g_v2g) = _call_native(
-            _C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", "backward",
-            **({"_out": bucket.views} if bucket is not None else {}))
+        kw = {"_out": bucket.views} if bucket is not None else {}
+        if ctx.camera:
+            kw["_camera"] = True
+        grads = _call_native(_C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", "backward", **kw)
+        (g_means2D, g_colors, g_opacity, g_means3D, g_cov3D, g_sh, g_scales, g_rot, g_v2g) = grads[:9]
         if bucket is not None:
             # extension (view-parallel training, gof_dp.GradBucket): the parameter gradients and this view's densification
             # statistics were written INTO the bucket -- they are read from bucket.views after bucket.all_reduce(), not from
             # .grad (autograd would copy the 256 MB out of the exchange buffer again)
             g_means3D = g_sh = g_opacity = g_scales = g_rot = None
         # one gradient per forward input, in input order (reference :152-163)
-        return (g_means3D, g_means2D, g_sh, g_colors, g_opacity, g_scales, g_rot, g_cov3D, g_v2g, None, None)
+        out = (g_means3D, g_means2D, g_sh, g_colors, g_opacity, g_scales, g_rot, g_cov3D, g_v2g, None, None)
+        if ctx.camera:
+            out += tuple(g if need else None for g, need in zip(grads[9:], ctx.needs_input_grad[11:]))
+        return out
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         view2gaussian_precomp, raster_settings):
+    """With grad mode on and raster_settings.viewmatrix or .campos requiring grad, the backward also differentiates the
+    render with respect to them (DESIGN.md 4.9); projmatrix is treated as a constant."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, view2gaussian_precomp, raster_settings, None)
+                                     cov3Ds_precomp, view2gaussian_precomp, raster_settings, None,
+                                     *_camera_inputs(raster_settings))
 
 
 def _absent():
@@ -144,6 +162,8 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp = _normalise_optionals(
             shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp)
         if self.grad_bucket is not None:
+            if _camera_inputs(self.raster_settings):
+                raise NotImplementedError("camera gradients (viewmatrix / campos requiring grad) are not available with a grad_bucket")
             return _RasterizeGaussians.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                              cov3D_precomp, view2gaussian_precomp, self.raster_settings, self.grad_bucket)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,

@@ -116,6 +116,23 @@ GOF_API int gof_rasterize_backward_stats(const gof_scene_t* scene, int num_rende
                            float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dens_sum,
                            float* dens_max, void* stream);
 
+/* gof_rasterize_backward_stats that also differentiates the loss with respect to the camera (no reference counterpart; the
+ * definition is DESIGN section 4.9).  dL_dviewmatrix [16] gets the gradient in the layout of scene->viewmatrix (vm[4k+i] is the
+ * coefficient of W2V[i][k]; the four vm[4k+3] are written as exact zeros) through view2gaussian, zero when view2gaussian_precomp
+ * is given; dL_dcampos [3] gets minus the SH-direction part of dL_dmean3D, zero with colors_precomp.  Both are sums over the
+ * Gaussians with radii > 0, accumulated in double in a fixed order and rounded to float once: bit-reproducible for the same
+ * per-Gaussian inputs.  The 2D mip-filter coefficient, the projection matrix, means2D and the tile binning are constants.
+ * scratch: gof_rasterize_backward_camera_scratch_bytes(P) device bytes, 8-byte aligned, contents irrelevant (the library does
+ * not allocate).  P == 0 or no visible Gaussian writes zeros.  Both NULL: plain gof_rasterize_backward_stats (scratch unused);
+ * exactly one NULL fails with GOF_E_INVALID. */
+GOF_API size_t gof_rasterize_backward_camera_scratch_bytes(int P);
+GOF_API int gof_rasterize_backward_camera(const gof_scene_t* scene, int num_rendered, const int* radii, void* geom_buffer,
+                           const void* binning_buffer, const void* image_buffer, const float* dL_dpix, float* dL_dmean2D,
+                           float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                           float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dens_sum,
+                           float* dens_max, float* dL_dviewmatrix /*[16]*/, float* dL_dcampos /*[3]*/, void* scratch,
+                           size_t scratch_bytes, void* stream);
+
 /* View-parallel training (one view per GPU, gradients summed over the GPUs; no reference counterpart -- the reference is
  * single-GPU).  The SH gradient of ONE view is an outer product: dL_dsh[g][k][c] = w_k(dir(mean_g, camera)) * dL_dRGB[g][c]
  * (backward.cu:45-139), so the ranks exchange the 3 floats of the clamp-masked dL_dRGB per Gaussian and view instead of the
