@@ -3,26 +3,7 @@
 #include <stdarg.h>
 #include <stdlib.h>
 
-#include <chrono>
-
 #include "gof_common.cuh"
-
-// GOF_TRACE=1: host-side phase timings of every forward call on stderr (aux tracing; the reference has none)
-static bool gof_trace_on() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("GOF_TRACE"); on = (e && e[0] == '1') ? 1 : 0; }
-  return on == 1;
-}
-struct GofTrace {
-  std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-  double last = 0;
-  void mark(const char* what) {
-    if (!gof_trace_on()) return;
-    double t = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
-    fprintf(stderr, "[gof trace] %-22s +%9.1f us (t=%9.1f us)\n", what, t - last, t);
-    last = t;
-  }
-};
 
 // ---- launch counter + optional per-kernel event timing ----------------------------------------------------
 #include <map>
@@ -176,11 +157,10 @@ static int finish_async_read_u32(SideCopy* sc, uint32_t* out) {
 }
 
 // ---- per-device launch state ---------------------------------------------------------------------------------
-// Function attributes, SM counts and the statistics counters belong to one device; a process may drive several, from
-// several host threads (autograd runs the backward on its own thread).  One mutex guards all of it.
+// Function attributes and SM counts belong to one device; a process may drive several, from several host threads
+// (autograd runs the backward on its own thread).  One mutex guards all of it.
 static std::mutex g_dev_mu;
 static std::map<std::pair<int, const void*>, int> g_dev_once;   // (device, key) -> the value its setup left
-static std::map<int, unsigned long long*> g_stats_dev;           // device -> GOF_STATS counters
 
 int gof_device_once(const void* key, int (*setup)(int dev, int* value), int* value) {
   int dev = 0;
@@ -204,26 +184,6 @@ int gof_sm_count() {
     return GOF_OK;
   }, &n);
   return n;
-}
-
-unsigned long long* gof_stats_buffer() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("GOF_STATS"); on = (e && e[0] == '1') ? 1 : 0; }
-  if (!on) return nullptr;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lk(g_dev_mu);
-  unsigned long long*& buf = g_stats_dev[dev];
-  if (!buf) { cudaMalloc(&buf, 8 * sizeof(unsigned long long)); cudaMemset(buf, 0, 8 * sizeof(unsigned long long)); }
-  return buf;
-}
-// copies the current device's 8 counters to `out` (host) and clears them; returns 0 if statistics are disabled
-extern "C" int gof_stats_read(unsigned long long* out) {
-  unsigned long long* buf = gof_stats_buffer();
-  if (!buf) return 0;
-  cudaMemcpy(out, buf, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-  cudaMemset(buf, 0, 8 * sizeof(unsigned long long));
-  return 1;
 }
 
 static thread_local char g_err[1024] = "";
@@ -277,8 +237,7 @@ static int validate_scene(const gof_scene_t* s) {
 // The Gaussian side of the forward and of the opacity-field query: geometry and image scratch, preprocess, depth sort, the
 // instance count (it sizes the binning buffer, rasterizer_impl.cu:334-340, and is read while the depth sort runs) and the tile
 // binning.  box_margin (gof_cull_bbox) is 0 for the forward and 0.5 for the query, whose corner rays reach half a pixel beyond
-// the centre ray; only the forward's binning buffer carries the blend masks its backward reads.  tr: the forward's GOF_TRACE
-// marks, or NULL.
+// the centre ray; only the forward's binning buffer carries the blend masks its backward reads.
 struct GaussianSide {
   GofGeomLayout GL;
   GofImageLayout IL;
@@ -288,14 +247,13 @@ struct GaussianSide {
 };
 static int gaussian_side(const gof_scene_t* s, const GofView& v, gof_alloc_fn geom_alloc, void* geom_user, gof_alloc_fn binning_alloc,
                          void* binning_user, gof_alloc_fn image_alloc, void* image_user, int* radii, float box_margin, bool with_masks,
-                         int* num_rendered, GofTrace* tr, cudaStream_t st, GaussianSide& g) {
+                         int* num_rendered, cudaStream_t st, GaussianSide& g) {
   int rc;
   g.GL = gof_geom_layout((size_t)s->P);
   g.geom = (char*)geom_alloc(geom_user, g.GL.bytes);
   g.IL = gof_image_layout(s->width, s->height);
   g.img = (char*)image_alloc(image_user, g.IL.bytes);
   if (!g.geom || !g.img) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
-  if (tr) tr->mark("alloc geom+img");
 
   if ((rc = gof_launch_preprocess(s, v, g.geom, g.GL, radii, box_margin, st)) != GOF_OK) return rc;
   SideCopy* sc = s->debug ? nullptr : begin_async_read_u32(g.geom + g.GL.total, st);
@@ -303,12 +261,10 @@ static int gaussian_side(const gof_scene_t* s, const GofView& v, gof_alloc_fn ge
   rc = sc ? finish_async_read_u32(sc, &g.R) : gof_read_back(&g.R, g.geom + g.GL.total, sizeof(uint32_t), st);
   if (rc != GOF_OK) return rc;
   *num_rendered = (int)g.R;
-  if (tr) tr->mark("pre+sort, num_rendered");
 
   g.BL = gof_bin_layout((size_t)g.R, s->width, s->height, with_masks);
   g.bin = (char*)binning_alloc(binning_user, g.BL.bytes);
   if (!g.bin && g.BL.bytes) { gof_set_error("binning allocator returned NULL"); return GOF_E_ALLOC; }
-  if (tr) tr->mark("alloc binning");
   return gof_bin_tiles(s->P, (size_t)g.R, v, g.geom, g.GL, g.bin, g.BL, g.img, g.IL, s->debug != 0, st);
 }
 
@@ -342,14 +298,11 @@ extern "C" int gof_rasterize_forward(const gof_scene_t* s, gof_alloc_fn geom_all
   if (s->P == 0) return GOF_OK;   // rasterize_points.cu:85
   if (!out_color || !radii) { gof_set_error("out_color / radii must be non-NULL"); return GOF_E_INVALID; }
   const GofView v = gof_make_view(s);
-  GofTrace tr;
   GaussianSide g;
   if ((rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.0f, true,
-                          num_rendered, &tr, st, g)) != GOF_OK)
+                          num_rendered, st, g)) != GOF_OK)
     return rc;
-  if ((rc = gof_launch_render_forward(s, v, g.geom, g.GL, g.bin, g.BL, g.img, g.IL, out_color, st)) != GOF_OK) return rc;
-  tr.mark("launch bin+render");
-  return GOF_OK;
+  return gof_launch_render_forward(s, v, g.geom, g.GL, g.bin, g.BL, g.img, g.IL, out_color, st);
 }
 
 extern "C" int gof_rasterize_backward(const gof_scene_t* s, int num_rendered, const int* radii,
@@ -557,7 +510,7 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
   const GofView v = gof_make_view(s);
   GaussianSide g;
   if ((rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.5f, false,
-                          num_rendered, nullptr, st, g)) != GOF_OK)
+                          num_rendered, st, g)) != GOF_OK)
     return rc;
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
@@ -590,7 +543,7 @@ extern "C" int gof_integrate_prepare(const gof_scene_t* s, gof_alloc_fn geom_all
   const GofView v = gof_make_view(s);
   GaussianSide g{};
   if (s->P > 0 && (rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.5f,
-                                      false, num_rendered, nullptr, st, g)) != GOF_OK)
+                                      false, num_rendered, st, g)) != GOF_OK)
     return rc;
   const GofIntCacheLayout CL = gof_int_cache_layout((size_t)s->P, s->width, s->height, (size_t)g.R);
   char* cache = (char*)cache_alloc(cache_user, CL.bytes);

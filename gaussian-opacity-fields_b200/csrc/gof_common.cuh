@@ -60,8 +60,6 @@ int gof_sm_count();
 // returns the value it left in *value (may be NULL).  A setup that does not return GOF_OK runs again on the next call.
 // setup runs under the state's mutex and must not call these functions itself.
 int gof_device_once(const void* key, int (*setup)(int dev, int* value), int* value);
-// GOF_STATS=1: the current device's counters of the backward blend (pairs visited / evaluated / contributing); nullptr otherwise
-unsigned long long* gof_stats_buffer();
 
 // ---- shared-memory access with an explicit base register ----------------------------------------------
 // On sm_90 and later a shared address carries the CTA's rank in its cluster; ptxas re-derives that window base

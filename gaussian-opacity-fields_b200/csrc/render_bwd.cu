@@ -38,7 +38,6 @@ struct BwdArgs {
                        // the view2gaussian chain rule amplifies to percents in dL_dscale / dL_drot; the order moves a double
                        // sum only in its last bits, so after k_preprocess_backward's one rounding to float the gradients
                        // agree from run to run unless a sum lies that close to a float rounding boundary
-  unsigned long long* stats;   // optional [8] counters (GOF_STATS=1), else nullptr
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
@@ -77,11 +76,7 @@ __device__ __forceinline__ void quarter_reduce16(const float (&a)[16], int lane,
   }
 }
 
-// STATS (GOF_STATS=1): also count visits, pairs and reds into BwdArgs::stats.  That build is compiled for 3 resident CTAs
-// per SM, which leaves the counters 80 registers instead of 64.
-template <bool STATS>
-__global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backward(const BwdArgs a) {
-  unsigned long long st_visit = 0, st_eval = 0, st_pass = 0, st_contrib = 0, st_anyhit = 0, st_red = 0;
+__global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_backward(const BwdArgs a) {
   // rows of 96 bytes per staged Gaussian = GofSplat (64 B) | GofSplatBwd (32 B: means2D, 2D conic, own index); one row base
   // register serves every load of a visit (see gof_smem_base)
   extern __shared__ __align__(128) float4 s_dyn[];
@@ -172,7 +167,6 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
     // the 16 partial gradients of ONE (pixel, Gaussian) pair: row = the staged record, contributor = its zero-based index in the
     // tile list (the reference's `contributor` after its decrement, backward.cu:763), contrib = this pixel blended it
     auto pair_grad = [&](const uint32_t row, const uint32_t contributor, const bool contrib, float (&g)[16]) {
-      if (STATS) { st_eval += contrib; st_pass += contrib; }
       const float4 q0 = gof_lds128<0>(row), q1 = gof_lds128<16>(row), q2 = gof_lds128<32>(row);
       const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
       GofPair p;
@@ -186,7 +180,6 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
         G = F_EXP(power);
         alpha = fminf(F_MUL(q2.z, G), GOF_ALPHA_MAX);
       }
-      if (STATS) st_contrib += contrib;
 
 #pragma unroll
       for (int q = 0; q < 16; ++q) g[q] = 0.f;
@@ -203,8 +196,8 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
         T = T * r1a;
         const float w = alpha * T;
         // Every sum of two products below names the product that is fused (F_FMA) and the one that is rounded (F_MUL), as
-        // gof_math.cuh does for the forward: left to ptxas, the choice differs between instantiations of this kernel, and
-        // the view2gaussian chain rule turns the last-ulp difference into percents in dL_dscale / dL_drot.
+        // gof_math.cuh does for the forward: left to ptxas, the choice can change with any edit of this kernel, and the
+        // view2gaussian chain rule turns the last-ulp difference into percents in dL_dscale / dL_drot.
         // colour, :824-837
         const float2 q3 = gof_lds64<48>(row);
         const float c0 = q2.w, c1 = q3.x, c2 = q3.y;
@@ -307,7 +300,6 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
       if (act) qb &= ~(1u << b);
       const uint32_t row = s_base + (first + (uint32_t)b) * 96u;
       const bool contrib = act && ((mybits >> b) & 1u) != 0u;
-      if (STATS) { st_visit += (lane == 0); st_anyhit += act && !(lane & 11); }
       float g[16];
       pair_grad(row, (uint32_t)base + first + (uint32_t)b, contrib, g);
       float r0, r1;
@@ -317,29 +309,10 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, STATS ? 3 : 4) k_render_backwa
         double* dst = a.grad_acc + ((size_t)gid * 16 + ((lane & 8) ? 1 : 0) + ((lane & 2) ? 2 : 0) + ((lane & 1) ? 4 : 0));
         if (r0 != 0.f) atomicAdd(dst, (double)r0);
         if (r1 != 0.f) atomicAdd(dst + 8, (double)r1);
-        if (STATS) st_red += (r0 != 0.f) + (r1 != 0.f);
       }
       if (qb == 0u) next_group();
     }
   }
-  if (STATS && a.stats) {
-    atomicAdd(a.stats + 0, st_visit); atomicAdd(a.stats + 1, st_eval); atomicAdd(a.stats + 2, st_pass);
-    atomicAdd(a.stats + 3, st_contrib); atomicAdd(a.stats + 4, st_anyhit); atomicAdd(a.stats + 7, st_red);
-    if (threadIdx.x == 0) { atomicAdd(a.stats + 5, (unsigned long long)used); atomicAdd(a.stats + 6, (unsigned long long)(range.y - range.x)); }
-  }
-}
-
-template <bool STATS>
-int launch_backward(const BwdArgs& a, int tiles, cudaStream_t st) {
-  const int rc = gof_device_once((const void*)k_render_backward<STATS>, [](int, int*) -> int {
-    const int need = (STATS ? 3 : 4) * (SMEM_BYTES + 1024);   // only what the resident CTAs need: the rest stays L1
-    GOF_CUDA_OK(cudaFuncSetAttribute(k_render_backward<STATS>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                     (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
-    return GOF_OK;
-  }, nullptr);
-  if (rc != GOF_OK) return rc;
-  GOF_LAUNCH("render_bwd", st, k_render_backward<STATS><<<tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
-  return GOF_OK;
 }
 
 }  // namespace
@@ -362,9 +335,14 @@ int gof_launch_render_backward(const gof_scene_t* s, const GofView& v, char* geo
   a.vstride = BL.vmask_stride;
   a.grad_acc = reinterpret_cast<double*>(geom + GL.grad_acc);
   GOF_CUDA_OK(cudaMemsetAsync(a.grad_acc, 0, (size_t)s->P * 128, st));
-  a.stats = gof_stats_buffer();
-  const int rc = a.stats ? launch_backward<true>(a, v.tiles, st) : launch_backward<false>(a, v.tiles, st);
+  const int rc = gof_device_once((const void*)k_render_backward, [](int, int*) -> int {
+    const int need = 4 * (SMEM_BYTES + 1024);   // only what the resident CTAs need: the rest stays L1
+    GOF_CUDA_OK(cudaFuncSetAttribute(k_render_backward, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
+    return GOF_OK;
+  }, nullptr);
   if (rc != GOF_OK) return rc;
+  GOF_LAUNCH("render_bwd", st, k_render_backward<<<v.tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
   GOF_LAUNCH_CHECK(s->debug, st);
   return GOF_OK;
 }

@@ -289,11 +289,6 @@ GOF_API int gof_profile_report(char* buf, int cap);
 /* "<kernel> <start_ms> <end_ms>" per bracketed launch since the last reset (origin: the first of them): shows idle
  * gaps between launches.  Returns the bytes needed. */
 GOF_API int gof_profile_timeline(char* buf, int cap);
-/* GOF_STATS=1 only: copies the current device's 8 counters of the backward blend (each device keeps its own) to `out`
- * (host) and clears them; 0 if disabled.
- * [0] walk iterations, [1..3] pairs evaluated / passed / contributing, [4] (quarter-)warp visits, [5] list entries walked,
- * [6] list entries, [7] double atomics issued into the accumulator rows. */
-GOF_API int gof_stats_read(unsigned long long* out);
 
 /* The exchange step of view-parallel training (no reference counterpart: the reference is single-GPU): sum over
  * ranks of a flat f32 buffer over NVLink peer memory.  peers[r] = address, valid in THIS process, of rank r's buffer

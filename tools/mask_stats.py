@@ -4,7 +4,9 @@
 For one view of a config it answers: how many (pixel block, Gaussian) visits do the forward (box hits) and the backward
 (blocks with >= 1 blended pixel) make for block shapes 8x4 (a warp today), 4x4, 4x2 and 2x2 -- and how many warp iterations
 result if the sub-blocks of a warp walk INDEPENDENT lists in lockstep (max over the sub-blocks, per group of 32 list
-entries or per batch of 256).  Developer tool; prints one JSON line and writes tool_out/mask_stats_<cfg>.json."""
+entries or per batch of 256).  "backward_counters" is the work of the backward blend as built (k_render_backward: 4x2
+quarters in lockstep per batch of 256), counted from the masks it reads.  Developer tool; prints one JSON line and writes
+tool_out/mask_stats_<cfg>.json."""
 import json
 import os
 import sys
@@ -41,11 +43,15 @@ def main():
     tiles = gx * gy
     ranges = st["ranges"].to(torch.int64)                       # [tiles,2]
     lens = ranges[:, 1] - ranges[:, 0]
+    # groups of 32 and batches of 256 list entries are numbered densely over all tiles, from per-tile offsets
     ngroups = (lens + 31) // 32
-    G = int(ngroups.sum())
+    nbatches = (lens + 255) // 256
+    G, B = int(ngroups.sum()), int(nbatches.sum())
     tile_of_group = torch.repeat_interleave(torch.arange(tiles, device=dev), ngroups)
     first_group = torch.cumsum(ngroups, 0) - ngroups
+    first_batch = torch.cumsum(nbatches, 0) - nbatches
     g_in_tile = torch.arange(G, device=dev) - first_group[tile_of_group]
+    batch_of_group = first_batch[tile_of_group] + g_in_tile // 8
     gstart = ranges[tile_of_group, 0] + 32 * tile_of_group + 32 * g_in_tile      # word offset of lane 0
     vm = st["blend_masks"]                                                       # [8, R + 32*tiles]
     idx = gstart[:, None] + torch.arange(32, device=dev)[None, :]                # [G,32]
@@ -72,9 +78,6 @@ def main():
             acc = acc | sel[:, :, k]
         return acc                                                               # [8,G]
 
-    # batch id: (tile, g_in_tile // 8)
-    batch_id = tile_of_group * 64 + (g_in_tile // 8)
-    uniq, inv = torch.unique(batch_id, return_inverse=True)
     shapes = {"8x4": [lane >= 0], "4x4": [lx < 4, lx >= 4], "4x2": [(lx < 4) & (ly < 2), (lx >= 4) & (ly < 2), (lx < 4) & (ly >= 2), (lx >= 4) & (ly >= 2)],
               "2x2": [((lx // 2) == a) & ((ly // 2) == b) for a in range(4) for b in range(2)]}
     bw = {}
@@ -82,12 +85,20 @@ def main():
         cnts = torch.stack([popc(or_over(torch.nonzero(m).flatten())) for m in subs], 0)   # [S,8,G]
         visits = int(cnts.sum())
         lock_group = int(cnts.amax(dim=0).sum())
-        per_batch = torch.zeros(len(subs), 8, uniq.numel(), dtype=torch.int64, device=dev)
-        per_batch.index_add_(2, inv, cnts)
+        per_batch = torch.zeros(len(subs), 8, B, dtype=torch.int64, device=dev)
+        per_batch.index_add_(2, batch_of_group, cnts)
         lock_batch = int(per_batch.amax(dim=0).sum())
         bw[sname] = {"block_visits": visits, "warp_iters_lockstep_group32": lock_group, "warp_iters_lockstep_batch256": lock_batch,
                      "lanes_active_per_visit": out["pairs_blended"] / max(visits, 1) }
     out["backward"] = bw
+    # What k_render_backward does: warp_iterations (per tile, warp and batch, the most entries any quarter has in the
+    # batch), pairs evaluated, quarter_visits, entries_walked (per tile, the deepest entry any pixel blended, at most the
+    # list length), list_entries.  Each lane of a visiting quarter issues at most two reds and skips zero sums, so the
+    # double reds into the accumulator rows are at most 16 per quarter-visit.
+    walked = torch.minimum(pix_last.reshape(tiles, 256).amax(dim=1), lens)
+    out["backward_counters"] = {"warp_iterations": bw["4x2"]["warp_iters_lockstep_batch256"], "pairs": out["pairs_blended"],
+                                "quarter_visits": bw["4x2"]["block_visits"], "entries_walked": int(walked.sum()),
+                                "list_entries": int(lens.sum()), "reds_at_most": 16 * bw["4x2"]["block_visits"]}
 
     # ---- forward: alpha-support box hits per block shape, up to the block's saturation point -------------------------
     rec = geom[:P * 64].view(torch.int32).view(P, 16)
@@ -101,18 +112,16 @@ def main():
     tx, ty = (ent_tile % gx) * 16, (ent_tile // gx) * 16
     fw = {}
     pix_last_t = pad.view(gy, 16, gx, 16).permute(0, 2, 1, 3).reshape(tiles, 16, 16)        # [tile, y, x]
-    ent_group = ent_tile * 4096 + ent_pos // 32
-    ent_batch = ent_tile * 4096 + ent_pos // 256
-    ug, invg = torch.unique(ent_group, return_inverse=True)
-    ub, invb = torch.unique(ent_batch, return_inverse=True)
+    ent_group = first_group[ent_tile] + ent_pos // 32
+    ent_batch = first_batch[ent_tile] + ent_pos // 256
     for sname, (bwid, bhei) in {"8x4": (8, 4), "4x4": (4, 4), "4x2": (4, 2), "2x2": (2, 2)}.items():
         nbx, nby = 16 // bwid, 16 // bhei
         blast = pix_last_t.view(tiles, nby, bhei, nbx, bwid).amax(dim=(2, 4))      # [tiles, nby, nbx]: the block's last blended entry (1-based)
         hits_total = 0
         warps = 8
         per_warp_sub = (nbx * nby) // warps                                         # sub-blocks per warp
-        cnt_g = torch.zeros(nbx * nby, ug.numel(), dtype=torch.int64, device=dev)
-        cnt_b = torch.zeros(nbx * nby, ub.numel(), dtype=torch.int64, device=dev)
+        cnt_g = torch.zeros(nbx * nby, G, dtype=torch.int64, device=dev)
+        cnt_b = torch.zeros(nbx * nby, B, dtype=torch.int64, device=dev)
         for by in range(nby):
             for bx in range(nbx):
                 wx0, wy0 = tx + bx * bwid, ty + by * bhei
@@ -123,8 +132,8 @@ def main():
                 alive = ent_pos < blast[ent_tile, by, bx]
                 h = (hit & alive).to(torch.int64)
                 hits_total += int(h.sum())
-                cnt_g[by * nbx + bx].index_add_(0, invg, h)
-                cnt_b[by * nbx + bx].index_add_(0, invb, h)
+                cnt_g[by * nbx + bx].index_add_(0, ent_group, h)
+                cnt_b[by * nbx + bx].index_add_(0, ent_batch, h)
         # group the sub-blocks of one warp: 8x4 warp footprint = consecutive sub-blocks inside it
         def lock(cnt):
             # sub-block (by,bx) belongs to warp ((by*bhei)//4)*2 + (bx*bwid)//8
