@@ -427,4 +427,8 @@ int gof_launch_render_forward(const gof_scene_t* s, const GofView& v, const char
                               const GofImageLayout& IL, float* out_color, cudaStream_t st);
 int gof_launch_render_backward(const gof_scene_t* s, const GofView& v, char* geom,
                                const GofGeomLayout& GL, const char* bin, const GofBinLayout& BL,
-                               const char* img, const GofImageLayout& IL, const float* dL_dpix, cudaStream_t st);
+                               const char* img, const GofImageLayout& IL, const float* dL_dpix, double* rays,
+                               float* dL_dtan_fov, cudaStream_t st);
+// bytes of `rays` above: the ray-gradient pass (rays non-NULL) leaves [2][H][W] per-pixel dL/dr and [tiles][2] tile sums there,
+// and writes dL_dtan_fov [2]
+size_t gof_ray_grad_scratch_bytes(int W, int H);

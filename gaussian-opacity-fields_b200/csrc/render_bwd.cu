@@ -38,6 +38,7 @@ struct BwdArgs {
                        // the view2gaussian chain rule amplifies to percents in dL_dscale / dL_drot; the order moves a double
                        // sum only in its last bits, so after k_preprocess_backward's one rounding to float the gradients
                        // agree from run to run unless a sum lies that close to a float rounding boundary
+  double* drays;       // RAYS only: [2][H][W] dL/drx, dL/dry of every pixel | [tiles][2] the tile's sums of rx dL/drx, ry dL/dry
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
@@ -76,6 +77,11 @@ __device__ __forceinline__ void quarter_reduce16(const float (&a)[16], int lane,
   }
 }
 
+// RAYS (DESIGN.md 4.10): also differentiate the loss with respect to the pixel's ray r = (rx, ry, 1).  Each pair adds, in
+// float, what the gradients it already holds give through n = M r, AA = r.n and BB; each lane sums its pixel's terms in double
+// in the walk's own back-to-front order, so the per-pixel values and the tile sums involve no atomics.  RAYS = false is the
+// plain backward, compiled to the same instructions as before the template.
+template <bool RAYS>
 __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_backward(const BwdArgs a) {
   // rows of 96 bytes per staged Gaussian = GofSplat (64 B) | GofSplatBwd (32 B: means2D, 2D conic, own index); one row base
   // register serves every load of a visit (see gof_smem_base)
@@ -133,6 +139,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_backward(const Bwd
   float last_c0 = 0.f, last_c1 = 0.f, last_c2 = 0.f, acc_c0 = 0.f, acc_c1 = 0.f, acc_c2 = 0.f;
   float last_n0 = 0.f, last_n1 = 0.f, last_n2 = 0.f, acc_n0 = 0.f, acc_n1 = 0.f, acc_n2 = 0.f;
   const float ddelx_dx = 0.5f * a.W, ddely_dy = 0.5f * a.H;
+  double ray_x = 0.0, ray_y = 0.0;   // RAYS: this pixel's dL/drx, dL/dry
 
   // The 16 values of a pair's partial gradient g[] and of the accumulator row:
   //   0..9 -> dL_dview2gaussian[0..9] (9 = dL_dC also yields dL_dopacity = -2/opacity * that sum: both are
@@ -261,6 +268,13 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_backward(const Bwd
         g[6] = dB2 * rx;
         g[7] = dB2 * ry;
         g[8] = dB2;
+        if constexpr (RAYS) {
+          // dL/drx = dnrm . dn/drx (n = M r, first column of M) + dA n0 (AA = r.n at fixed n) + dB2 v6 (BB), likewise for ry
+          const float tx = F_FMA(dB2, v[6], F_FMA(dA, p.n0, F_FMA(dnrm2, v[2], F_FMA(dnrm1, v[1], F_MUL(dnrm0, v[0])))));
+          const float ty = F_FMA(dB2, v[7], F_FMA(dA, p.n1, F_FMA(dnrm2, v[4], F_FMA(dnrm1, v[3], F_MUL(dnrm0, v[1])))));
+          ray_x = D_ADD(ray_x, (double)tx);
+          ray_y = D_ADD(ray_y, (double)ty);
+        }
       }
     };
 
@@ -313,13 +327,79 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_backward(const Bwd
       if (qb == 0u) next_group();
     }
   }
+
+  if constexpr (RAYS) {
+    if (inside) { a.drays[pid] = ray_x; a.drays[HW + pid] = ray_y; }
+    // the tile's sums of rx dL/drx and ry dL/dry: a fixed shuffle tree per warp, then the eight warps in order
+    double sx = D_MUL((double)rx, ray_x), sy = D_MUL((double)ry, ray_y);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      sx = D_ADD(sx, __shfl_down_sync(0xffffffffu, sx, o));
+      sy = D_ADD(sy, __shfl_down_sync(0xffffffffu, sy, o));
+    }
+    __syncthreads();   // every warp is done with the staged records: their buffer takes the warp sums
+    double* const s_sum = reinterpret_cast<double*>(s_dyn);
+    if (lane == 0) { s_sum[2 * warp] = sx; s_sum[2 * warp + 1] = sy; }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+      double t = s_sum[threadIdx.x];
+#pragma unroll
+      for (int w = 1; w < WARPS; ++w) t = D_ADD(t, s_sum[2 * w + threadIdx.x]);
+      a.drays[2 * HW + 2 * (size_t)tile + threadIdx.x] = t;
+    }
+  }
+}
+
+// dL/dtan_fov from the tile sums of k_render_backward<true>: thread j adds tiles j, j + 1024, ... in index order, a fixed tree
+// joins the threads, and each sum is divided by tan_fov and rounded to float once.  rx = (px + 0.5 - W/2) 2 tan_fovx / W, so
+// d rx / d tan_fovx = rx / tan_fovx.
+constexpr int FOCAL_SUM_THREADS = 1024;
+__global__ void __launch_bounds__(FOCAL_SUM_THREADS) k_focal_grad_sum(int tiles, const double* __restrict__ partial, float tan_fovx,
+                                                                        float tan_fovy, float* __restrict__ dL_dtan_fov) {
+  __shared__ double s[2][FOCAL_SUM_THREADS];
+  double sx = 0.0, sy = 0.0;
+  for (int t = threadIdx.x; t < tiles; t += FOCAL_SUM_THREADS) {
+    sx = D_ADD(sx, partial[2 * (size_t)t]);
+    sy = D_ADD(sy, partial[2 * (size_t)t + 1]);
+  }
+  s[0][threadIdx.x] = sx;
+  s[1][threadIdx.x] = sy;
+  __syncthreads();
+#pragma unroll
+  for (int n = FOCAL_SUM_THREADS / 2; n > 0; n >>= 1) {
+    if ((int)threadIdx.x < n) {
+      s[0][threadIdx.x] = D_ADD(s[0][threadIdx.x], s[0][threadIdx.x + n]);
+      s[1][threadIdx.x] = D_ADD(s[1][threadIdx.x], s[1][threadIdx.x + n]);
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    dL_dtan_fov[0] = (float)(s[0][0] / (double)tan_fovx);
+    dL_dtan_fov[1] = (float)(s[1][0] / (double)tan_fovy);
+  }
+}
+
+template <bool RAYS>
+int carveout_once() {
+  return gof_device_once((const void*)k_render_backward<RAYS>, [](int, int*) -> int {
+    const int need = 4 * (SMEM_BYTES + 1024);   // only what the resident CTAs need: the rest stays L1
+    GOF_CUDA_OK(cudaFuncSetAttribute(k_render_backward<RAYS>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
+    return GOF_OK;
+  }, nullptr);
 }
 
 }  // namespace
 
+size_t gof_ray_grad_scratch_bytes(int W, int H) {
+  if (W <= 0 || H <= 0) return 0;
+  const size_t tiles = (size_t)((W + 15) / 16) * ((H + 15) / 16);
+  return (2 * (size_t)W * H + 2 * tiles) * sizeof(double);
+}
+
 int gof_launch_render_backward(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& GL,
                                const char* bin, const GofBinLayout& BL, const char* img, const GofImageLayout& IL,
-                               const float* dL_dpix, cudaStream_t st) {
+                               const float* dL_dpix, double* rays, float* dL_dtan_fov, cudaStream_t st) {
   BwdArgs a{};
   a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
   a.ranges = reinterpret_cast<const uint2*>(img + IL.ranges);
@@ -335,14 +415,20 @@ int gof_launch_render_backward(const gof_scene_t* s, const GofView& v, char* geo
   a.vstride = BL.vmask_stride;
   a.grad_acc = reinterpret_cast<double*>(geom + GL.grad_acc);
   GOF_CUDA_OK(cudaMemsetAsync(a.grad_acc, 0, (size_t)s->P * 128, st));
-  const int rc = gof_device_once((const void*)k_render_backward, [](int, int*) -> int {
-    const int need = 4 * (SMEM_BYTES + 1024);   // only what the resident CTAs need: the rest stays L1
-    GOF_CUDA_OK(cudaFuncSetAttribute(k_render_backward, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                     (need * 100 + 233471) / 233472 > 100 ? 100 : (need * 100 + 233471) / 233472));
+  if (rays == nullptr) {
+    const int rc = carveout_once<false>();
+    if (rc != GOF_OK) return rc;
+    GOF_LAUNCH("render_bwd", st, k_render_backward<false><<<v.tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
+    GOF_LAUNCH_CHECK(s->debug, st);
     return GOF_OK;
-  }, nullptr);
+  }
+  a.drays = rays;
+  const int rc = carveout_once<true>();
   if (rc != GOF_OK) return rc;
-  GOF_LAUNCH("render_bwd", st, k_render_backward<<<v.tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
+  GOF_LAUNCH("render_bwd_rays", st, k_render_backward<true><<<v.tiles, GOF_BLOCK_SIZE, SMEM_BYTES, st>>>(a));
+  GOF_LAUNCH_CHECK(s->debug, st);
+  GOF_LAUNCH("focal_grad_sum", st, k_focal_grad_sum<<<1, FOCAL_SUM_THREADS, 0, st>>>(v.tiles, rays + 2 * (size_t)v.W * v.H, s->tan_fovx,
+                                                                                     s->tan_fovy, dL_dtan_fov));
   GOF_LAUNCH_CHECK(s->debug, st);
   return GOF_OK;
 }

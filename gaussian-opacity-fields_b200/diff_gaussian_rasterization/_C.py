@@ -61,6 +61,10 @@ _lib.gof_rasterize_backward_camera_scratch_bytes.restype = ctypes.c_size_t
 _lib.gof_rasterize_backward_camera_scratch_bytes.argtypes = [ctypes.c_int]
 _lib.gof_rasterize_backward_camera.restype = ctypes.c_int
 _lib.gof_rasterize_backward_camera.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 20 + [ctypes.c_size_t, ctypes.c_void_p]
+_lib.gof_rasterize_backward_intrinsics_scratch_bytes.restype = ctypes.c_size_t
+_lib.gof_rasterize_backward_intrinsics_scratch_bytes.argtypes = [ctypes.c_int] * 3
+_lib.gof_rasterize_backward_intrinsics.restype = ctypes.c_int
+_lib.gof_rasterize_backward_intrinsics.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 21 + [ctypes.c_size_t, ctypes.c_void_p]
 _lib.gof_sh_grad_from_views.restype = ctypes.c_int
 _lib.gof_sh_grad_from_views.argtypes = [ctypes.c_int] * 3 + [_fp, ctypes.c_void_p, _fp, ctypes.c_void_p]
 _lib.gof_mark_visible.restype = ctypes.c_int
@@ -192,6 +196,10 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _scalar(x):
+    return float(x.detach()) if isinstance(x, torch.Tensor) else float(x)
+
+
 def _scene(keep, bg, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, v2g_precomp,
            viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset, H, W, sh, degree, campos,
            prefiltered, debug):
@@ -203,7 +211,9 @@ def _scene(keep, bg, means3D, colors, opacity, scales, rotations, scale_modifier
     s.D = int(degree)
     s.M = int(sh.size(1)) if (sh is not None and sh.numel() != 0 and sh.size(0) != 0) else 0
     s.width, s.height = int(W), int(H)
-    s.tan_fovx, s.tan_fovy = float(tan_fovx), float(tan_fovy)
+    # tan_fovx / tan_fovy: Python floats or one-element tensors (a tensor that requires grad carries the focal-length gradient,
+    # DESIGN.md 4.10).  Reading a CUDA tensor's value costs one synchronisation of the current stream per call.
+    s.tan_fovx, s.tan_fovy = _scalar(tan_fovx), _scalar(tan_fovy)
     s.kernel_size, s.scale_modifier = float(kernel_size), float(scale_modifier)
     for name, t in (("background", bg), ("means3D", means3D), ("shs", sh), ("colors_precomp", colors),
                     ("opacities", opacity), ("scales", scales), ("rotations", rotations),
@@ -247,11 +257,13 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
                                  cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                                  kernel_size, subpixel_offset, dL_dout_color, sh, degree, campos, geomBuffer, R,
-                                 binningBuffer, imageBuffer, debug, _out=None, _camera=False):
+                                 binningBuffer, imageBuffer, debug, _out=None, _camera=False, _intrinsics=False, _ray_map=False):
     """RasterizeGaussiansBackwardCUDA (rasterize_points.cu:124-211).  Returns, in the reference's order
     (:210): (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
     dL_drotations, dL_dview2gaussian).  `_camera=True` (extension, gof_rasterize_backward_camera) appends
-    dL_dviewmatrix and dL_dcampos, shaped like viewmatrix and campos."""
+    dL_dviewmatrix and dL_dcampos, shaped like viewmatrix and campos.  `_intrinsics=True` (extension,
+    gof_rasterize_backward_intrinsics) then appends dL_dtanfovx and dL_dtanfovy, 0-dim float32 tensors on the device.
+    `_ray_map=True` (tests only; needs _intrinsics) appends the per-pixel float64 [2,H,W] dL/drx, dL/dry of the call."""
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
     keep = []
@@ -274,6 +286,10 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     factored = _out is not None and "dsh_rgb" in _out
     if factored and _camera:
         raise NotImplementedError("gof_b200: camera gradients are not available with the factored SH gradient (_out['dsh_rgb'])")
+    if factored and _intrinsics:
+        raise NotImplementedError("gof_b200: focal-length gradients are not available with the factored SH gradient (_out['dsh_rgb'])")
+    if _ray_map and not _intrinsics:
+        raise RuntimeError("gof_b200: _ray_map needs _intrinsics=True")
     if factored:
         rgb_t, hdr_t = _out["dsh_rgb"], _out.get("sh_hdr")
         if sh is None or sh.numel() == 0:
@@ -328,7 +344,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             raise RuntimeError("gof_b200: camera gradients need a 16-element viewmatrix and a 3-element campos")
         cam_out = torch.empty(19, dtype=torch.float32, device=means3D.device)
         dL_dviewmatrix, dL_dcampos = cam_out[:16], cam_out[16:]
-    if P != 0 or _camera:   # with P == 0 the camera entry point writes zeros
+    if _intrinsics:
+        fov_out = torch.empty(2, dtype=torch.float32, device=means3D.device)
+    if P != 0 or _camera or _intrinsics:   # with P == 0 the camera and intrinsics entry points write zeros
         g = dL_dout_color.contiguous()
         rad = radii.contiguous()
         with torch.cuda.device(means3D.device):
@@ -347,7 +365,13 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                       (_ptr(full_t) if full_t is not None else None) if factored else _ptr(dL_dsh),
                       dL_dscales.data_ptr(), dL_drotations.data_ptr(), dL_dv2g.data_ptr(),
                       ds.data_ptr() if ds is not None else None, dm.data_ptr() if dm is not None else None)
-            if _camera:
+            if _intrinsics:
+                nbytes = int(_lib.gof_rasterize_backward_intrinsics_scratch_bytes(P, W, H))
+                scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=means3D.device)
+                _check(_lib.gof_rasterize_backward_intrinsics(*common, dL_dviewmatrix.data_ptr() if _camera else None,
+                                                              dL_dcampos.data_ptr() if _camera else None, fov_out.data_ptr(),
+                                                              scratch.data_ptr() if nbytes else None, nbytes, _stream()))
+            elif _camera:
                 nbytes = int(_lib.gof_rasterize_backward_camera_scratch_bytes(P))
                 scratch = torch.empty(nbytes, dtype=torch.uint8, device=means3D.device)
                 _check(_lib.gof_rasterize_backward_camera(*common, dL_dviewmatrix.data_ptr(), dL_dcampos.data_ptr(),
@@ -358,6 +382,15 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations, dL_dv2g)
     if _camera:
         grads += (dL_dviewmatrix.view(viewmatrix.shape), dL_dcampos.view(campos.shape))
+    if _intrinsics:
+        grads += (fov_out[0], fov_out[1])
+    if _ray_map:
+        # the per-pixel [2][H][W] doubles follow the camera pass's rows in the scratch (api.cu, intrinsics_camera_bytes)
+        if P == 0:
+            grads += (torch.zeros((2, H, W), dtype=torch.float64, device=means3D.device),)
+        else:
+            off = nbytes - 16 * (W * H + ((W + 15) // 16) * ((H + 15) // 16))
+            grads += (scratch[off:off + 16 * W * H].view(torch.float64).view(2, H, W),)
     return grads
 
 
@@ -451,7 +484,7 @@ def integrate_points_cached(cache, background, points3D, viewmatrix, tan_fovx, t
     dev = cache.buffer.device
     s = _Scene()
     s.P, s.width, s.height = cache.P, cache.W, cache.H
-    s.tan_fovx, s.tan_fovy = float(tan_fovx), float(tan_fovy)
+    s.tan_fovx, s.tan_fovy = _scalar(tan_fovx), _scalar(tan_fovy)
     bg, vm, p3 = _c(background), _c(viewmatrix), _c(points3D)
     s.background, s.viewmatrix, s.debug = _ptr(bg, device=dev), _ptr(vm, device=dev), int(bool(debug))
     PN = p3.size(0)

@@ -26,7 +26,7 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
 class GaussianRasterizationSettings(NamedTuple):
     image_height: int
     image_width: int
-    tanfovx: float
+    tanfovx: float          # or a one-element tensor (extension): one that requires grad receives the focal-length gradient
     tanfovy: float
     kernel_size: float
     subpixel_offset: torch.Tensor
@@ -69,15 +69,34 @@ def _camera_inputs(rs):
     return ()
 
 
+def _intrinsics_inputs(rs):
+    """(tanfovx, tanfovy) when autograd is to differentiate the render with respect to the focal length (either is a tensor that
+    requires grad), otherwise ()."""
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rs.tanfovx, rs.tanfovy)):
+        return (rs.tanfovx, rs.tanfovy)
+    return ()
+
+
+def _extra_inputs(rs):
+    """The inputs of _RasterizeGaussians after grad_bucket: today's (viewmatrix, campos) or nothing, and, when the focal length
+    is to receive gradients, (tanfovx, tanfovy) after them."""
+    cam, fov = _camera_inputs(rs), _intrinsics_inputs(rs)
+    return (cam or (None, None)) + fov if fov else cam
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                view2gaussian_precomp, raster_settings, grad_bucket=None, viewmatrix=None, campos=None):
-        """viewmatrix / campos (extension): raster_settings' own camera tensors, passed as inputs only when they are to
-        receive gradients (the render reads them from raster_settings either way)."""
+                view2gaussian_precomp, raster_settings, grad_bucket=None, viewmatrix=None, campos=None, tanfovx=None,
+                tanfovy=None):
+        """viewmatrix / campos, tanfovx / tanfovy (extension): raster_settings' own camera tensors, passed as inputs only
+        when they are to receive gradients (the render reads them from raster_settings either way)."""
         rs = raster_settings
         ctx.grad_bucket = grad_bucket
         ctx.camera = viewmatrix is not None
+        ctx.intrinsics = tanfovx is not None
+        # shape, dtype and device of each tan_fov input that is a tensor: its gradient is returned like it
+        ctx.fov_like = [(t.shape, t.dtype, t.device) if isinstance(t, torch.Tensor) else None for t in (tanfovx, tanfovy)]
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
                 view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, sh, rs.sh_degree,
                                                              rs.campos, rs.prefiltered, rs.debug)
@@ -102,6 +121,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         kw = {"_out": bucket.views} if bucket is not None else {}
         if ctx.camera:
             kw["_camera"] = True
+        if ctx.intrinsics:
+            kw["_intrinsics"] = True
         grads = _call_native(_C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", "backward", **kw)
         (g_means2D, g_colors, g_opacity, g_means3D, g_cov3D, g_sh, g_scales, g_rot, g_v2g) = grads[:9]
         if bucket is not None:
@@ -112,17 +133,24 @@ class _RasterizeGaussians(torch.autograd.Function):
         # one gradient per forward input, in input order (reference :152-163)
         out = (g_means3D, g_means2D, g_sh, g_colors, g_opacity, g_scales, g_rot, g_cov3D, g_v2g, None, None)
         if ctx.camera:
-            out += tuple(g if need else None for g, need in zip(grads[9:], ctx.needs_input_grad[11:]))
+            out += tuple(g if need else None for g, need in zip(grads[9:11], ctx.needs_input_grad[11:13]))
+        if ctx.intrinsics:
+            if not ctx.camera:
+                out += (None, None)
+            out += tuple(g.to(dtype=like[1], device=like[2]).reshape(like[0]) if need and like is not None else None
+                         for g, like, need in zip(grads[-2:], ctx.fov_like, ctx.needs_input_grad[13:15]))
         return out
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         view2gaussian_precomp, raster_settings):
     """With grad mode on and raster_settings.viewmatrix or .campos requiring grad, the backward also differentiates the
-    render with respect to them (DESIGN.md 4.9); projmatrix is treated as a constant."""
+    render with respect to them (DESIGN.md 4.9); projmatrix is treated as a constant.  Likewise for raster_settings.tanfovx /
+    .tanfovy given as tensors that require grad (DESIGN.md 4.10): their gradients come back in their shape, dtype and
+    device."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                      cov3Ds_precomp, view2gaussian_precomp, raster_settings, None,
-                                     *_camera_inputs(raster_settings))
+                                     *_extra_inputs(raster_settings))
 
 
 def _absent():
@@ -164,6 +192,8 @@ class GaussianRasterizer(nn.Module):
         if self.grad_bucket is not None:
             if _camera_inputs(self.raster_settings):
                 raise NotImplementedError("camera gradients (viewmatrix / campos requiring grad) are not available with a grad_bucket")
+            if _intrinsics_inputs(self.raster_settings):
+                raise NotImplementedError("focal-length gradients (tanfovx / tanfovy requiring grad) are not available with a grad_bucket")
             return _RasterizeGaussians.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                              cov3D_precomp, view2gaussian_precomp, self.raster_settings, self.grad_bucket)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,

@@ -133,6 +133,23 @@ GOF_API int gof_rasterize_backward_camera(const gof_scene_t* scene, int num_rend
                            float* dens_max, float* dL_dviewmatrix /*[16]*/, float* dL_dcampos /*[3]*/, void* scratch,
                            size_t scratch_bytes, void* stream);
 
+/* gof_rasterize_backward_camera that also differentiates the loss with respect to the focal length (no reference counterpart;
+ * DESIGN section 4.10).  dL_dtan_fov [2] gets dL/dtan_fovx, dL/dtan_fovy through the pixel rays r = ((p + 0.5) - S/2) / focal
+ * of the blend: (1 / tan_fov) * sum over the pixels of rx dL/drx (ry dL/dry), where dL/dr is the derivative the blend backward
+ * assigns.  Each pixel's terms are summed in double in its back-to-front order and the pixels in a fixed order, with no atomics:
+ * bit-reproducible from call to call.  The 2D mip-filter coefficient, means2D, the tile binning and the culling boxes are
+ * constants.  dL_dviewmatrix / dL_dcampos: both (the camera gradient, as above) or neither (the plain preprocess backward).
+ * scratch: gof_rasterize_backward_intrinsics_scratch_bytes(P, width, height) device bytes (16 per pixel, plus the camera
+ * pass's rows), 8-byte aligned, contents irrelevant; it holds the per-pixel [2][H][W] double dL/drx, dL/dry after the call.
+ * P == 0 writes zeros.  dL_dtan_fov NULL, or a scratch NULL or too small, fails with GOF_E_INVALID. */
+GOF_API size_t gof_rasterize_backward_intrinsics_scratch_bytes(int P, int width, int height);
+GOF_API int gof_rasterize_backward_intrinsics(const gof_scene_t* scene, int num_rendered, const int* radii, void* geom_buffer,
+                           const void* binning_buffer, const void* image_buffer, const float* dL_dpix, float* dL_dmean2D,
+                           float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                           float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dens_sum,
+                           float* dens_max, float* dL_dviewmatrix /*[16] or NULL*/, float* dL_dcampos /*[3] or NULL*/,
+                           float* dL_dtan_fov /*[2]*/, void* scratch, size_t scratch_bytes, void* stream);
+
 /* View-parallel training (one view per GPU, gradients summed over the GPUs; no reference counterpart -- the reference is
  * single-GPU).  The SH gradient of ONE view is an outer product: dL_dsh[g][k][c] = w_k(dir(mean_g, camera)) * dL_dRGB[g][c]
  * (backward.cu:45-139), so the ranks exchange the 3 floats of the clamp-masked dL_dRGB per Gaussian and view instead of the
