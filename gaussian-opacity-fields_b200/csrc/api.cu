@@ -553,6 +553,68 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
                     out_color_integrated, st);
 }
 
+extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
+
+extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
+                                      void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
+                                      void* point_binning_buffer, const float* dL_dalpha, float* dL_dpoints3D, float* dL_dopacity,
+                                      float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
+                                      void* scratch, size_t scratch_bytes, void* stream) {
+  int rc = validate_scene(s);
+  if (rc != GOF_OK) return rc;
+  if (PN < 0) { gof_set_error("integrate_backward: PN < 0"); return GOF_E_INVALID; }
+  const size_t need = gof_integrate_backward_scratch(s->P);
+  if (scratch_bytes < need) {
+    gof_set_error("integrate_backward: scratch of %zu bytes, %zu needed (gof_integrate_backward_scratch_bytes)", scratch_bytes, need);
+    return GOF_E_INVALID;
+  }
+  if (s->P > 0 && !scratch) { gof_set_error("integrate_backward: scratch is NULL"); return GOF_E_INVALID; }
+  const size_t P = (size_t)s->P;
+  if ((PN > 0 && !dL_dalpha) || (P > 0 && (!dL_dopacity || !dL_dmean3D || !dL_dview2gaussian))) {
+    gof_set_error("integrate_backward: NULL argument");
+    return GOF_E_INVALID;
+  }
+  if (s->scales && s->rotations && P > 0 && (!dL_dscale || !dL_drot)) {
+    gof_set_error("integrate_backward: dL_dscale / dL_drot required");
+    return GOF_E_INVALID;
+  }
+  if (reinterpret_cast<uintptr_t>(dL_drot) & 15) {   // k_preprocess_backward writes each rotation gradient as one float4
+    gof_set_error("integrate_backward: dL_drot must be 16-byte aligned");
+    return GOF_E_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (P == 0 || PN == 0) {   // gof_integrate ran nothing: no alpha depends on anything
+    if (dL_dpoints3D && PN > 0) GOF_CUDA_OK(cudaMemsetAsync(dL_dpoints3D, 0, (size_t)PN * 12, st));
+    if (P > 0) {
+      GOF_CUDA_OK(cudaMemsetAsync(dL_dopacity, 0, P * 4, st));
+      GOF_CUDA_OK(cudaMemsetAsync(dL_dmean3D, 0, P * 12, st));
+      GOF_CUDA_OK(cudaMemsetAsync(dL_dview2gaussian, 0, P * 40, st));
+      if (dL_dscale) GOF_CUDA_OK(cudaMemsetAsync(dL_dscale, 0, P * 12, st));
+      if (dL_drot) GOF_CUDA_OK(cudaMemsetAsync(dL_drot, 0, P * 16, st));
+      if (dL_dcov3D) GOF_CUDA_OK(cudaMemsetAsync(dL_dcov3D, 0, P * 24, st));
+    }
+    return GOF_OK;
+  }
+  if (!points3D || !radii || !geom_buffer || !image_buffer || !point_buffer || !point_binning_buffer ||
+      (num_rendered > 0 && !binning_buffer) || num_rendered < 0) {
+    gof_set_error("integrate_backward: NULL forward state");
+    return GOF_E_INVALID;
+  }
+  const GofView v = gof_make_view(s);
+  const GofGeomLayout GL = gof_geom_layout(P);
+  const GofImageLayout IL = gof_image_layout(s->width, s->height);
+  const GofBinLayout BL = gof_bin_layout((size_t)num_rendered, s->width, s->height, false);
+  const GofPointLayout PL = gof_point_layout((size_t)PN);
+  const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count());
+  char* geom = static_cast<char*>(geom_buffer);
+  return gof_launch_integrate_backward(s, v, PN, points3D, radii, geom, GL,
+                                       reinterpret_cast<const uint32_t*>(static_cast<const char*>(binning_buffer) + BL.point_list),
+                                       reinterpret_cast<const uint2*>(static_cast<const char*>(image_buffer) + IL.ranges),
+                                       static_cast<const char*>(point_buffer), PL, static_cast<char*>(point_binning_buffer), PBL,
+                                       dL_dalpha, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale, dL_drot, dL_dview2gaussian,
+                                       dL_dcov3D, scratch, st);
+}
+
 // ---- the Gaussian side of the query, once per view --------------------------------------------------------------
 // extract_mesh.py calls integrate for the same 64 views 10 times (evaluage_alpha on the tetrahedra vertices, 8 bisection
 // steps, optionally the colours: extract_mesh.py:56,92,107) and only the query points change: preprocess, depth sort,

@@ -303,7 +303,7 @@ int sort_pairs(KeyT* ka, KeyT* kb, uint32_t* va, uint32_t* vb, uint32_t* scratch
   GOF_LAUNCH("radix_hist", st, k_digit_hist<KeyT><<<grid, THREADS, 0, st>>>(ka, n, dg, sc.ghist));
   GOF_LAUNCH_CHECK(debug, st);
   const int rc = onesweep_passes<KeyT>(ka, kb, va, vb, n, dg, sc, debug, st);
-  *result_in_b = dg.passes % 2;
+  *result_in_b = gof_radix_result_in_b(nbits);
   return rc;
 }
 
@@ -500,6 +500,13 @@ __global__ void __launch_bounds__(THREADS) k_run_heads(size_t n, const GofKeyWor
 }
 
 }  // namespace
+
+// every pass moves the pairs to the other buffers
+int gof_radix_result_in_b(int nbits) {
+  Digits dg;
+  split_digits(nbits, &dg);
+  return dg.passes % 2;
+}
 
 // Stable sort of the P (depth bits, gaussian id) pairs written by the preprocess kernel into key_a/val_a; 4 passes ->
 // result back in *_a.  (The scan of tiles_touched in that order happens inside the emit kernel, gof_bin_tiles.)

@@ -297,7 +297,8 @@ static inline int gof_bits_for(uint32_t n) {   // bits needed to represent value
   return b < 1 ? 1 : b;
 }
 
-// with_masks = false: the opacity-field query has no backward, its binning buffer carries no blend masks
+// with_masks = false: the opacity-field query's binning buffer carries no blend masks (its backward recomputes its
+// contributor lists instead)
 static inline GofBinLayout gof_bin_layout(size_t R, int W, int H, bool with_masks = true) {
   const uint32_t tiles = (uint32_t)((W + 15) / 16) * (uint32_t)((H + 15) / 16);
   GofBinLayout L;
@@ -384,6 +385,9 @@ int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLa
                   const GofBinLayout& BL, char* img, const GofImageLayout& IL, bool debug, cudaStream_t st);
 int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist,
                             uint2* ranges, int num_tiles, bool debug, cudaStream_t st, int* result_in_b);
+// *result_in_b of a radix sort of n > 0 pairs over nbits key bits (gof_sort_points_by_tile, gof_bin_tiles): 1 when the sorted pairs
+// end in the b buffers
+int gof_radix_result_in_b(int nbits);
 
 // integrate.cu
 struct GofPointLayout { size_t xy, depth, bytes; };
@@ -409,6 +413,15 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
                          const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, char* pts,
                          const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, float* out_color, float* out_alpha,
                          float* out_color_int, cudaStream_t st);
+// The backward of the query (DESIGN.md 4.11) from the state gof_launch_integrate left in geom / pts / pbin: dL_dalpha [PN] ->
+// dL_dpoints3D [PN][3] (optional) and, through the accumulator rows and k_preprocess_backward, the Gaussian gradients.  The
+// contributor slab in pbin and the accumulator rows in geom are rewritten.  scratch: gof_integrate_backward_scratch(P) bytes.
+size_t gof_integrate_backward_scratch(int P);
+int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const int* radii,
+                                  char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
+                                  const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
+                                  float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot,
+                                  float* dL_dv2g, float* dL_dcov3D, void* scratch, cudaStream_t st);
 
 // Per-view cache of the Gaussian side of the opacity-field query (gof_integrate_prepare / gof_integrate_cached): the records,
 // the tile ranges and the per-tile Gaussian lists are all a query needs, and they do not depend on the query points.

@@ -411,6 +411,21 @@ def integrate_gaussians_to_points(background, points3D, means3D, colors, opacity
                                   degree, campos, prefiltered, debug):
     """IntegrateGaussiansToPointsCUDA (rasterize_points.cu:234-343).  Returns (num_rendered, out_color,
     out_alpha_integrated, out_color_integrated, radii, geomBuffer, binningBuffer, imgBuffer)."""
+    return _integrate(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                      view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset,
+                      image_height, image_width, sh, degree, campos, prefiltered, debug)[:8]
+
+
+def integrate_gaussians_to_points_state(*args):
+    """integrate_gaussians_to_points (same arguments) that also returns the point-side buffers the backward reads:
+    (num_rendered, out_color, out_alpha_integrated, out_color_integrated, radii, geomBuffer, binningBuffer, imgBuffer,
+    pointBuffer, pointBinningBuffer) -- together the forward state of integrate_gaussians_to_points_backward."""
+    return _integrate(*args)
+
+
+def _integrate(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+               view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset, image_height,
+               image_width, sh, degree, campos, prefiltered, debug):
     if points3D.ndimension() != 2 or points3D.size(1) != 3:
         raise RuntimeError("points3D must have dimensions (num_points, 3)")
     keep = []
@@ -433,7 +448,60 @@ def integrate_gaussians_to_points(background, points3D, means3D, colors, opacity
             _check(_lib.gof_integrate(ctypes.byref(s), PN, _ptr(p3), geom.cb, None, binning.cb, None, img.cb, None,
                                       pts.cb, None, pbin.cb, None, out_color.data_ptr(), radii.data_ptr(),
                                       alpha_int.data_ptr(), color_int.data_ptr(), ctypes.byref(rendered), _stream()))
-    return rendered.value, out_color, alpha_int, color_int, radii, geom.tensor, binning.tensor, img.tensor
+    return (rendered.value, out_color, alpha_int, color_int, radii, geom.tensor, binning.tensor, img.tensor, pts.tensor,
+            pbin.tensor)
+
+
+_lib.gof_integrate_backward_scratch_bytes.restype = ctypes.c_size_t
+_lib.gof_integrate_backward_scratch_bytes.argtypes = [ctypes.c_int]
+_lib.gof_integrate_backward.restype = ctypes.c_int
+_lib.gof_integrate_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 15 + \
+    [ctypes.c_size_t, ctypes.c_void_p]
+
+
+def integrate_gaussians_to_points_backward(background, points3D, means3D, radii, colors, scales, rotations, scale_modifier,
+                                           cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                                           kernel_size, subpixel_offset, image_height, image_width, sh, degree, campos,
+                                           dL_dalpha, num_rendered, geomBuffer, binningBuffer, imgBuffer, pointBuffer,
+                                           pointBinningBuffer, debug, points_grad=True):
+    """gof_integrate_backward (extension, DESIGN.md 4.11): the gradient dL_dalpha [PN] of out_alpha_integrated ->
+    (dL_dpoints3D [PN,3] or None, dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drotations [P,4],
+    dL_dcov3D [P,6], dL_dview2gaussian [P,10]).  The state is what integrate_gaussians_to_points_state returned."""
+    P, PN = means3D.size(0), points3D.size(0)
+    keep = []
+    s = _scene(keep, background, means3D, colors, means3D, scales, rotations, scale_modifier, cov3D_precomp,
+               view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset, image_height,
+               image_width, sh, degree, campos, False, debug)
+    dev = means3D.device
+    # one block for the six outputs, each a 256-byte aligned view (64-float padding, as in rasterize_gaussians_backward): the
+    # rotation gradient is written with 16-byte stores
+    sizes = dict(dopacity=1, dmeans3D=3, dscales=3, drot=4, dcov3D=6, dv2g=10)
+    offs, total = {}, 0
+    for k, n in sizes.items():
+        offs[k] = total
+        total += (P * n + 63) // 64 * 64
+    block = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
+    out = {k: block[offs[k]:offs[k] + P * n].view(P, n) for k, n in sizes.items()}
+    dpts = torch.empty((PN, 3), dtype=torch.float32, device=dev) if points_grad else None
+    nbytes = int(_lib.gof_integrate_backward_scratch_bytes(P))
+    scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    p3, g = _c(points3D), _c(dL_dalpha)
+    if g.numel() != PN:
+        raise RuntimeError(f"gof_b200: dL_dalpha has {g.numel()} elements, expected {PN}")
+    has_sr = s.scales is not None and s.rotations is not None
+    buf = lambda t: t.data_ptr() if t is not None and t.numel() else None   # noqa: E731
+    with torch.cuda.device(dev):
+        _check(_lib.gof_integrate_backward(
+            ctypes.byref(s), PN, _ptr(p3, device=dev), int(num_rendered), _ptr(radii.contiguous(), torch.int32),
+            buf(geomBuffer), buf(binningBuffer), buf(imgBuffer), buf(pointBuffer), buf(pointBinningBuffer), _ptr(g, device=dev),
+            dpts.data_ptr() if dpts is not None and PN else None, out["dopacity"].data_ptr() if P else None,
+            out["dmeans3D"].data_ptr() if P else None, out["dscales"].data_ptr() if P and has_sr else None,
+            out["drot"].data_ptr() if P and has_sr else None, out["dv2g"].data_ptr() if P else None,
+            out["dcov3D"].data_ptr() if P else None, scratch.data_ptr() if nbytes else None, nbytes, _stream()))
+    if P and not has_sr:
+        out["dscales"].zero_()
+        out["drot"].zero_()
+    return dpts, out["dopacity"], out["dmeans3D"], out["dscales"], out["drot"], out["dcov3D"], out["dv2g"]
 
 
 _lib.gof_integrate_cache_bytes.restype = ctypes.c_size_t

@@ -8,6 +8,7 @@ Same import surface as the reference package of the same name
 * GaussianRasterizationSettings -- NamedTuple, same fields in the same order (reference :167-181)
 * GaussianRasterizer(raster_settings).forward / .integrate / .markVisible (reference :183-305)
 * rasterize_gaussians(...) and the autograd Function _RasterizeGaussians (reference :21-165)
+* integrate_gaussians(...) (extension): the opacity-field query with alpha_integrated differentiable (_IntegrateGaussians)
 
 so gaussian_renderer/__init__.py:14,99-108,199-209 of the reference runs unmodified on top of it.
 The native side is libgof_b200.so (hand-written sm_90a CUDA, C ABI in include/gof_rasterizer.h) reached
@@ -20,7 +21,7 @@ import torch.nn as nn
 
 from . import _C
 
-__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians"]
+__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "integrate_gaussians"]
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -151,6 +152,72 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                      cov3Ds_precomp, view2gaussian_precomp, raster_settings, None,
                                      *_extra_inputs(raster_settings))
+
+
+def _integrate_args(rs, points3D, means3D, colors_precomp, opacities, scales, rotations, cov3D_precomp, view2gaussian_precomp, shs):
+    return (rs.bg, points3D, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3D_precomp,
+            view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, shs, rs.sh_degree, rs.campos,
+                                                         rs.prefiltered, rs.debug)
+
+
+class _IntegrateGaussians(torch.autograd.Function):
+    """The opacity-field query with alpha_integrated differentiable with respect to points3D, means3D, opacities, scales,
+    rotations and view2gaussian_precomp (DESIGN.md 4.11).  color, color_integrated and radii carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, points3D, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                view2gaussian_precomp, raster_settings):
+        rs = raster_settings
+        args = _integrate_args(rs, points3D, means3D, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+                               view2gaussian_precomp, shs)
+        (num_rendered, color, alpha_integrated, color_integrated, radii, geom, binning, img, pts, pbin) = _call_native(
+            _C.integrate_gaussians_to_points_state, args, rs.debug, "snapshot_fw.dump", "forward")
+        ctx.raster_settings = rs
+        ctx.num_rendered = num_rendered
+        ctx.save_for_backward(points3D, means3D, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp, shs,
+                              radii, geom, binning, img, pts, pbin)
+        ctx.mark_non_differentiable(color, color_integrated, radii)
+        return color, alpha_integrated, color_integrated, radii
+
+    @staticmethod
+    def backward(ctx, _grad_color, grad_alpha, _grad_color_integrated, _grad_radii):
+        rs = ctx.raster_settings
+        (points3D, means3D, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp, shs, radii, geom, binning, img,
+         pts, pbin) = ctx.saved_tensors
+        if grad_alpha is None:
+            grad_alpha = torch.zeros(points3D.size(0), dtype=torch.float32, device=points3D.device)
+        args = (rs.bg, points3D, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3D_precomp,
+                view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, shs, rs.sh_degree, rs.campos,
+                                                             grad_alpha, ctx.num_rendered, geom, binning, img, pts, pbin, rs.debug)
+        g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g = _call_native(
+            _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
+            points_grad=ctx.needs_input_grad[0])
+        need = ctx.needs_input_grad
+        pick = lambda g, i: g if need[i] else None   # noqa: E731
+        return (pick(g_pts, 0), pick(g_means3D, 1), None, pick(g_opacity, 3), None, None, pick(g_scales, 6), pick(g_rot, 7),
+                pick(g_cov3D, 8), pick(g_v2g, 9), None)
+
+
+def integrate_gaussians(points3D, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                        view2gaussian_precomp, raster_settings):
+    """GaussianRasterizer.integrate with alpha_integrated differentiable (extension, DESIGN.md 4.11): returns the same
+    (color[9,H,W], alpha_integrated[PN], color_integrated[PN,3], radii[P]).  Optional inputs are None or empty tensors, as
+    for rasterize_gaussians.  With grad mode off, or with no input requiring grad, this is GaussianRasterizer.integrate."""
+    shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp = _normalise_optionals(
+        None if shs is None or shs.numel() == 0 else shs, None if colors_precomp is None or colors_precomp.numel() == 0 else colors_precomp,
+        None if scales is None or scales.numel() == 0 else scales, None if rotations is None or rotations.numel() == 0 else rotations,
+        None if cov3D_precomp is None or cov3D_precomp.numel() == 0 else cov3D_precomp,
+        None if view2gaussian_precomp is None or view2gaussian_precomp.numel() == 0 else view2gaussian_precomp)
+    inputs = (points3D, means3D, opacities, scales, rotations, cov3D_precomp, view2gaussian_precomp)
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs):
+        return _IntegrateGaussians.apply(points3D, means3D, means2D, opacities, shs, colors_precomp, scales, rotations,
+                                         cov3D_precomp, view2gaussian_precomp, raster_settings)
+    rs = raster_settings
+    (_num_rendered, color, alpha_integrated, color_integrated, radii, _g, _b, _i) = _call_native(
+        _C.integrate_gaussians_to_points, _integrate_args(rs, points3D, means3D, colors_precomp, opacities, scales, rotations,
+                                                          cov3D_precomp, view2gaussian_precomp, shs),
+        rs.debug, "snapshot_fw.dump", "forward")
+    return color, alpha_integrated, color_integrated, radii
 
 
 def _absent():

@@ -185,6 +185,24 @@ GOF_API int gof_integrate(const gof_scene_t* scene, int PN, const float* points3
                   float* out_alpha_integrated, float* out_color_integrated,
                   int* num_rendered, void* stream);
 
+/* The backward of gof_integrate (no reference counterpart; DESIGN section 4.11): dL_dalpha [PN], the gradient of a loss with respect
+ * to out_alpha_integrated, -> the gradients with respect to the points and the Gaussians.  With each point's contributor list,
+ * the alpha rejects and the alpha and depth clamps held fixed, d alpha_integrated / d alpha_j = prod_{i != j} (1 - alpha_i).
+ * The forward's state is everything gof_integrate left through its allocators (geometry, binning, image, point and point
+ * binning buffers) with its radii and num_rendered; the call rewrites the contributor lists in the point binning buffer and
+ * the accumulator rows in the geometry buffer, and reads the rest.  dL_dpoints3D [PN,3] (NULL: not computed) is formed per
+ * point in double and rounded once, with no atomics: bit-reproducible.  The Gaussian outputs are those of
+ * gof_rasterize_backward for the same scene (dL_dscale / dL_drot required with scales and rotations, dL_drot 16-byte aligned,
+ * dL_dcov3D [P,6] optional, written as zeros); colours, SHs and radii receive no gradient.  Points that do not project into the image get zeros.
+ * scratch: gof_integrate_backward_scratch_bytes(P) device bytes, 256-byte aligned, contents irrelevant.  P == 0 or PN == 0
+ * writes zeros (and then the state is not read); a scratch NULL or too small fails with GOF_E_INVALID. */
+GOF_API size_t gof_integrate_backward_scratch_bytes(int P);
+GOF_API int gof_integrate_backward(const gof_scene_t* scene, int PN, const float* points3D, int num_rendered, const int* radii,
+                  void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
+                  void* point_binning_buffer, const float* dL_dalpha, float* dL_dpoints3D, float* dL_dopacity,
+                  float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
+                  void* scratch, size_t scratch_bytes, void* stream);
+
 /* The same query with the Gaussian side cached per view.  extract_mesh.py:56,92,107 calls integrate for the SAME views ten
  * times (tetrahedra vertices, 8 bisection steps, colours) -- only points3D changes, so preprocess / depth sort / instance
  * emission / tile sort of the Gaussians (rasterizer_impl.cu:566-660) are identical in every pass.
