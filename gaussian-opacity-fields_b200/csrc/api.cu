@@ -273,14 +273,14 @@ static int gaussian_side(const gof_scene_t* s, const GofView& v, gof_alloc_fn ge
 static int point_side(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
                       const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, gof_alloc_fn point_alloc,
                       void* point_user, gof_alloc_fn point_binning_alloc, void* point_binning_user, float* out_color,
-                      float* out_alpha_integrated, float* out_color_integrated, cudaStream_t st) {
+                      float* out_alpha_integrated, float* out_color_integrated, const GofIntMin* mn, cudaStream_t st) {
   const GofPointLayout PL = gof_point_layout((size_t)PN);
   const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count());
   char* pts = (char*)point_alloc(point_user, PL.bytes);
   char* pbin = (char*)point_binning_alloc(point_binning_user, PBL.bytes);
   if (!img || !pts || !pbin) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
   return gof_launch_integrate(s, v, PN, points3D, splat, point_list, ranges, img, IL, pts, PL, pbin, PBL, out_color,
-                              out_alpha_integrated, out_color_integrated, st);
+                              out_alpha_integrated, out_color_integrated, mn, st);
 }
 
 extern "C" int gof_rasterize_forward(const gof_scene_t* s, gof_alloc_fn geom_alloc, void* geom_user,
@@ -550,7 +550,41 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
                     g.IL, point_alloc, point_user, point_binning_alloc, point_binning_user, out_color, out_alpha_integrated,
-                    out_color_integrated, st);
+                    out_color_integrated, nullptr, st);
+}
+
+// One view of the multi-view opacity field (DESIGN.md 4.12): gof_integrate's Gaussian and point sides, then k_integrate<true>
+// folds each projecting point's alpha into alpha_min / argmin instead of writing the query's outputs.
+extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
+                                 void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
+                                 void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
+                                 void* point_binning_user, int* radii, float* alpha_min, int* argmin, void* stream) {
+  int rc = validate_scene(s);
+  if (rc != GOF_OK) return rc;
+  if (!geom_alloc || !binning_alloc || !image_alloc || !point_alloc || !point_binning_alloc) {
+    gof_set_error("integrate_min: allocators must be non-NULL");
+    return GOF_E_INVALID;
+  }
+  if (view < 0 || view >= (1 << 30)) {   // 2^30 is argmin's "no view" value
+    gof_set_error("integrate_min: view %d outside [0, 2^30)", view);
+    return GOF_E_INVALID;
+  }
+  if (s->P == 0 || PN <= 0) return GOF_OK;
+  if (!points3D || !radii || !alpha_min || !argmin) {
+    gof_set_error("integrate_min: NULL argument");
+    return GOF_E_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const GofView v = gof_make_view(s);
+  GaussianSide g;
+  int num_rendered = 0;
+  if ((rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.5f, false,
+                          &num_rendered, st, g)) != GOF_OK)
+    return rc;
+  const GofIntMin mn{alpha_min, argmin, view};
+  return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
+                    reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
+                    g.IL, point_alloc, point_user, point_binning_alloc, point_binning_user, nullptr, nullptr, nullptr, &mn, st);
 }
 
 extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
@@ -674,5 +708,5 @@ extern "C" int gof_integrate_cached(const gof_scene_t* s, int PN, const float* p
   const char* c = (const char*)cache;
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(c + CL.splat), reinterpret_cast<const uint32_t*>(c + CL.point_list),
                     reinterpret_cast<const uint2*>(c + CL.ranges), img, IL, point_alloc, point_user, point_binning_alloc,
-                    point_binning_user, out_color, out_alpha_integrated, out_color_integrated, st);
+                    point_binning_user, out_color, out_alpha_integrated, out_color_integrated, nullptr, st);
 }

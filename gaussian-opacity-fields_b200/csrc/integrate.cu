@@ -84,6 +84,10 @@ struct IntArgs {
   float* out_color;     // [9][H][W]
   float* out_alpha;     // [PN]
   float* out_color_int; // [PN][3]
+  // k_integrate<true> (the running minimum over views, DESIGN.md 4.12): writes only these two
+  float* alpha_min;     // [PN]
+  int* argmin;          // [PN]
+  int view;
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
@@ -237,6 +241,10 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
   return Pass1{range, T0, C0, C1, C2, tmax, Aacc, last_contributor, n_local};
 }
 
+// MIN_UPDATE: the query of one view of the multi-view opacity field (DESIGN.md 4.12).  Each point that projects folds its alpha
+// into alpha_min / argmin with the strict `<` of evaluate_alpha; views run in stream order and a point is one thread of one call,
+// so no atomics are needed.  Nothing else is written: no image, no point colour, no pixel state.
+template <bool MIN_UPDATE>
 __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a) {
   __shared__ float4 s_rec[BATCH][5];   // 80-byte rows: GofSplat | (thr, -, -, -), see render_fwd.cu
   __shared__ uint32_t s_cnt[256];      // contributors recorded per pixel (slot = thread of that pixel)
@@ -263,14 +271,19 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
     const uint32_t last_contributor = p1.last_contributor, n_local = p1.n_local;
 
     // forward.cu:997-1008
-    const size_t slot = (size_t)tile * 256 + threadIdx.x;
-    a.final_T[slot] = T0;
-    a.ncontrib[slot] = last_contributor;
-    a.ncontrib[(size_t)a.tiles * 256 + slot] = n_local;
-    const float col0 = F_FMA(T0, a.bg[0], C0), col1 = F_FMA(T0, a.bg[1], C1), col2 = F_FMA(T0, a.bg[2], C2);
+    float col0 = 0.f, col1 = 0.f, col2 = 0.f;
+    if constexpr (!MIN_UPDATE) {
+      const size_t slot = (size_t)tile * 256 + threadIdx.x;
+      a.final_T[slot] = T0;
+      a.ncontrib[slot] = last_contributor;
+      a.ncontrib[(size_t)a.tiles * 256 + slot] = n_local;
+      col0 = F_FMA(T0, a.bg[0], C0); col1 = F_FMA(T0, a.bg[1], C1); col2 = F_FMA(T0, a.bg[2], C2);
+    }
     s_cnt[threadIdx.x] = n_local;
-    s_col[threadIdx.x][0] = col0; s_col[threadIdx.x][1] = col1; s_col[threadIdx.x][2] = col2;
-    s_proj[threadIdx.x] = 0u;
+    if constexpr (!MIN_UPDATE) {
+      s_col[threadIdx.x][0] = col0; s_col[threadIdx.x][1] = col1; s_col[threadIdx.x][2] = col2;
+      s_proj[threadIdx.x] = 0u;
+    }
     __threadfence_block();
     __syncthreads();
 
@@ -286,7 +299,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
         int lx = gof_f2i_rz(xy.x) - tile_x * 16, ly = gof_f2i_rz(xy.y) - tile_y * 16;
         lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
         const int pslot = ((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7);
-        atomicAdd(&s_proj[pslot], 1u);
+        if constexpr (!MIN_UPDATE) atomicAdd(&s_proj[pslot], 1u);
         const float rx = (float)D_DIV(D_FMA((double)a.W, -0.5, (double)xy.x), (double)a.focal_x);
         const float ry = (float)D_DIV(D_FMA((double)a.H, -0.5, (double)xy.y), (double)a.focal_y);
         const uint32_t cnt = s_cnt[pslot];
@@ -310,14 +323,21 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
           point_alpha = F_FMA(al, point_T, point_alpha);
           point_T = F_MUL(point_T, F_SUB(1.0f, al));
         }
-        a.out_alpha[id] = point_alpha;
-        a.out_color_int[3 * (size_t)id + 0] = s_col[pslot][0];
-        a.out_color_int[3 * (size_t)id + 1] = s_col[pslot][1];
-        a.out_color_int[3 * (size_t)id + 2] = s_col[pslot][2];
+        if constexpr (MIN_UPDATE) {
+          if (point_alpha < a.alpha_min[id]) {   // evaluate_alpha's update, in view order
+            a.alpha_min[id] = point_alpha;
+            a.argmin[id] = a.view;
+          }
+        } else {
+          a.out_alpha[id] = point_alpha;
+          a.out_color_int[3 * (size_t)id + 0] = s_col[pslot][0];
+          a.out_color_int[3 * (size_t)id + 1] = s_col[pslot][1];
+          a.out_color_int[3 * (size_t)id + 2] = s_col[pslot][2];
+        }
       }
     }
     __syncthreads();
-    if (inside) {
+    if (!MIN_UPDATE && inside) {
       const size_t pid = (size_t)pix_y * a.W + pix_x;
       a.out_color[0 * HW + pid] = col0;
       a.out_color[1 * HW + pid] = col1;
@@ -529,7 +549,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM) k_integra
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
                          const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, char* pts,
                          const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, float* out_color, float* out_alpha,
-                         float* out_color_int, cudaStream_t st) {
+                         float* out_color_int, const GofIntMin* mn, cudaStream_t st) {
   const bool debug = s->debug != 0;
   PtArgs pa{};
   pa.PN = PN; pa.W = v.W; pa.H = v.H; pa.grid_x = v.grid_x; pa.grid_y = v.grid_y; pa.tiles = v.tiles;
@@ -558,7 +578,12 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
   a.final_T = reinterpret_cast<float*>(img + IL.accum);
   a.ncontrib = reinterpret_cast<uint32_t*>(img + IL.ncontrib);
   a.out_color = out_color; a.out_alpha = out_alpha; a.out_color_int = out_color_int;
-  GOF_LAUNCH("integrate", st, k_integrate<<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
+  if (mn) {
+    a.alpha_min = mn->alpha_min; a.argmin = mn->argmin; a.view = mn->view;
+    GOF_LAUNCH("integrate_min", st, k_integrate<true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
+  } else {
+    GOF_LAUNCH("integrate", st, k_integrate<false><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
+  }
   GOF_LAUNCH_CHECK(debug, st);
   return GOF_OK;
 }

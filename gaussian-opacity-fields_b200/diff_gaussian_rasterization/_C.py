@@ -452,6 +452,42 @@ def _integrate(background, points3D, means3D, colors, opacity, scales, rotations
             pbin.tensor)
 
 
+_lib.gof_integrate_min.restype = ctypes.c_int
+_lib.gof_integrate_min.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_ALLOC_FN, ctypes.c_void_p] * 5 + \
+    [_fp, _fp, _fp, ctypes.c_void_p]
+
+
+def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier,
+                                      cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size,
+                                      subpixel_offset, image_height, image_width, sh, degree, campos, prefiltered, debug, view,
+                                      alpha_min, argmin):
+    """gof_integrate_min (extension, DESIGN.md 4.12): integrate_gaussians_to_points for view index `view`, folded into the running
+    minimum over views in place: where a point's alpha_integrated < alpha_min, alpha_min takes it and argmin takes `view`.
+    alpha_min (float32 [PN], start at 1) and argmin (int32 [PN], start at 2^30) must be contiguous.  Returns radii [P]."""
+    if points3D.ndimension() != 2 or points3D.size(1) != 3:
+        raise RuntimeError("points3D must have dimensions (num_points, 3)")
+    PN = points3D.size(0)
+    for name, t, dt in (("alpha_min", alpha_min, torch.float32), ("argmin", argmin, torch.int32)):
+        if t.dtype != dt or tuple(t.shape) != (PN,) or not t.is_contiguous():
+            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape ({PN},)")
+    keep = []
+    s = _scene(keep, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+               view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset,
+               image_height, image_width, sh, degree, campos, prefiltered, debug)
+    dev = means3D.device
+    radii = torch.zeros((s.P,), dtype=torch.int32, device=dev)
+    if s.P != 0 and PN != 0:
+        sdev = dev if means3D.is_cuda else torch.device("cuda")
+        geom, binning, img = _Scratch(sdev, "geom"), _Scratch(sdev, "binning", 1.25), _Scratch(sdev, "image")
+        pts, pbin = _Scratch(sdev, "points"), _Scratch(sdev, "point_binning")
+        p3 = points3D.contiguous()
+        with torch.cuda.device(dev):
+            _check(_lib.gof_integrate_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), geom.cb, None, binning.cb, None, img.cb,
+                                          None, pts.cb, None, pbin.cb, None, radii.data_ptr(), _ptr(alpha_min, device=dev),
+                                          _ptr(argmin, torch.int32, device=dev), _stream()))
+    return radii
+
+
 _lib.gof_integrate_backward_scratch_bytes.restype = ctypes.c_size_t
 _lib.gof_integrate_backward_scratch_bytes.argtypes = [ctypes.c_int]
 _lib.gof_integrate_backward.restype = ctypes.c_int

@@ -160,6 +160,14 @@ def _integrate_args(rs, points3D, means3D, colors_precomp, opacities, scales, ro
                                                          rs.prefiltered, rs.debug)
 
 
+def _integrate_backward_args(rs, points3D, means3D, radii, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp,
+                             shs, grad_alpha, num_rendered, geom, binning, img, pts, pbin):
+    """The argument tuple of _C.integrate_gaussians_to_points_backward for the state of a query made with _integrate_args."""
+    return (rs.bg, points3D, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3D_precomp,
+            view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, shs, rs.sh_degree, rs.campos,
+                                                         grad_alpha, num_rendered, geom, binning, img, pts, pbin, rs.debug)
+
+
 class _IntegrateGaussians(torch.autograd.Function):
     """The opacity-field query with alpha_integrated differentiable with respect to points3D, means3D, opacities, scales,
     rotations and view2gaussian_precomp (DESIGN.md 4.11).  color, color_integrated and radii carry no gradient."""
@@ -186,9 +194,8 @@ class _IntegrateGaussians(torch.autograd.Function):
          pts, pbin) = ctx.saved_tensors
         if grad_alpha is None:
             grad_alpha = torch.zeros(points3D.size(0), dtype=torch.float32, device=points3D.device)
-        args = (rs.bg, points3D, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3D_precomp,
-                view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, shs, rs.sh_degree, rs.campos,
-                                                             grad_alpha, ctx.num_rendered, geom, binning, img, pts, pbin, rs.debug)
+        args = _integrate_backward_args(rs, points3D, means3D, radii, colors_precomp, scales, rotations, cov3D_precomp,
+                                        view2gaussian_precomp, shs, grad_alpha, ctx.num_rendered, geom, binning, img, pts, pbin)
         g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g = _call_native(
             _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
             points_grad=ctx.needs_input_grad[0])

@@ -6,6 +6,8 @@ reference's extract_mesh.py, restated with view sharding over the GPUs of one bo
                        initialised every rank processes views[rank::world] and the partial minima are merged with one
                        all_reduce(MIN) (colour: the lowest view index attaining the minimum wins, like the reference's
                        strict `<` update in view order).
+* opacity_field     -- evaluate_alpha's field with gradients to the points and the Gaussians (DESIGN §4.12), view-sharded
+                       like it, in memory that does not grow with the number of views.
 * binary_search     == the 8-step bisection of extract_mesh.py:88-102 on the edge endpoints returned by
                        gof_tetmesh.marching_tetrahedra.
 * make_integrate_fn == gaussian_renderer.integrate (gaussian_renderer/__init__.py:118-218) for plain tensors.
@@ -90,6 +92,127 @@ def make_integrate_fn(means3D, opacities, scales, rotations, shs, sh_degree, set
             rotations=rotations)
         return alpha_integrated, color_integrated
     return fn
+
+
+_NO_VIEW = 2 ** 30   # argmin of a point no view lowered below 1
+
+
+def _field_inputs(scales, rotations, shs):
+    """(colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp, shs) as GaussianRasterizer.integrate passes them
+    for shs, scales and rotations: the optional inputs make_integrate_fn's queries leave out, in the reference's empty encoding."""
+    import diff_gaussian_rasterization as dgr
+    shs, colors, scales, rotations, cov3D, v2g = dgr._normalise_optionals(shs, None, scales, rotations, None, None)
+    return colors, scales, rotations, cov3D, v2g, shs
+
+
+def _field_args(rs, points, means3D, opacities, scales, rotations, shs):
+    """The argument tuple of the _C query entry points for GaussianRasterizer(rs).integrate(points3D=points, means3D=means3D,
+    opacities=opacities, shs=shs, scales=scales, rotations=rotations): what make_integrate_fn's queries receive."""
+    import diff_gaussian_rasterization as dgr
+    colors, scales, rotations, cov3D, v2g, shs = _field_inputs(scales, rotations, shs)
+    return dgr._integrate_args(rs, points, means3D, colors, opacities, scales, rotations, cov3D, v2g, shs)
+
+
+class _OpacityField(torch.autograd.Function):
+    """alpha = 1 - min over views of alpha_integrated (DESIGN.md 4.12), differentiable with respect to the points and the
+    Gaussians.  The forward keeps a running minimum and the winning view per point (8 bytes a point, nothing per view); the
+    backward rebuilds one view's query state at a time, on the points that view won."""
+
+    @staticmethod
+    def forward(ctx, points, means3D, opacities, scales, rotations, shs, views, settings_for_view, group):
+        import diff_gaussian_rasterization as dgr
+        from diff_gaussian_rasterization import _C
+        rank, world = _world(group)
+        n, dev = points.shape[0], points.device
+        alpha_min = torch.ones(n, dtype=torch.float32, device=dev)
+        argmin = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev)
+        views = list(views)
+        for vi in range(rank, len(views), world):
+            rs = settings_for_view(views[vi])
+            args = _field_args(rs, points, means3D, opacities, scales, rotations, shs) + (vi, alpha_min, argmin)
+            dgr._call_native(_C.integrate_gaussians_to_points_min, args, rs.debug, "snapshot_fw.dump", "forward")
+        if world > 1:
+            # evaluate_alpha's merge: the global minimum, won by the lowest view index that attains it (and is < 1)
+            local = alpha_min.clone()
+            dist.all_reduce(alpha_min, op=dist.ReduceOp.MIN, group=group)
+            argmin = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
+            dist.all_reduce(argmin, op=dist.ReduceOp.MIN, group=group)
+        ctx.save_for_backward(points, means3D, opacities, scales, rotations, shs, argmin)
+        ctx.views, ctx.settings_for_view, ctx.group = views, settings_for_view, group
+        return 1 - alpha_min
+
+    @staticmethod
+    def backward(ctx, grad_alpha):
+        import diff_gaussian_rasterization as dgr
+        from diff_gaussian_rasterization import _C
+        points, means3D, opacities, scales, rotations, shs, argmin = ctx.saved_tensors
+        rank, world = _world(ctx.group)
+        need = ctx.needs_input_grad
+        gaussians = any(need[1:5])
+        n, P, dev = points.shape[0], means3D.shape[0], points.device
+        dA = -grad_alpha.to(torch.float32).contiguous()   # d alpha / d alpha_min = -1, at each point's winning view only
+        if world > 1:
+            # a rank runs the backward of the views it owns only, so it needs every rank's dL/dalpha: the gradients are those of
+            # the sum of the ranks' losses
+            dA = dA.clone()
+            dist.all_reduce(dA, op=dist.ReduceOp.SUM, group=ctx.group)
+        # one flat buffer: a single all-reduce carries every gradient across ranks
+        sizes = (3 * n, 3 * P, P, 3 * P, 4 * P)
+        flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
+        g_pts, g_means, g_op, g_scales, g_rot = torch.split(flat, sizes)
+        g_pts, g_means, g_scales, g_rot = g_pts.view(n, 3), g_means.view(P, 3), g_scales.view(P, 3), g_rot.view(P, 4)
+        if n and P:
+            colors, scales_, rotations_, cov3D, v2g, shs_ = _field_inputs(scales, rotations, shs)
+            mine = torch.nonzero((argmin != _NO_VIEW) & (argmin % world == rank)).flatten()
+            order = mine[torch.argsort(argmin[mine], stable=True)]
+            won, counts = torch.unique_consecutive(argmin[order], return_counts=True)
+            start = 0
+            for vi, c in zip(won.tolist(), counts.tolist()):
+                sel = order[start:start + c]
+                start += c
+                rs = ctx.settings_for_view(ctx.views[vi])
+                p = points[sel]
+                args = dgr._integrate_args(rs, p, means3D, colors, opacities, scales_, rotations_, cov3D, v2g, shs_)
+                R, _color, _a, _c, radii, geom, binning, img, pts, pbin = dgr._call_native(
+                    _C.integrate_gaussians_to_points_state, args, rs.debug, "snapshot_fw.dump", "forward")
+                del _color, _a, _c
+                bargs = dgr._integrate_backward_args(rs, p, means3D, radii, colors, scales_, rotations_, cov3D, v2g, shs_, dA[sel], R,
+                                                     geom, binning, img, pts, pbin)
+                del geom, binning, img, pts, pbin
+                dp, dop, dm, dsc, drot, _dcov, _dv2g = dgr._call_native(
+                    _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward", points_grad=need[0])
+                del bargs   # the state goes back to the scratch pool before the next view
+                if dp is not None:
+                    g_pts[sel] = dp
+                if gaussians:
+                    g_means += dm
+                    g_op += dop.view(-1)
+                    g_scales += dsc
+                    g_rot += drot
+        if world > 1:
+            dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=ctx.group)
+        pick = lambda g, i, like: g.view_as(like) if need[i] else None   # noqa: E731
+        return (pick(g_pts, 0, points), pick(g_means, 1, means3D), pick(g_op, 2, opacities), pick(g_scales, 3, scales),
+                pick(g_rot, 4, rotations), None, None, None, None)
+
+
+def opacity_field(points, means3D, opacities, scales, rotations, shs, sh_degree, views, settings_for_view, group=None):
+    """The multi-view opacity field alpha [N] = 1 - min over views of alpha_integrated: the tensor
+    evaluate_alpha(points, views, make_integrate_fn(means3D, opacities, scales, rotations, shs, sh_degree, settings_for_view),
+    group=group) returns, bit for bit, but differentiable with respect to points, means3D, opacities, scales and rotations
+    (DESIGN.md 4.12).  As in make_integrate_fn, the SH degree the query uses is settings_for_view(view).sh_degree.
+
+    The gradient of a point goes through the view attaining its minimum (the lowest view index on a tie); a point that no view
+    lowered below 1 gets zeros.  Memory does not grow with the number of views: the forward keeps 8 bytes a point, and the
+    backward rebuilds the query state of one view at a time on the points that view won.
+
+    With torch.distributed initialised, each rank queries views[rank::world] and the ranks merge as evaluate_alpha does, so
+    every rank holds the whole field.  The backward is a collective: every rank of `group` must call backward() through the
+    field.  The gradients are those of the SUM of the ranks' losses: the backward all-reduces dL/dalpha before it runs each
+    rank's views, and all-reduces the gradients after, so every rank's .grad is the single-GPU gradient of that sum, up to
+    summation order.  A rank without a loss of its own backpropagates zeros (e.g. (alpha * 0).sum()); a loss computed
+    identically on every rank counts once per rank (divide it by the world size, or compute it on one rank only)."""
+    return _OpacityField.apply(points, means3D, opacities, scales, rotations, shs, views, settings_for_view, group)
 
 
 class CachedIntegrator:

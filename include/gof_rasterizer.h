@@ -185,6 +185,21 @@ GOF_API int gof_integrate(const gof_scene_t* scene, int PN, const float* points3
                   float* out_alpha_integrated, float* out_color_integrated,
                   int* num_rendered, void* stream);
 
+/* One view of the multi-view opacity field (no reference counterpart; DESIGN section 4.12): the query of gof_integrate for
+ * `view`, with each point that projects folded into a running minimum by evaluate_alpha's update in view order,
+ *     if (alpha < alpha_min[k]) { alpha_min[k] = alpha; argmin[k] = view; }
+ * alpha_min [PN] and argmin [PN] are initialised by the caller to 1 and 2^30 and passed to every view's call on one stream; points
+ * that do not project are not written.  Neither the image nor the point colours are formed.  The allocators are gof_integrate's
+ * (the buffers are scratch once the call has been ordered on the stream); every entry of radii [P] is written.  A view outside
+ * [0, 2^30) fails with GOF_E_INVALID; with P == 0 or PN <= 0 nothing is written. */
+GOF_API int gof_integrate_min(const gof_scene_t* scene, int PN, const float* points3D, int view,
+                  gof_alloc_fn geom_alloc, void* geom_user,
+                  gof_alloc_fn binning_alloc, void* binning_user,
+                  gof_alloc_fn image_alloc, void* image_user,
+                  gof_alloc_fn point_alloc, void* point_user,
+                  gof_alloc_fn point_binning_alloc, void* point_binning_user,
+                  int* radii, float* alpha_min, int* argmin, void* stream);
+
 /* The backward of gof_integrate (no reference counterpart; DESIGN section 4.11): dL_dalpha [PN], the gradient of a loss with respect
  * to out_alpha_integrated, -> the gradients with respect to the points and the Gaussians.  With each point's contributor list,
  * the alpha rejects and the alpha and depth clamps held fixed, d alpha_integrated / d alpha_j = prod_{i != j} (1 - alpha_i).
