@@ -555,10 +555,11 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
 
 // One view of the multi-view opacity field (DESIGN.md 4.12): gof_integrate's Gaussian and point sides, then k_integrate<true>
 // folds each projecting point's alpha into alpha_min / argmin instead of writing the query's outputs.
-extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
-                                 void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
-                                 void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
-                                 void* point_binning_user, int* radii, float* alpha_min, int* argmin, void* stream) {
+// with_color: gof_integrate_min_color, k_integrate<true, true> also writes the winner's colour to color_min (DESIGN.md 4.13)
+static int integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc, void* geom_user,
+                         gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc, void* image_user,
+                         gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc, void* point_binning_user,
+                         int* radii, float* alpha_min, int* argmin, bool with_color, float* color_min, void* stream) {
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
   if (!geom_alloc || !binning_alloc || !image_alloc || !point_alloc || !point_binning_alloc) {
@@ -570,7 +571,7 @@ extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* poin
     return GOF_E_INVALID;
   }
   if (s->P == 0 || PN <= 0) return GOF_OK;
-  if (!points3D || !radii || !alpha_min || !argmin) {
+  if (!points3D || !radii || !alpha_min || !argmin || (with_color && !color_min)) {
     gof_set_error("integrate_min: NULL argument");
     return GOF_E_INVALID;
   }
@@ -581,19 +582,39 @@ extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* poin
   if ((rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.5f, false,
                           &num_rendered, st, g)) != GOF_OK)
     return rc;
-  const GofIntMin mn{alpha_min, argmin, view};
+  const GofIntMin mn{alpha_min, argmin, view, with_color ? color_min : nullptr};
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
                     g.IL, point_alloc, point_user, point_binning_alloc, point_binning_user, nullptr, nullptr, nullptr, &mn, st);
 }
 
+extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
+                                 void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
+                                 void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
+                                 void* point_binning_user, int* radii, float* alpha_min, int* argmin, void* stream) {
+  return integrate_min(s, PN, points3D, view, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, point_alloc,
+                       point_user, point_binning_alloc, point_binning_user, radii, alpha_min, argmin, false, nullptr, stream);
+}
+
+extern "C" int gof_integrate_min_color(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
+                                       void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
+                                       void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
+                                       void* point_binning_user, int* radii, float* alpha_min, int* argmin, float* color_min,
+                                       void* stream) {
+  return integrate_min(s, PN, points3D, view, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, point_alloc,
+                       point_user, point_binning_alloc, point_binning_user, radii, alpha_min, argmin, true, color_min, stream);
+}
+
 extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
 
-extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
-                                      void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
-                                      void* point_binning_buffer, const float* dL_dalpha, float* dL_dpoints3D, float* dL_dopacity,
-                                      float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
-                                      void* scratch, size_t scratch_bytes, void* stream) {
+// with_color: gof_integrate_backward_color (DESIGN.md 4.13): dL_dalpha and dL_dcolor_int may be NULL, dL_dcolors is required and
+// dL_dsh too with SHs
+static int integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
+                              void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
+                              void* point_binning_buffer, const float* dL_dalpha, const float* dL_dcolor_int, float* dL_dpoints3D,
+                              float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian,
+                              float* dL_dcov3D, bool with_color, float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes,
+                              void* stream) {
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
   if (PN < 0) { gof_set_error("integrate_backward: PN < 0"); return GOF_E_INVALID; }
@@ -604,8 +625,13 @@ extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float*
   }
   if (s->P > 0 && !scratch) { gof_set_error("integrate_backward: scratch is NULL"); return GOF_E_INVALID; }
   const size_t P = (size_t)s->P;
-  if ((PN > 0 && !dL_dalpha) || (P > 0 && (!dL_dopacity || !dL_dmean3D || !dL_dview2gaussian))) {
+  if ((PN > 0 && !dL_dalpha && !with_color) || (P > 0 && (!dL_dopacity || !dL_dmean3D || !dL_dview2gaussian)) ||
+      (with_color && P > 0 && !dL_dcolors)) {
     gof_set_error("integrate_backward: NULL argument");
+    return GOF_E_INVALID;
+  }
+  if (with_color && s->shs && P > 0 && !dL_dsh) {
+    gof_set_error("integrate_backward: dL_dsh required with SHs");
     return GOF_E_INVALID;
   }
   if (s->scales && s->rotations && P > 0 && (!dL_dscale || !dL_drot)) {
@@ -617,9 +643,12 @@ extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float*
     return GOF_E_INVALID;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  if (P == 0 || PN == 0) {   // gof_integrate ran nothing: no alpha depends on anything
+  // P == 0 or PN == 0: gof_integrate ran nothing, no output depends on anything; likewise with no loss at all
+  if (P == 0 || PN == 0 || (!dL_dalpha && !dL_dcolor_int)) {
     if (dL_dpoints3D && PN > 0) GOF_CUDA_OK(cudaMemsetAsync(dL_dpoints3D, 0, (size_t)PN * 12, st));
     if (P > 0) {
+      if (with_color) GOF_CUDA_OK(cudaMemsetAsync(dL_dcolors, 0, P * 12, st));
+      if (with_color && s->shs) GOF_CUDA_OK(cudaMemsetAsync(dL_dsh, 0, P * (size_t)s->M * 12, st));
       GOF_CUDA_OK(cudaMemsetAsync(dL_dopacity, 0, P * 4, st));
       GOF_CUDA_OK(cudaMemsetAsync(dL_dmean3D, 0, P * 12, st));
       GOF_CUDA_OK(cudaMemsetAsync(dL_dview2gaussian, 0, P * 40, st));
@@ -646,7 +675,29 @@ extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float*
                                        reinterpret_cast<const uint2*>(static_cast<const char*>(image_buffer) + IL.ranges),
                                        static_cast<const char*>(point_buffer), PL, static_cast<char*>(point_binning_buffer), PBL,
                                        dL_dalpha, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale, dL_drot, dL_dview2gaussian,
-                                       dL_dcov3D, scratch, st);
+                                       dL_dcov3D, with_color ? dL_dcolor_int : nullptr, with_color ? dL_dcolors : nullptr,
+                                       with_color ? dL_dsh : nullptr, scratch, st);
+}
+
+extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
+                                      void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
+                                      void* point_binning_buffer, const float* dL_dalpha, float* dL_dpoints3D, float* dL_dopacity,
+                                      float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
+                                      void* scratch, size_t scratch_bytes, void* stream) {
+  return integrate_backward(s, PN, points3D, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, point_buffer,
+                            point_binning_buffer, dL_dalpha, nullptr, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale, dL_drot,
+                            dL_dview2gaussian, dL_dcov3D, false, nullptr, nullptr, scratch, scratch_bytes, stream);
+}
+
+extern "C" int gof_integrate_backward_color(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
+                                            void* geom_buffer, const void* binning_buffer, const void* image_buffer,
+                                            const void* point_buffer, void* point_binning_buffer, const float* dL_dalpha,
+                                            const float* dL_dcolor_integrated, float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D,
+                                            float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
+                                            float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes, void* stream) {
+  return integrate_backward(s, PN, points3D, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, point_buffer,
+                            point_binning_buffer, dL_dalpha, dL_dcolor_integrated, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale,
+                            dL_drot, dL_dview2gaussian, dL_dcov3D, true, dL_dcolors, dL_dsh, scratch, scratch_bytes, stream);
 }
 
 // ---- the Gaussian side of the query, once per view --------------------------------------------------------------

@@ -414,6 +414,7 @@ struct GofIntMin {
   float* alpha_min;   // [PN]
   int* argmin;        // [PN]
   int view;
+  float* color_min;   // [PN][3] or NULL: also the winning view's colour (gof_integrate_min_color, DESIGN.md 4.13)
 };
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
                          const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, char* pts,
@@ -422,12 +423,15 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
 // The backward of the query (DESIGN.md 4.11) from the state gof_launch_integrate left in geom / pts / pbin: dL_dalpha [PN] ->
 // dL_dpoints3D [PN][3] (optional) and, through the accumulator rows and k_preprocess_backward, the Gaussian gradients.  The
 // contributor slab in pbin and the accumulator rows in geom are rewritten.  scratch: gof_integrate_backward_scratch(P) bytes.
+// dL_dcolors NULL: the alpha-only backward (no SH chain).  Otherwise (DESIGN.md 4.13) dL_dcolor_int [PN][3] (NULL: no colour
+// loss) also goes through the colour walk, dL_dalpha may be NULL, and dL_dcolors [P][3] / dL_dsh receive the colour's chain.
 size_t gof_integrate_backward_scratch(int P);
 int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const int* radii,
                                   char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
                                   const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
                                   float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot,
-                                  float* dL_dv2g, float* dL_dcov3D, void* scratch, cudaStream_t st);
+                                  float* dL_dv2g, float* dL_dcov3D, const float* dL_dcolor_int, float* dL_dcolors, float* dL_dsh,
+                                  void* scratch, cudaStream_t st);
 
 // Per-view cache of the Gaussian side of the opacity-field query (gof_integrate_prepare / gof_integrate_cached): the records,
 // the tile ranges and the per-tile Gaussian lists are all a query needs, and they do not depend on the query points.

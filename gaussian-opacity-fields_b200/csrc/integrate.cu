@@ -15,6 +15,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "gof_common.cuh"
 #include "gof_math.cuh"
@@ -88,6 +89,7 @@ struct IntArgs {
   float* alpha_min;     // [PN]
   int* argmin;          // [PN]
   int view;
+  float* color_min;     // [PN][3], k_integrate<true, true>: the winning view's pixel colour (DESIGN.md 4.13)
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
@@ -157,10 +159,27 @@ struct Pass1 {
   uint32_t last_contributor, n_local;
 };
 
+// One batch of the tile list into shared memory: the record and the reject threshold of ray_step (pass 1 and the colour walk)
+__device__ __forceinline__ void int_load_batch(const uint32_t* __restrict__ point_list, const GofSplat* __restrict__ splat,
+                                               float4 (*s_rec)[5], uint2 range, int progress, int total) {
+  if (progress < total) {
+    const uint32_t g = point_list[range.x + progress];
+    const float4* src = reinterpret_cast<const float4*>(splat + g);
+    const float4 r2 = __ldg(src + 2);
+    s_rec[threadIdx.x][0] = __ldg(src); s_rec[threadIdx.x][1] = __ldg(src + 1);
+    s_rec[threadIdx.x][2] = r2; s_rec[threadIdx.x][3] = __ldg(src + 3);
+    const float op = r2.z;
+    s_rec[threadIdx.x][4].x = (op > 0.f) ? (-logf(255.0f * op) - 2e-3f) : __int_as_float(0x7f800000);
+  }
+}
+
+// CTOT: also sum the centre ray's blend in double, ctot = (T, C_0, C_1, C_2) with C = sum_j T_j alpha_j c_j (the colour walk's
+// totals, DESIGN.md 4.13); the float state is the same either way
+template <bool CTOT = false>
 __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                                            const GofSplat* __restrict__ splat, float4 (*s_rec)[5], uint32_t s_base, int tile, int wx0,
                                            int wy0, uint32_t pix_x, uint32_t pix_y, bool inside, int W, int H, float focal_x,
-                                           float focal_y, uint16_t* my_ids) {
+                                           float focal_y, uint16_t* my_ids, double* ctot = nullptr) {
   const int lane = threadIdx.x & 31;
   bool done = !inside;
 
@@ -184,16 +203,7 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
 
   for (int i = 0; i < rounds; ++i) {
     __syncthreads();
-    const int progress = i * BATCH + (int)threadIdx.x;
-    if (progress < total) {
-      const uint32_t g = point_list[range.x + progress];
-      const float4* src = reinterpret_cast<const float4*>(splat + g);
-      const float4 r2 = __ldg(src + 2);
-      s_rec[threadIdx.x][0] = __ldg(src); s_rec[threadIdx.x][1] = __ldg(src + 1);
-      s_rec[threadIdx.x][2] = r2; s_rec[threadIdx.x][3] = __ldg(src + 3);
-      const float op = r2.z;
-      s_rec[threadIdx.x][4].x = (op > 0.f) ? (-logf(255.0f * op) - 2e-3f) : __int_as_float(0x7f800000);
-    }
+    int_load_batch(point_list, splat, s_rec, range, i * BATCH + (int)threadIdx.x, total);
     __syncthreads();
     const int nb = min(BATCH, total - i * BATCH);
 #pragma unroll 1
@@ -223,6 +233,11 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
           C1 = F_FMA(T0, F_MUL(al, q3.x), C1);
           C2 = F_FMA(T0, F_MUL(al, q3.y), C2);
           Aacc = F_FMA(T0, al, Aacc);
+          if constexpr (CTOT) {
+            const double w = ctot[0] * (double)al;
+            ctot[1] += w * (double)q2.w; ctot[2] += w * (double)q3.x; ctot[3] += w * (double)q3.y;
+            ctot[0] *= 1.0 - (double)al;
+          }
           T0 = tt; used = true;
         }
         if (ray_step<1>(v, op, thr, rxm, rym, T1, tmax, &al, &tt)) { T1 = tt; used = true; }
@@ -243,8 +258,9 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
 
 // MIN_UPDATE: the query of one view of the multi-view opacity field (DESIGN.md 4.12).  Each point that projects folds its alpha
 // into alpha_min / argmin with the strict `<` of evaluate_alpha; views run in stream order and a point is one thread of one call,
-// so no atomics are needed.  Nothing else is written: no image, no point colour, no pixel state.
-template <bool MIN_UPDATE>
+// so no atomics are needed.  Nothing else is written: no image, no point colour, no pixel state.  MIN_COLOR (DESIGN.md 4.13):
+// the same update also writes the point's colour of this view, C + T*bg as k_integrate<false> forms it, to color_min.
+template <bool MIN_UPDATE, bool MIN_COLOR = false>
 __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a) {
   __shared__ float4 s_rec[BATCH][5];   // 80-byte rows: GofSplat | (thr, -, -, -), see render_fwd.cu
   __shared__ uint32_t s_cnt[256];      // contributors recorded per pixel (slot = thread of that pixel)
@@ -279,11 +295,12 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
       a.ncontrib[(size_t)a.tiles * 256 + slot] = n_local;
       col0 = F_FMA(T0, a.bg[0], C0); col1 = F_FMA(T0, a.bg[1], C1); col2 = F_FMA(T0, a.bg[2], C2);
     }
+    if constexpr (MIN_COLOR) { col0 = F_FMA(T0, a.bg[0], C0); col1 = F_FMA(T0, a.bg[1], C1); col2 = F_FMA(T0, a.bg[2], C2); }
     s_cnt[threadIdx.x] = n_local;
-    if constexpr (!MIN_UPDATE) {
+    if constexpr (!MIN_UPDATE || MIN_COLOR) {
       s_col[threadIdx.x][0] = col0; s_col[threadIdx.x][1] = col1; s_col[threadIdx.x][2] = col2;
-      s_proj[threadIdx.x] = 0u;
     }
+    if constexpr (!MIN_UPDATE) s_proj[threadIdx.x] = 0u;
     __threadfence_block();
     __syncthreads();
 
@@ -327,6 +344,11 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
           if (point_alpha < a.alpha_min[id]) {   // evaluate_alpha's update, in view order
             a.alpha_min[id] = point_alpha;
             a.argmin[id] = a.view;
+            if constexpr (MIN_COLOR) {
+              a.color_min[3 * (size_t)id + 0] = s_col[pslot][0];
+              a.color_min[3 * (size_t)id + 1] = s_col[pslot][1];
+              a.color_min[3 * (size_t)id + 2] = s_col[pslot][2];
+            }
           }
         } else {
           a.out_alpha[id] = point_alpha;
@@ -371,6 +393,12 @@ struct IntBwdArgs {
   double* grad_acc;         // [P][16]: dL_dview2gaussian[10] of every pair lands in 0..9 (zeroed by the launcher)
   float* dL_dpoints3D;      // [PN][3] or NULL (zeroed by the launcher: points that do not project keep the zeros)
 };
+// k_integrate_backward<true> (DESIGN.md 4.13); dL_dalpha may then be NULL (no alpha walk).  A type of its own, so that the
+// alpha-only instantiation keeps its parameter block.
+struct IntBwdColorArgs : IntBwdArgs {
+  const float* dL_dcolor;   // [PN][3], the gradient of color_integrated: dL/dcolor lands in rows 10..12 of grad_acc
+  const float* bg;          // [3]
+};
 
 // One pair of walk 1 / walk 2: the forward's float alpha (same operations as k_integrate's pass 2) and what its derivative needs.
 struct PairEval {
@@ -397,7 +425,110 @@ __device__ __forceinline__ PairEval pair_eval(const float* v, float op, float rx
 // 94 registers: two CTAs per SM (the query's three do not fit), and the grid is that many, so no CTA waits for a second wave
 constexpr int INT_BWD_CTAS_PER_SM = 2;
 
-__global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM) k_integrate_backward(const IntBwdArgs a) {
+// The colour walk of one tile (DESIGN.md 4.13).  color_integrated of a point is its pixel's C + T*bg on the centre ray, so
+// dL/dC of a pixel is the sum of dL/dcolor_integrated over its points.  The walk replays pass 1's centre ray over the tile list
+// -- the same batches, the same box test, the same ray_step<0> with the same float T -- up to the pixel's last contributor (the
+// forward's cap ends every ray there), so it visits exactly the Gaussians the forward blended, with their true list positions
+// (the recorded uint16 ids wrap past 65 535).  With T_j, the suffix S_j = tot - sum_{i<=j} T_i alpha_i c_i (tot from pass 1, in
+// double):  dL/dc_j = T_j alpha_j dL/dC  and  dL/dalpha_j = dL/dC . (T_j c_j - S_j / (1 - alpha_j)).  A warp visits its candidate
+// Gaussians in step, so each pair's 13 rows are summed over the warp and sent by one lane.
+__device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 (*s_rec)[5], uint32_t s_base, uint2 range, int wx0,
+                                               int wy0, uint32_t pix_x, uint32_t pix_y, const double* dC, const double* tot,
+                                               uint32_t last, uint32_t* s_last) {
+  const int lane = threadIdx.x & 31;
+  const bool want = last > 0 && (dC[0] != 0.0 || dC[1] != 0.0 || dC[2] != 0.0);
+  if (threadIdx.x == 0) *s_last = 0u;
+  __syncthreads();
+  if (want) atomicMax(s_last, last);
+  __syncthreads();
+  const int total = (int)*s_last;   // no wanting pixel of the CTA blended anything past it
+  if (total == 0) return;           // uniform
+  const bool warp_wants = __any_sync(0xffffffffu, want);
+  const uint32_t warp_last = __reduce_max_sync(0xffffffffu, want ? last : 0u);
+
+  const float pfx = F_ADD((float)pix_x, 0.5f), pfy = F_ADD((float)pix_y, 0.5f);
+  const float rx0 = (float)D_DIV(D_SUB((double)pfx, D_MUL((double)a.W, 0.5)), (double)a.focal_x);
+  const float ry0 = (float)D_DIV(D_SUB((double)pfy, D_MUL((double)a.H, 0.5)), (double)a.focal_y);
+  float T0 = 1.f, tmax = 0.f;
+  double T = 1.0, pre0 = 0.0, pre1 = 0.0, pre2 = 0.0;
+  const int rounds = (total + BATCH - 1) / BATCH;
+  for (int i = 0; i < rounds; ++i) {
+    __syncthreads();
+    int_load_batch(a.point_list, a.splat, s_rec, range, i * BATCH + (int)threadIdx.x, total);
+    __syncthreads();
+    if (!warp_wants) continue;
+    const int nb = min(BATCH, total - i * BATCH);
+#pragma unroll 1
+    for (int k = 0; k < BATCH / 32; ++k) {
+      if (k * 32 >= nb || (uint32_t)(i * BATCH + k * 32) >= warp_last) break;
+      const int idx = k * 32 + lane;
+      const float4 qb = s_rec[idx][3];
+      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
+      while (m) {
+        const int j = k * 32 + __ffs(m) - 1;
+        m &= m - 1;
+        const uint32_t contributor = (uint32_t)(i * BATCH + j + 1);
+        double d[13];
+#pragma unroll
+        for (int r = 0; r < 13; ++r) d[r] = 0.0;
+        bool has = false;
+        if (want && contributor <= last) {
+          const uint32_t row = s_base + (uint32_t)j * 80u;
+          const float4 q0 = gof_lds128<0>(row), q1 = gof_lds128<16>(row), q2 = gof_lds128<32>(row);
+          const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
+          const float op = q2.z;
+          float al, tt;
+          if (ray_step<0>(v, op, gof_lds32<64>(row), rx0, ry0, T0, tmax, &al, &tt)) {
+            T0 = tt;
+            has = true;
+            const float2 q3 = gof_lds64<48>(row);
+            const double c[3] = {(double)q2.w, (double)q3.x, (double)q3.y};
+            const double alpha = al, w = T * alpha, om = 1.0 - alpha;
+            pre0 += w * c[0]; pre1 += w * c[1]; pre2 += w * c[2];
+            const double S[3] = {tot[1] - pre0, tot[2] - pre1, tot[3] - pre2};
+            double dLdal = 0.0;
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) {
+              d[10 + ch] = w * dC[ch];
+              dLdal += dC[ch] * (T * c[ch] - S[ch] / om);
+            }
+            T *= om;
+            // the derivative pieces of ray_step's alpha: power = -1/2 (CC - BB^2 / (4 AA)), stationary in t = -BB / (2 AA)
+            float AA, BB;
+            pair_geom_k<0>(v, rx0, ry0, &AA, &BB);
+            const float t = F_DIV(-BB, F_ADD(AA, AA));
+            const float power = (float)D_MUL(D_FMA((double)F_DIV(-BB, AA), D_MUL((double)BB, 0.25), (double)v[9]), -0.5);
+            if (power <= 0.0f && F_MUL(op, F_EXP(power)) <= GOF_ALPHA_MAX) {
+              const double f = -0.5 * dLdal * alpha;   // dL/dpower times d power / d CC
+              const double x = rx0, y = ry0, td = t, ft2 = f * td * td, ft = f * td;
+              d[0] = ft2 * x * x; d[1] = 2.0 * ft2 * x * y; d[2] = 2.0 * ft2 * x;
+              d[3] = ft2 * y * y; d[4] = 2.0 * ft2 * y; d[5] = ft2;
+              d[6] = 2.0 * ft * x; d[7] = 2.0 * ft * y; d[8] = 2.0 * ft; d[9] = f;
+            }
+          }
+        }
+        const uint32_t with = __ballot_sync(0xffffffffu, has);
+        if (!with) continue;
+        const int src = __ffs(with) - 1;
+        if (__popc(with) > 1) {
+#pragma unroll
+          for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+            for (int r = 0; r < 13; ++r) d[r] += __shfl_xor_sync(0xffffffffu, d[r], off);
+        }
+        if (lane == src) {
+          double* acc = a.grad_acc + (size_t)a.point_list[range.x + contributor - 1] * 16;
+#pragma unroll
+          for (int r = 0; r < 13; ++r) atomicAdd(acc + r, d[r]);
+        }
+      }
+    }
+  }
+}
+
+template <bool COLOR>
+__global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
+    k_integrate_backward(const std::conditional_t<COLOR, IntBwdColorArgs, IntBwdArgs> a) {
   __shared__ float4 s_rec[BATCH][5];
   __shared__ uint32_t s_cnt[256];
 
@@ -414,14 +545,15 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM) k_integra
     const uint32_t pix_x = wx0 + (lane & 7), pix_y = wy0 + (lane >> 3);
     const bool inside = pix_x < (uint32_t)a.W && pix_y < (uint32_t)a.H;
 
-    const Pass1 p1 = int_pass1(a.ranges, a.point_list, a.splat, s_rec, s_base, tile, wx0, wy0, pix_x, pix_y, inside, a.W, a.H,
-                               a.focal_x, a.focal_y, my_ids);
+    double tot[4] = {1.0, 0.0, 0.0, 0.0};
+    const Pass1 p1 = int_pass1<COLOR>(a.ranges, a.point_list, a.splat, s_rec, s_base, tile, wx0, wy0, pix_x, pix_y, inside, a.W,
+                                      a.H, a.focal_x, a.focal_y, my_ids, COLOR ? tot : nullptr);
     const uint2 range = p1.range;
     s_cnt[threadIdx.x] = p1.n_local;
     __threadfence_block();
     __syncthreads();
 
-    for (uint32_t base = pr.x; base < pr.y; base += BATCH) {
+    for (uint32_t base = pr.x; base < (COLOR && a.dL_dalpha == nullptr ? pr.x : pr.y); base += BATCH) {
       const uint32_t q = base + threadIdx.x;
       const bool valid = q < pr.y;
       uint32_t id = 0;
@@ -540,6 +672,45 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM) k_integra
         }
       }
     }
+    if constexpr (COLOR) {
+      // dL/dC of each pixel: its points' dL/dcolor_integrated summed in double in the point sort's order (a pixel's points are
+      // neighbours there, a run may cross batches), by the first point of the run in each batch
+      __shared__ double s_dC[256][3];
+      __shared__ uint32_t s_slot[BATCH + 1];
+      __shared__ float s_g[BATCH][3];
+      __shared__ uint32_t s_last;
+      s_dC[threadIdx.x][0] = s_dC[threadIdx.x][1] = s_dC[threadIdx.x][2] = 0.0;
+      for (uint32_t base = pr.x; base < pr.y; base += BATCH) {
+        const uint32_t q = base + threadIdx.x;
+        uint32_t pslot = 256;
+        float g[3] = {0.f, 0.f, 0.f};
+        if (q < pr.y) {
+          const uint32_t id = a.pt_list[q];
+          const float2 xy = a.pt_xy[id];
+          int lx = gof_f2i_rz(xy.x) - tile_x * 16, ly = gof_f2i_rz(xy.y) - tile_y * 16;
+          lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
+          pslot = ((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7);
+#pragma unroll
+          for (int ch = 0; ch < 3; ++ch) g[ch] = a.dL_dcolor[3 * (size_t)id + ch];
+        }
+        __syncthreads();   // s_slot / s_g of the previous batch are read
+        s_slot[threadIdx.x] = pslot;
+        s_g[threadIdx.x][0] = g[0]; s_g[threadIdx.x][1] = g[1]; s_g[threadIdx.x][2] = g[2];
+        if (threadIdx.x == 0) s_slot[BATCH] = 256;
+        __syncthreads();
+        if (pslot < 256 && (threadIdx.x == 0 || s_slot[threadIdx.x - 1] != pslot)) {
+          double acc[3] = {s_dC[pslot][0], s_dC[pslot][1], s_dC[pslot][2]};
+          for (int k = threadIdx.x; s_slot[k] == pslot; ++k)
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) acc[ch] += (double)s_g[k][ch];
+          s_dC[pslot][0] = acc[0]; s_dC[pslot][1] = acc[1]; s_dC[pslot][2] = acc[2];
+        }
+      }
+      __syncthreads();
+      const double dC[3] = {s_dC[threadIdx.x][0], s_dC[threadIdx.x][1], s_dC[threadIdx.x][2]};
+      tot[1] += tot[0] * (double)a.bg[0]; tot[2] += tot[0] * (double)a.bg[1]; tot[3] += tot[0] * (double)a.bg[2];
+      int_color_walk(a, s_rec, s_base, range, wx0, wy0, pix_x, pix_y, dC, tot, p1.last_contributor, &s_last);
+    }
     __syncthreads();
   }
 }
@@ -579,8 +750,11 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
   a.ncontrib = reinterpret_cast<uint32_t*>(img + IL.ncontrib);
   a.out_color = out_color; a.out_alpha = out_alpha; a.out_color_int = out_color_int;
   if (mn) {
-    a.alpha_min = mn->alpha_min; a.argmin = mn->argmin; a.view = mn->view;
-    GOF_LAUNCH("integrate_min", st, k_integrate<true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
+    a.alpha_min = mn->alpha_min; a.argmin = mn->argmin; a.view = mn->view; a.color_min = mn->color_min;
+    if (mn->color_min)
+      GOF_LAUNCH("integrate_min_color", st, k_integrate<true, true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
+    else
+      GOF_LAUNCH("integrate_min", st, k_integrate<true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
   } else {
     GOF_LAUNCH("integrate", st, k_integrate<false><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
   }
@@ -594,9 +768,10 @@ int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN
                                   char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
                                   const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
                                   float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot,
-                                  float* dL_dv2g, float* dL_dcov3D, void* scratch, cudaStream_t st) {
+                                  float* dL_dv2g, float* dL_dcov3D, const float* dL_dcolor_int, float* dL_dcolors, float* dL_dsh,
+                                  void* scratch, cudaStream_t st) {
   const bool debug = s->debug != 0;
-  IntBwdArgs a{};
+  IntBwdColorArgs a{};
   a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.tiles = v.tiles; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
   a.ranges = ranges; a.point_list = point_list; a.splat = reinterpret_cast<const GofSplat*>(geom + GL.splat);
   a.pranges = reinterpret_cast<const uint2*>(pbin + PBL.pranges);
@@ -607,18 +782,23 @@ int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN
   a.ids = reinterpret_cast<uint16_t*>(pbin + PBL.ids);
   a.grad_acc = reinterpret_cast<double*>(geom + GL.grad_acc);
   a.dL_dpoints3D = dL_dpoints3D;
+  a.dL_dcolor = dL_dcolor_int; a.bg = s->background;
   GOF_CUDA_OK(cudaMemsetAsync(a.grad_acc, 0, (size_t)s->P * 128, st));
   if (dL_dpoints3D) GOF_CUDA_OK(cudaMemsetAsync(dL_dpoints3D, 0, (size_t)PN * 12, st));
   // persistent CTAs: each strides over the tiles and uses the slab of its blockIdx.x (PBL.nblk slabs exist)
   const int grid = std::min(PBL.nblk, INT_BWD_CTAS_PER_SM * gof_sm_count());
-  GOF_LAUNCH("integrate_bwd", st, k_integrate_backward<<<grid, GOF_BLOCK_SIZE, 0, st>>>(a));
+  if (dL_dcolor_int)
+    GOF_LAUNCH("integrate_bwd_color", st, k_integrate_backward<true><<<grid, GOF_BLOCK_SIZE, 0, st>>>(a));
+  else
+    GOF_LAUNCH("integrate_bwd", st, k_integrate_backward<false><<<grid, GOF_BLOCK_SIZE, 0, st>>>(static_cast<const IntBwdArgs&>(a)));
   GOF_LAUNCH_CHECK(debug, st);
-  // the accumulator rows -> the Gaussian parameters, exactly as after the blend backward.  The query has no colour gradient: the
-  // scene goes in without SHs, and dL_dcolor / dL_dmean2D (zero rows) land in the scratch.
+  // the accumulator rows -> the Gaussian parameters, exactly as after the blend backward.  Without dL_dcolors (the alpha-only
+  // entry) the scene goes in without SHs, and dL_dcolor / dL_dmean2D (zero rows) land in the scratch; with it, rows 10..12 go
+  // through the SH (or colors_precomp) backward as after the blend.
   gof_scene_t sg = *s;
-  sg.shs = nullptr;
-  float* dcolor = static_cast<float*>(scratch);
+  if (!dL_dcolors) sg.shs = nullptr;
+  float* dcolor = dL_dcolors ? dL_dcolors : static_cast<float*>(scratch);
   float* dmean2D = reinterpret_cast<float*>(static_cast<char*>(scratch) + gof_align_up((size_t)s->P * 12, 256));
-  return gof_launch_preprocess_backward(&sg, v, geom, GL, radii, dmean2D, dL_dopacity, dcolor, dL_dv2g, dL_dmean3D, nullptr, dL_dscale,
-                                        dL_drot, dL_dcov3D, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, st);
+  return gof_launch_preprocess_backward(&sg, v, geom, GL, radii, dmean2D, dL_dopacity, dcolor, dL_dv2g, dL_dmean3D, dL_dcolors ? dL_dsh : nullptr,
+                                        dL_dscale, dL_drot, dL_dcov3D, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, st);
 }

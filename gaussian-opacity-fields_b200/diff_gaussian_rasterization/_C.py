@@ -455,21 +455,29 @@ def _integrate(background, points3D, means3D, colors, opacity, scales, rotations
 _lib.gof_integrate_min.restype = ctypes.c_int
 _lib.gof_integrate_min.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_ALLOC_FN, ctypes.c_void_p] * 5 + \
     [_fp, _fp, _fp, ctypes.c_void_p]
+_lib.gof_integrate_min_color.restype = ctypes.c_int
+_lib.gof_integrate_min_color.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + \
+    [_ALLOC_FN, ctypes.c_void_p] * 5 + [_fp, _fp, _fp, _fp, ctypes.c_void_p]
 
 
 def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier,
                                       cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size,
                                       subpixel_offset, image_height, image_width, sh, degree, campos, prefiltered, debug, view,
-                                      alpha_min, argmin):
+                                      alpha_min, argmin, color_min=None):
     """gof_integrate_min (extension, DESIGN.md 4.12): integrate_gaussians_to_points for view index `view`, folded into the running
     minimum over views in place: where a point's alpha_integrated < alpha_min, alpha_min takes it and argmin takes `view`.
-    alpha_min (float32 [PN], start at 1) and argmin (int32 [PN], start at 2^30) must be contiguous.  Returns radii [P]."""
+    alpha_min (float32 [PN], start at 1) and argmin (int32 [PN], start at 2^30) must be contiguous.  With color_min (float32
+    [PN,3], contiguous; gof_integrate_min_color, DESIGN.md 4.13) the same update also stores the point's color_integrated of
+    that view.  Returns radii [P]."""
     if points3D.ndimension() != 2 or points3D.size(1) != 3:
         raise RuntimeError("points3D must have dimensions (num_points, 3)")
     PN = points3D.size(0)
-    for name, t, dt in (("alpha_min", alpha_min, torch.float32), ("argmin", argmin, torch.int32)):
-        if t.dtype != dt or tuple(t.shape) != (PN,) or not t.is_contiguous():
-            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape ({PN},)")
+    checks = [("alpha_min", alpha_min, torch.float32, (PN,)), ("argmin", argmin, torch.int32, (PN,))]
+    if color_min is not None:
+        checks.append(("color_min", color_min, torch.float32, (PN, 3)))
+    for name, t, dt, shape in checks:
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape {shape}")
     keep = []
     s = _scene(keep, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset,
@@ -481,10 +489,15 @@ def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opa
         geom, binning, img = _Scratch(sdev, "geom"), _Scratch(sdev, "binning", 1.25), _Scratch(sdev, "image")
         pts, pbin = _Scratch(sdev, "points"), _Scratch(sdev, "point_binning")
         p3 = points3D.contiguous()
+        allocs = (geom.cb, None, binning.cb, None, img.cb, None, pts.cb, None, pbin.cb, None)
         with torch.cuda.device(dev):
-            _check(_lib.gof_integrate_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), geom.cb, None, binning.cb, None, img.cb,
-                                          None, pts.cb, None, pbin.cb, None, radii.data_ptr(), _ptr(alpha_min, device=dev),
-                                          _ptr(argmin, torch.int32, device=dev), _stream()))
+            if color_min is None:
+                _check(_lib.gof_integrate_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), *allocs, radii.data_ptr(),
+                                              _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev), _stream()))
+            else:
+                _check(_lib.gof_integrate_min_color(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), *allocs, radii.data_ptr(),
+                                                    _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev),
+                                                    _ptr(color_min, device=dev), _stream()))
     return radii
 
 
@@ -493,16 +506,21 @@ _lib.gof_integrate_backward_scratch_bytes.argtypes = [ctypes.c_int]
 _lib.gof_integrate_backward.restype = ctypes.c_int
 _lib.gof_integrate_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 15 + \
     [ctypes.c_size_t, ctypes.c_void_p]
+_lib.gof_integrate_backward_color.restype = ctypes.c_int
+_lib.gof_integrate_backward_color.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 18 + \
+    [ctypes.c_size_t, ctypes.c_void_p]
 
 
 def integrate_gaussians_to_points_backward(background, points3D, means3D, radii, colors, scales, rotations, scale_modifier,
                                            cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                                            kernel_size, subpixel_offset, image_height, image_width, sh, degree, campos,
                                            dL_dalpha, num_rendered, geomBuffer, binningBuffer, imgBuffer, pointBuffer,
-                                           pointBinningBuffer, debug, points_grad=True):
+                                           pointBinningBuffer, debug, points_grad=True, dL_dcolor=None):
     """gof_integrate_backward (extension, DESIGN.md 4.11): the gradient dL_dalpha [PN] of out_alpha_integrated ->
     (dL_dpoints3D [PN,3] or None, dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drotations [P,4],
-    dL_dcov3D [P,6], dL_dview2gaussian [P,10]).  The state is what integrate_gaussians_to_points_state returned."""
+    dL_dcov3D [P,6], dL_dview2gaussian [P,10]).  The state is what integrate_gaussians_to_points_state returned.
+    With dL_dcolor [PN,3], the gradient of out_color_integrated (gof_integrate_backward_color, DESIGN.md 4.13), dL_dalpha may be
+    None, and two more outputs follow: dL_dcolors [P,3] and dL_dsh [P,M,3] (None without SHs)."""
     P, PN = means3D.size(0), points3D.size(0)
     keep = []
     s = _scene(keep, background, means3D, colors, means3D, scales, rotations, scale_modifier, cov3D_precomp,
@@ -521,23 +539,37 @@ def integrate_gaussians_to_points_backward(background, points3D, means3D, radii,
     dpts = torch.empty((PN, 3), dtype=torch.float32, device=dev) if points_grad else None
     nbytes = int(_lib.gof_integrate_backward_scratch_bytes(P))
     scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-    p3, g = _c(points3D), _c(dL_dalpha)
-    if g.numel() != PN:
+    p3 = _c(points3D)
+    color = dL_dcolor is not None
+    g = None if color and dL_dalpha is None else _c(dL_dalpha)
+    if g is not None and g.numel() != PN:
         raise RuntimeError(f"gof_b200: dL_dalpha has {g.numel()} elements, expected {PN}")
     has_sr = s.scales is not None and s.rotations is not None
     buf = lambda t: t.data_ptr() if t is not None and t.numel() else None   # noqa: E731
-    with torch.cuda.device(dev):
-        _check(_lib.gof_integrate_backward(
-            ctypes.byref(s), PN, _ptr(p3, device=dev), int(num_rendered), _ptr(radii.contiguous(), torch.int32),
-            buf(geomBuffer), buf(binningBuffer), buf(imgBuffer), buf(pointBuffer), buf(pointBinningBuffer), _ptr(g, device=dev),
-            dpts.data_ptr() if dpts is not None and PN else None, out["dopacity"].data_ptr() if P else None,
-            out["dmeans3D"].data_ptr() if P else None, out["dscales"].data_ptr() if P and has_sr else None,
-            out["drot"].data_ptr() if P and has_sr else None, out["dv2g"].data_ptr() if P else None,
-            out["dcov3D"].data_ptr() if P else None, scratch.data_ptr() if nbytes else None, nbytes, _stream()))
+    head = (ctypes.byref(s), PN, _ptr(p3, device=dev), int(num_rendered), _ptr(radii.contiguous(), torch.int32), buf(geomBuffer),
+            buf(binningBuffer), buf(imgBuffer), buf(pointBuffer), buf(pointBinningBuffer), None if g is None else _ptr(g, device=dev))
+    grads = (dpts.data_ptr() if dpts is not None and PN else None, out["dopacity"].data_ptr() if P else None,
+             out["dmeans3D"].data_ptr() if P else None, out["dscales"].data_ptr() if P and has_sr else None,
+             out["drot"].data_ptr() if P and has_sr else None, out["dv2g"].data_ptr() if P else None,
+             out["dcov3D"].data_ptr() if P else None)
+    tail = (scratch.data_ptr() if nbytes else None, nbytes, _stream())
+    if not color:
+        with torch.cuda.device(dev):
+            _check(_lib.gof_integrate_backward(*head, *grads, *tail))
+    else:
+        gc = _c(dL_dcolor)
+        if gc.numel() != 3 * PN:
+            raise RuntimeError(f"gof_b200: dL_dcolor has {gc.numel()} elements, expected {3 * PN}")
+        dcolors = torch.empty((P, 3), dtype=torch.float32, device=dev)
+        dsh = torch.empty((P, s.M, 3), dtype=torch.float32, device=dev) if s.M > 0 else None
+        with torch.cuda.device(dev):
+            _check(_lib.gof_integrate_backward_color(*head, _ptr(gc, device=dev), *grads, dcolors.data_ptr() if P else None,
+                                                     dsh.data_ptr() if dsh is not None and dsh.numel() else None, *tail))
     if P and not has_sr:
         out["dscales"].zero_()
         out["drot"].zero_()
-    return dpts, out["dopacity"], out["dmeans3D"], out["dscales"], out["drot"], out["dcov3D"], out["dv2g"]
+    res = (dpts, out["dopacity"], out["dmeans3D"], out["dscales"], out["drot"], out["dcov3D"], out["dv2g"])
+    return res + (dcolors, dsh) if color else res
 
 
 _lib.gof_integrate_cache_bytes.restype = ctypes.c_size_t

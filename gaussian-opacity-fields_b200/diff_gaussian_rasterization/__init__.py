@@ -170,7 +170,8 @@ def _integrate_backward_args(rs, points3D, means3D, radii, colors_precomp, scale
 
 class _IntegrateGaussians(torch.autograd.Function):
     """The opacity-field query with alpha_integrated differentiable with respect to points3D, means3D, opacities, scales,
-    rotations and view2gaussian_precomp (DESIGN.md 4.11).  color, color_integrated and radii carry no gradient."""
+    rotations and view2gaussian_precomp (DESIGN.md 4.11), and color_integrated with respect to the same Gaussian inputs, shs and
+    colors_precomp (DESIGN.md 4.13; the points get nothing from it).  color and radii carry no gradient."""
 
     @staticmethod
     def forward(ctx, points3D, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
@@ -184,38 +185,46 @@ class _IntegrateGaussians(torch.autograd.Function):
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(points3D, means3D, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp, shs,
                               radii, geom, binning, img, pts, pbin)
-        ctx.mark_non_differentiable(color, color_integrated, radii)
+        ctx.mark_non_differentiable(color, radii)
+        ctx.set_materialize_grads(False)   # a color_integrated without a gradient keeps the alpha-only backward
         return color, alpha_integrated, color_integrated, radii
 
     @staticmethod
-    def backward(ctx, _grad_color, grad_alpha, _grad_color_integrated, _grad_radii):
+    def backward(ctx, _grad_color, grad_alpha, grad_color_integrated, _grad_radii):
         rs = ctx.raster_settings
         (points3D, means3D, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp, shs, radii, geom, binning, img,
          pts, pbin) = ctx.saved_tensors
-        if grad_alpha is None:
+        if grad_alpha is None and grad_color_integrated is None:
             grad_alpha = torch.zeros(points3D.size(0), dtype=torch.float32, device=points3D.device)
         args = _integrate_backward_args(rs, points3D, means3D, radii, colors_precomp, scales, rotations, cov3D_precomp,
                                         view2gaussian_precomp, shs, grad_alpha, ctx.num_rendered, geom, binning, img, pts, pbin)
-        g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g = _call_native(
-            _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
-            points_grad=ctx.needs_input_grad[0])
+        g_colors = g_sh = None
+        if grad_color_integrated is None:
+            g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g = _call_native(
+                _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
+                points_grad=ctx.needs_input_grad[0])
+        else:
+            g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g, g_colors, g_sh = _call_native(
+                _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
+                points_grad=ctx.needs_input_grad[0], dL_dcolor=grad_color_integrated)
         need = ctx.needs_input_grad
         pick = lambda g, i: g if need[i] else None   # noqa: E731
-        return (pick(g_pts, 0), pick(g_means3D, 1), None, pick(g_opacity, 3), None, None, pick(g_scales, 6), pick(g_rot, 7),
-                pick(g_cov3D, 8), pick(g_v2g, 9), None)
+        return (pick(g_pts, 0), pick(g_means3D, 1), None, pick(g_opacity, 3), pick(g_sh, 4), pick(g_colors, 5), pick(g_scales, 6),
+                pick(g_rot, 7), pick(g_cov3D, 8), pick(g_v2g, 9), None)
 
 
 def integrate_gaussians(points3D, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
                         view2gaussian_precomp, raster_settings):
-    """GaussianRasterizer.integrate with alpha_integrated differentiable (extension, DESIGN.md 4.11): returns the same
-    (color[9,H,W], alpha_integrated[PN], color_integrated[PN,3], radii[P]).  Optional inputs are None or empty tensors, as
-    for rasterize_gaussians.  With grad mode off, or with no input requiring grad, this is GaussianRasterizer.integrate."""
+    """GaussianRasterizer.integrate with alpha_integrated (extension, DESIGN.md 4.11) and color_integrated (DESIGN.md 4.13)
+    differentiable: returns the same (color[9,H,W], alpha_integrated[PN], color_integrated[PN,3], radii[P]).  Optional inputs
+    are None or empty tensors, as for rasterize_gaussians.  With grad mode off, or with no input requiring grad, this is
+    GaussianRasterizer.integrate."""
     shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp = _normalise_optionals(
         None if shs is None or shs.numel() == 0 else shs, None if colors_precomp is None or colors_precomp.numel() == 0 else colors_precomp,
         None if scales is None or scales.numel() == 0 else scales, None if rotations is None or rotations.numel() == 0 else rotations,
         None if cov3D_precomp is None or cov3D_precomp.numel() == 0 else cov3D_precomp,
         None if view2gaussian_precomp is None or view2gaussian_precomp.numel() == 0 else view2gaussian_precomp)
-    inputs = (points3D, means3D, opacities, scales, rotations, cov3D_precomp, view2gaussian_precomp)
+    inputs = (points3D, means3D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp)
     if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs):
         return _IntegrateGaussians.apply(points3D, means3D, means2D, opacities, shs, colors_precomp, scales, rotations,
                                          cov3D_precomp, view2gaussian_precomp, raster_settings)

@@ -7,7 +7,8 @@ reference's extract_mesh.py, restated with view sharding over the GPUs of one bo
                        all_reduce(MIN) (colour: the lowest view index attaining the minimum wins, like the reference's
                        strict `<` update in view order).
 * opacity_field     -- evaluate_alpha's field with gradients to the points and the Gaussians (DESIGN §4.12), view-sharded
-                       like it, in memory that does not grow with the number of views.
+                       like it, in memory that does not grow with the number of views; optionally its colour, with
+                       gradients to the Gaussians and their SHs (DESIGN §4.13).
 * binary_search     == the 8-step bisection of extract_mesh.py:88-102 on the edge endpoints returned by
                        gof_tetmesh.marching_tetrahedra.
 * make_integrate_fn == gaussian_renderer.integrate (gaussian_renderer/__init__.py:118-218) for plain tensors.
@@ -115,51 +116,74 @@ def _field_args(rs, points, means3D, opacities, scales, rotations, shs):
 
 class _OpacityField(torch.autograd.Function):
     """alpha = 1 - min over views of alpha_integrated (DESIGN.md 4.12), differentiable with respect to the points and the
-    Gaussians.  The forward keeps a running minimum and the winning view per point (8 bytes a point, nothing per view); the
-    backward rebuilds one view's query state at a time, on the points that view won."""
+    Gaussians; with return_color also the winning view's color_integrated (DESIGN.md 4.13).  The forward keeps a running minimum
+    and the winning view per point (8 bytes a point, 20 with the colour, nothing per view); the backward rebuilds one view's query
+    state at a time, on the points that view won."""
 
     @staticmethod
-    def forward(ctx, points, means3D, opacities, scales, rotations, shs, views, settings_for_view, group):
+    def forward(ctx, points, means3D, opacities, scales, rotations, shs, views, settings_for_view, group, return_color):
         import diff_gaussian_rasterization as dgr
         from diff_gaussian_rasterization import _C
         rank, world = _world(group)
         n, dev = points.shape[0], points.device
         alpha_min = torch.ones(n, dtype=torch.float32, device=dev)
         argmin = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev)
+        color = torch.ones(n, 3, dtype=torch.float32, device=dev) if return_color else None
         views = list(views)
         for vi in range(rank, len(views), world):
             rs = settings_for_view(views[vi])
             args = _field_args(rs, points, means3D, opacities, scales, rotations, shs) + (vi, alpha_min, argmin)
-            dgr._call_native(_C.integrate_gaussians_to_points_min, args, rs.debug, "snapshot_fw.dump", "forward")
+            dgr._call_native(_C.integrate_gaussians_to_points_min, args, rs.debug, "snapshot_fw.dump", "forward",
+                             **({"color_min": color} if return_color else {}))
         if world > 1:
             # evaluate_alpha's merge: the global minimum, won by the lowest view index that attains it (and is < 1)
             local = alpha_min.clone()
             dist.all_reduce(alpha_min, op=dist.ReduceOp.MIN, group=group)
-            argmin = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
+            cand = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
+            argmin = cand.clone()
             dist.all_reduce(argmin, op=dist.ReduceOp.MIN, group=group)
+            if return_color:   # the winner's rank contributes its colour, as in evaluate_alpha
+                won = argmin < _NO_VIEW
+                contrib = torch.where(((cand == argmin) & won).reshape(-1, 1), color, torch.zeros_like(color))
+                dist.all_reduce(contrib, op=dist.ReduceOp.SUM, group=group)
+                color = torch.where(won.reshape(-1, 1), contrib, torch.ones_like(contrib))
         ctx.save_for_backward(points, means3D, opacities, scales, rotations, shs, argmin)
         ctx.views, ctx.settings_for_view, ctx.group = views, settings_for_view, group
-        return 1 - alpha_min
+        if not return_color:
+            return 1 - alpha_min
+        ctx.set_materialize_grads(False)
+        return 1 - alpha_min, color
 
     @staticmethod
-    def backward(ctx, grad_alpha):
+    def backward(ctx, grad_alpha, grad_color=None):
         import diff_gaussian_rasterization as dgr
         from diff_gaussian_rasterization import _C
         points, means3D, opacities, scales, rotations, shs, argmin = ctx.saved_tensors
         rank, world = _world(ctx.group)
         need = ctx.needs_input_grad
-        gaussians = any(need[1:5])
+        gaussians = any(need[1:6])
         n, P, dev = points.shape[0], means3D.shape[0], points.device
-        dA = -grad_alpha.to(torch.float32).contiguous()   # d alpha / d alpha_min = -1, at each point's winning view only
+        if grad_alpha is None:
+            grad_alpha = torch.zeros(n, dtype=torch.float32, device=dev)
+        with_color = grad_color is not None
+        # d alpha / d alpha_min = -1, at each point's winning view only; the colour's gradient goes to the same view
+        dA = -grad_alpha.to(torch.float32).contiguous()
+        dC = grad_color.to(torch.float32).contiguous() if with_color else None
         if world > 1:
-            # a rank runs the backward of the views it owns only, so it needs every rank's dL/dalpha: the gradients are those of
-            # the sum of the ranks' losses
-            dA = dA.clone()
-            dist.all_reduce(dA, op=dist.ReduceOp.SUM, group=ctx.group)
+            # a rank runs the backward of the views it owns only, so it needs every rank's dL/dalpha (and dL/dcolour): the
+            # gradients are those of the sum of the ranks' losses
+            if with_color:
+                dAC = torch.cat([dA.view(-1, 1), dC.view(-1, 3)], 1)
+                dist.all_reduce(dAC, op=dist.ReduceOp.SUM, group=ctx.group)
+                dA, dC = dAC[:, 0].contiguous(), dAC[:, 1:].contiguous()
+            else:
+                dA = dA.clone()
+                dist.all_reduce(dA, op=dist.ReduceOp.SUM, group=ctx.group)
         # one flat buffer: a single all-reduce carries every gradient across ranks
-        sizes = (3 * n, 3 * P, P, 3 * P, 4 * P)
+        n_sh = shs.numel() if with_color and need[5] else 0
+        sizes = (3 * n, 3 * P, P, 3 * P, 4 * P, n_sh)
         flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
-        g_pts, g_means, g_op, g_scales, g_rot = torch.split(flat, sizes)
+        g_pts, g_means, g_op, g_scales, g_rot, g_sh = torch.split(flat, sizes)
         g_pts, g_means, g_scales, g_rot = g_pts.view(n, 3), g_means.view(P, 3), g_scales.view(P, 3), g_rot.view(P, 4)
         if n and P:
             colors, scales_, rotations_, cov3D, v2g, shs_ = _field_inputs(scales, rotations, shs)
@@ -179,8 +203,16 @@ class _OpacityField(torch.autograd.Function):
                 bargs = dgr._integrate_backward_args(rs, p, means3D, radii, colors, scales_, rotations_, cov3D, v2g, shs_, dA[sel], R,
                                                      geom, binning, img, pts, pbin)
                 del geom, binning, img, pts, pbin
-                dp, dop, dm, dsc, drot, _dcov, _dv2g = dgr._call_native(
-                    _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward", points_grad=need[0])
+                if with_color:
+                    dp, dop, dm, dsc, drot, _dcov, _dv2g, _dcol, dsh = dgr._call_native(
+                        _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward",
+                        points_grad=need[0], dL_dcolor=dC[sel])
+                    if n_sh:
+                        g_sh += dsh.view(-1)
+                else:
+                    dp, dop, dm, dsc, drot, _dcov, _dv2g = dgr._call_native(
+                        _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward",
+                        points_grad=need[0])
                 del bargs   # the state goes back to the scratch pool before the next view
                 if dp is not None:
                     g_pts[sel] = dp
@@ -193,10 +225,11 @@ class _OpacityField(torch.autograd.Function):
             dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=ctx.group)
         pick = lambda g, i, like: g.view_as(like) if need[i] else None   # noqa: E731
         return (pick(g_pts, 0, points), pick(g_means, 1, means3D), pick(g_op, 2, opacities), pick(g_scales, 3, scales),
-                pick(g_rot, 4, rotations), None, None, None, None)
+                pick(g_rot, 4, rotations), g_sh.view_as(shs) if n_sh else None, None, None, None, None)
 
 
-def opacity_field(points, means3D, opacities, scales, rotations, shs, sh_degree, views, settings_for_view, group=None):
+def opacity_field(points, means3D, opacities, scales, rotations, shs, sh_degree, views, settings_for_view, group=None,
+                  return_color=False):
     """The multi-view opacity field alpha [N] = 1 - min over views of alpha_integrated: the tensor
     evaluate_alpha(points, views, make_integrate_fn(means3D, opacities, scales, rotations, shs, sh_degree, settings_for_view),
     group=group) returns, bit for bit, but differentiable with respect to points, means3D, opacities, scales and rotations
@@ -211,8 +244,13 @@ def opacity_field(points, means3D, opacities, scales, rotations, shs, sh_degree,
     field.  The gradients are those of the SUM of the ranks' losses: the backward all-reduces dL/dalpha before it runs each
     rank's views, and all-reduces the gradients after, so every rank's .grad is the single-GPU gradient of that sum, up to
     summation order.  A rank without a loss of its own backpropagates zeros (e.g. (alpha * 0).sum()); a loss computed
-    identically on every rank counts once per rank (divide it by the world size, or compute it on one rank only)."""
-    return _OpacityField.apply(points, means3D, opacities, scales, rotations, shs, views, settings_for_view, group)
+    identically on every rank counts once per rank (divide it by the world size, or compute it on one rank only).
+
+    return_color=True returns (alpha, colour [N,3]): the colour evaluate_alpha(..., return_color=True) returns, bit for bit --
+    the winning view's color_integrated, (1, 1, 1) where no view lowered the minimum (DESIGN.md 4.13).  Its gradient reaches
+    means3D, opacities, scales, rotations and shs through the winning view only; the points get nothing from it (the colour
+    is piecewise constant in the point).  With a group, dL/dcolour is all-reduced together with dL/dalpha."""
+    return _OpacityField.apply(points, means3D, opacities, scales, rotations, shs, views, settings_for_view, group, return_color)
 
 
 class CachedIntegrator:

@@ -200,6 +200,18 @@ GOF_API int gof_integrate_min(const gof_scene_t* scene, int PN, const float* poi
                   gof_alloc_fn point_binning_alloc, void* point_binning_user,
                   int* radii, float* alpha_min, int* argmin, void* stream);
 
+/* gof_integrate_min that also keeps the winning view's colour (no reference counterpart; DESIGN section 4.13): whenever a view
+ * updates alpha_min[k] / argmin[k], color_min [PN,3] (initialised by the caller, to 1 for evaluate_alpha's field) takes that view's
+ * color_integrated of the point, C + T*bg of its pixel exactly as gof_integrate writes it.  color_min NULL fails with
+ * GOF_E_INVALID; everything else as gof_integrate_min. */
+GOF_API int gof_integrate_min_color(const gof_scene_t* scene, int PN, const float* points3D, int view,
+                  gof_alloc_fn geom_alloc, void* geom_user,
+                  gof_alloc_fn binning_alloc, void* binning_user,
+                  gof_alloc_fn image_alloc, void* image_user,
+                  gof_alloc_fn point_alloc, void* point_user,
+                  gof_alloc_fn point_binning_alloc, void* point_binning_user,
+                  int* radii, float* alpha_min, int* argmin, float* color_min, void* stream);
+
 /* The backward of gof_integrate (no reference counterpart; DESIGN section 4.11): dL_dalpha [PN], the gradient of a loss with respect
  * to out_alpha_integrated, -> the gradients with respect to the points and the Gaussians.  With each point's contributor list,
  * the alpha rejects and the alpha and depth clamps held fixed, d alpha_integrated / d alpha_j = prod_{i != j} (1 - alpha_i).
@@ -217,6 +229,21 @@ GOF_API int gof_integrate_backward(const gof_scene_t* scene, int PN, const float
                   void* point_binning_buffer, const float* dL_dalpha, float* dL_dpoints3D, float* dL_dopacity,
                   float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
                   void* scratch, size_t scratch_bytes, void* stream);
+
+/* gof_integrate_backward that also differentiates out_color_integrated (no reference counterpart; DESIGN section 4.13).  A point's
+ * colour is C + T*bg of its pixel's centre ray, so dL_dcolor_integrated [PN,3] is summed per pixel (in double, in a fixed order)
+ * and taken through that ray's blend with its Gaussians, rejects and clamps held fixed: dC/dc_j = T_j alpha_j and dC/dalpha_j =
+ * T_j c_j - (sum_{i>j} T_i alpha_i c_i + T bg) / (1 - alpha_j).  dL_dalpha [PN] and dL_dcolor_integrated may each be NULL (no
+ * loss on that output; both NULL writes zeros).  dL_dcolors [P,3] receives dL/dcolors_precomp, or without them the colour's
+ * gradient before the SH evaluation; dL_dsh [P,M,3] (required with SHs, zeros above the active degree) and the SH-direction term
+ * of dL_dmean3D follow as in gof_rasterize_backward.  The points receive nothing from the colour (it is piecewise constant in the
+ * point): dL_dpoints3D is the alpha's, bit for bit.  The Gaussian sums use double atomics (reproducible up to summation order).
+ * Every other argument, the scratch (gof_integrate_backward_scratch_bytes) and the argument checks are gof_integrate_backward's. */
+GOF_API int gof_integrate_backward_color(const gof_scene_t* scene, int PN, const float* points3D, int num_rendered, const int* radii,
+                  void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
+                  void* point_binning_buffer, const float* dL_dalpha, const float* dL_dcolor_integrated, float* dL_dpoints3D,
+                  float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
+                  float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes, void* stream);
 
 /* The same query with the Gaussian side cached per view.  extract_mesh.py:56,92,107 calls integrate for the SAME views ten
  * times (tetrahedra vertices, 8 bisection steps, colours) -- only points3D changes, so preprocess / depth sort / instance

@@ -1,9 +1,9 @@
-"""Cost of the opacity-field query's backward (DESIGN.md 4.11): one view of a C5-sized scene (3 M Gaussians, 1920x1080) queried
-at N points sampled around the Gaussians' centres.  Times, with CUDA events around single calls after warm-up: the plain
+"""Cost of the opacity-field query's backward (DESIGN.md 4.11, 4.13): one view of a C5-sized scene (3 M Gaussians, 1920x1080)
+queried at N points sampled around the Gaussians' centres.  Times, with CUDA events around single calls after warm-up: the plain
 forward (`_C.integrate_gaussians_to_points`), the forward that keeps its state (`integrate_gaussians_to_points_state`) and the
-backward (`integrate_gaussians_to_points_backward`), alternating; medians and spreads, plus the per-kernel split of the library's
-event brackets (integrate vs integrate_bwd + preprocess_bwd).  Checks that the point gradients of two backward calls are
-bit-identical.
+backward (`integrate_gaussians_to_points_backward`) of an alpha loss, of a colour loss and of both, alternating; medians and
+spreads, plus the per-kernel split of the library's event brackets (integrate vs integrate_bwd / integrate_bwd_color +
+preprocess_bwd).  Checks that the point gradients of two backward calls are bit-identical.
 
   python tools/integrate_grad_bench.py [--config C5] [--view 5] [--points 2000000] [--reps 20]
 
@@ -56,12 +56,16 @@ def main():
           cam.world_view_transform.to(dev), cam.full_proj_transform.to(dev), cam.tanfovx, cam.tanfovy, 0.0,
           torch.zeros((H, W, 2), device=dev), H, W, g["shs"], gs["sh_degree"], cam.camera_center.to(dev), False, False)
     dL = torch.randn(a.points, generator=torch.Generator().manual_seed(2)).to(dev)
+    dC = torch.randn(a.points, 3, generator=torch.Generator().manual_seed(3)).to(dev)
+    losses = dict(backward=(dL, None), backward_color=(None, dC), backward_both=(dL, dC))
 
-    def bwd(state):
+    def bwd(state, mode="backward"):
         R, _c, _a, _ci, radii, geom, binning, img, pt, pbin = state
         (bg, p3, m3, col, op, sc, rot, sm, cov, v2g, vm, pm, tfx, tfy, ks, sub, H_, W_, sh, deg, cp, _pf, dbg) = ia
+        da, dc = losses[mode]
+        kw = {} if dc is None else dict(dL_dcolor=dc)
         return _C.integrate_gaussians_to_points_backward(bg, p3, m3, radii, col, sc, rot, sm, cov, v2g, vm, pm, tfx, tfy, ks, sub, H_,
-                                                         W_, sh, deg, cp, dL, R, geom, binning, img, pt, pbin, dbg)
+                                                         W_, sh, deg, cp, da, R, geom, binning, img, pt, pbin, dbg, **kw)
 
     def timed(fn):
         s, t = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -75,25 +79,29 @@ def main():
     for _ in range(3):
         _C.integrate_gaussians_to_points(*ia)
         state = _C.integrate_gaussians_to_points_state(*ia)
-        bwd(state)
+        for mode in losses:
+            bwd(state, mode)
     torch.cuda.synchronize()
-    t = dict(forward=[], forward_state=[], backward=[])
+    t = dict(forward=[], forward_state=[], backward=[], backward_color=[], backward_both=[])
     first = None
     for _ in range(a.reps):
         t["forward"].append(timed(lambda: _C.integrate_gaussians_to_points(*ia))[0])
         ms, state = timed(lambda: _C.integrate_gaussians_to_points_state(*ia))
         t["forward_state"].append(ms)
-        ms, g_ = timed(lambda: bwd(state))
-        t["backward"].append(ms)
-        if first is None:
-            first = g_[0].clone()
-        else:
-            assert torch.equal(first, g_[0]), "point gradients of two backward calls differ"
+        for mode in losses:   # the backward reads the forward state and rewrites only its own scratch: one state serves all three
+            ms, g_ = timed(lambda: bwd(state, mode))
+            t[mode].append(ms)
+            if mode == "backward_color":
+                assert not bool(g_[0].any()), "a colour loss moved the points"
+            elif first is None:
+                first = g_[0].clone()
+            else:
+                assert torch.equal(first, g_[0]), "point gradients of two backward calls differ"
     _C.profile_reset()
     _C.profile_enable(True)
-    for _ in range(5):
-        state = _C.integrate_gaussians_to_points_state(*ia)
-        bwd(state)
+    state = _C.integrate_gaussians_to_points_state(*ia)
+    for mode in losses:   # one bracketed call of each kernel
+        bwd(state, mode)
     torch.cuda.synchronize()
     rep = _C.profile_report()
     _C.profile_enable(False)
@@ -103,10 +111,10 @@ def main():
         summary[f"{k}_ms_median"] = round(float(np.median(v)), 3)
         summary[f"{k}_ms_spread"] = [round(float(v.min()), 3), round(float(v.max()), 3)]
         print(f"{k:14s} median {np.median(v):8.3f} ms  min {v.min():8.3f}  max {v.max():8.3f}")
-    for k in ("integrate", "integrate_bwd", "preprocess_bwd", "preprocess_points", "preprocess_fwd"):
+    for k in ("integrate", "integrate_bwd", "integrate_bwd_color", "preprocess_bwd", "preprocess_points", "preprocess_fwd"):
         if k in rep:
             summary[f"kernel_{k}_ms"] = round(rep[k][1] / rep[k][0], 3)
-            print(f"kernel {k:18s} {rep[k][1] / rep[k][0]:8.3f} ms")
+            print(f"kernel {k:20s} {rep[k][1] / rep[k][0]:8.3f} ms  ({rep[k][0]} calls)")
     print(json.dumps(summary))
 
 

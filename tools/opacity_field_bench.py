@@ -3,7 +3,7 @@
 
 Times, with CUDA events after warm-up, alternating: the plain multi-view query (`evaluate_alpha` over
 `GaussianRasterizer.integrate`, one call per view), the forward of `gof_extract.opacity_field` (one `gof_integrate_min` per
-view) and its backward.  Reports ms per view for both forwards, the backward's ms in all and per winning view, and the
+view), the same forward with `return_color=True` (one `gof_integrate_min_color` per view, DESIGN.md 4.13) and the backward.  Reports ms per view for both forwards, the backward's ms in all and per winning view, and the
 per-kernel split of the library's event brackets.  Then the peak `torch.cuda.max_memory_allocated` growth over forward and
 backward of `opacity_field` against the naive composition (per-view `integrate_gaussians` kept by autograd, torch.min).  Checks
 that the field equals evaluate_alpha bit for bit and that the point gradients of two backward calls are bit-identical.
@@ -69,8 +69,9 @@ def main():
         q = {k: v.clone().requires_grad_(k != "shs") for k, v in g.items()}
         return pts.clone().requires_grad_(True), q
 
-    def field(p, q):
-        return gof_extract.opacity_field(p, q["means3D"], q["opacities"], q["scales"], q["rotations"], q["shs"], gs["sh_degree"], cams, sf)
+    def field(p, q, return_color=False):
+        return gof_extract.opacity_field(p, q["means3D"], q["opacities"], q["scales"], q["rotations"], q["shs"], gs["sh_degree"], cams, sf,
+                                         return_color=return_color)
 
     def timed(fn):
         s, t = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -84,8 +85,13 @@ def main():
         plain()
         p, q = leaves()
         (field(p, q) * dL).sum().backward()
+        with torch.no_grad():
+            field(p, q, True)
     torch.cuda.synchronize()
-    t = dict(plain=[], forward=[], backward=[])
+    with torch.no_grad():
+        fn = gof_extract.make_integrate_fn(g["means3D"], g["opacities"], g["scales"], g["rotations"], g["shs"], gs["sh_degree"], sf)
+        ref_color = gof_extract.evaluate_alpha(pts, cams, fn, return_color=True)[1]
+    t = dict(plain=[], forward=[], forward_color=[], backward=[])
     first = None
     for _ in range(a.reps):
         ms, ref = timed(plain)
@@ -94,6 +100,11 @@ def main():
         ms, alpha = timed(lambda: field(p, q))
         t["forward"].append(ms)
         assert torch.equal(alpha.detach(), ref), "opacity_field differs from evaluate_alpha"
+        with torch.no_grad():
+            ms, (alpha_c, color) = timed(lambda: field(p, q, True))
+        t["forward_color"].append(ms)
+        assert torch.equal(alpha_c, ref) and torch.equal(color, ref_color), "return_color differs from evaluate_alpha"
+        del alpha_c, color
         ms, _ = timed(lambda: (alpha * dL).sum().backward())
         t["backward"].append(ms)
         if first is None:
@@ -105,6 +116,8 @@ def main():
     plain()
     p, q = leaves()
     (field(p, q) * dL).sum().backward()
+    with torch.no_grad():
+        field(p, q, True)
     torch.cuda.synchronize()
     rep = _C.profile_report()
     _C.profile_enable(False)
@@ -122,10 +135,12 @@ def main():
         print(f"{k:10s} median {np.median(v):9.3f} ms  min {v.min():9.3f}  max {v.max():9.3f}")
     summary["plain_ms_per_view"] = round(summary["plain_ms_median"] / a.views, 3)
     summary["forward_ms_per_view"] = round(summary["forward_ms_median"] / a.views, 3)
+    summary["forward_color_ms_per_view"] = round(summary["forward_color_ms_median"] / a.views, 3)
     summary["backward_ms_per_winning_view"] = round(summary["backward_ms_median"] / max(winners, 1), 3)
-    print(f"per view: plain {summary['plain_ms_per_view']} ms, opacity_field forward {summary['forward_ms_per_view']} ms; backward "
+    print(f"per view: plain {summary['plain_ms_per_view']} ms, opacity_field forward {summary['forward_ms_per_view']} ms, with "
+          f"return_color {summary['forward_color_ms_per_view']} ms; backward "
           f"{summary['backward_ms_per_winning_view']} ms per winning view ({winners} of {a.views})")
-    for k in ("integrate", "integrate_min", "integrate_bwd", "preprocess_bwd", "preprocess_points", "preprocess_fwd"):
+    for k in ("integrate", "integrate_min", "integrate_min_color", "integrate_bwd", "preprocess_bwd", "preprocess_points", "preprocess_fwd"):
         if k in rep:
             summary[f"kernel_{k}_ms"] = round(rep[k][1] / rep[k][0], 3)
             print(f"kernel {k:18s} {rep[k][1] / rep[k][0]:8.3f} ms  ({rep[k][0]} launches)")
