@@ -196,7 +196,7 @@ void gof_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* gof_last_error(void) { return g_err; }
-extern "C" int gof_version(void) { return 100; }
+extern "C" int gof_version(void) { return 101; }
 
 static int validate_scene(const gof_scene_t* s) {
   if (!s) { gof_set_error("scene is NULL"); return GOF_E_INVALID; }
@@ -305,85 +305,68 @@ extern "C" int gof_rasterize_forward(const gof_scene_t* s, gof_alloc_fn geom_all
   return gof_launch_render_forward(s, v, g.geom, g.GL, g.bin, g.BL, g.img, g.IL, out_color, st);
 }
 
-extern "C" int gof_rasterize_backward(const gof_scene_t* s, int num_rendered, const int* radii,
-                                      void* geom_buffer, const void* binning_buffer,
-                                      const void* image_buffer, const float* dL_dpix, float* dL_dmean2D,
-                                      float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D,
-                                      float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-                                      float* dL_dview2gaussian, void* stream) {
-  return gof_rasterize_backward_stats(s, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic,
-                                      dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dview2gaussian,
-                                      nullptr, nullptr, stream);
-}
-
-extern "C" int gof_rasterize_backward_stats(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
-                                            const void* binning_buffer, const void* image_buffer, const float* dL_dpix,
-                                            float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                            float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-                                            float* dL_dview2gaussian, float* dens_sum, float* dens_max, void* stream) {
-  return gof_rasterize_backward_dp(s, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic,
-                                   dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dview2gaussian, dens_sum,
-                                   dens_max, nullptr, nullptr, stream);
-}
-
-// Where the intrinsics scratch keeps the camera pass's rows (first) and the ray pass's per-pixel values (256-byte aligned after them)
+// Where the focal-length scratch keeps the camera pass's rows (first) and the ray pass's per-pixel values (256-byte aligned after them)
 static size_t intrinsics_camera_bytes(int P) { return (gof_camera_grad_scratch_bytes(P) + 255) / 256 * 256; }
 
-// The backward of every entry point: _dp's argument list plus the camera gradient (dL_dviewmatrix / dL_dcampos, both or neither) and
-// the focal-length gradient (dL_dtan_fov; its scratch also carries the camera pass's rows).
-static int rasterize_backward(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer, const void* binning_buffer,
-                              const void* image_buffer, const float* dL_dpix, float* dL_dmean2D, float* dL_dopacity, float* dL_dcolor,
-                              float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-                              float* dL_dview2gaussian, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
-                              float* dL_dviewmatrix, float* dL_dcampos, void* cam_scratch, size_t cam_scratch_bytes, float* dL_dtan_fov,
-                              void* stream) {
+extern "C" size_t gof_rasterize_backward_scratch_bytes(int P, int width, int height, int camera, int intrinsics) {
+  if (P <= 0) return 0;
+  if (intrinsics) return width > 0 && height > 0 ? intrinsics_camera_bytes(P) + gof_ray_grad_scratch_bytes(width, height) : 0;
+  return camera ? gof_camera_grad_scratch_bytes(P) : 0;
+}
+
+extern "C" int gof_rasterize_backward_ex(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
+                                         const void* binning_buffer, const void* image_buffer, const float* dL_dpix,
+                                         const gof_backward_out_t* out, void* stream) {
+  if (!out) { gof_set_error("backward: out is NULL"); return GOF_E_INVALID; }
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
-  const bool camera = dL_dviewmatrix != nullptr;
-  const bool intrinsics = dL_dtan_fov != nullptr;
-  if (camera != (dL_dcampos != nullptr)) {
+  const gof_backward_out_t& o = *out;
+  const bool camera = o.dL_dviewmatrix != nullptr;
+  const bool intrinsics = o.dL_dtan_fov != nullptr;
+  if (camera != (o.dL_dcampos != nullptr)) {
     gof_set_error("backward: dL_dviewmatrix and dL_dcampos come together");
     return GOF_E_INVALID;
   }
-  double* rays = nullptr;
-  if (intrinsics) {
-    const size_t need = gof_rasterize_backward_intrinsics_scratch_bytes(s->P, s->width, s->height);
-    if (cam_scratch_bytes < need) {
-      gof_set_error("backward: intrinsics scratch of %zu bytes, %zu needed (gof_rasterize_backward_intrinsics_scratch_bytes)",
-                    cam_scratch_bytes, need);
-      return GOF_E_INVALID;
-    }
-    if (s->P > 0 && !cam_scratch) { gof_set_error("backward: intrinsics scratch is NULL"); return GOF_E_INVALID; }
-    if (s->P > 0) rays = reinterpret_cast<double*>(static_cast<char*>(cam_scratch) + intrinsics_camera_bytes(s->P));
-  } else if (camera && cam_scratch_bytes < gof_camera_grad_scratch_bytes(s->P)) {
-    gof_set_error("backward: camera scratch of %zu bytes, %zu needed (gof_rasterize_backward_camera_scratch_bytes)", cam_scratch_bytes,
-                  gof_camera_grad_scratch_bytes(s->P));
+  if ((o.sh_rgb || o.sh_hdr) && (camera || intrinsics)) {
+    gof_set_error("backward: sh_rgb / sh_hdr do not combine with the camera or focal-length gradient");
     return GOF_E_INVALID;
   }
-  if (camera && s->P > 0 && !cam_scratch) { gof_set_error("backward: camera scratch is NULL"); return GOF_E_INVALID; }
-  if (s->P == 0) {   // rasterize_points.cu:172; the camera and focal-length gradients of no Gaussians are zero
-    if (camera) {
-      GOF_CUDA_OK(cudaMemsetAsync(dL_dviewmatrix, 0, 16 * sizeof(float), (cudaStream_t)stream));
-      GOF_CUDA_OK(cudaMemsetAsync(dL_dcampos, 0, 3 * sizeof(float), (cudaStream_t)stream));
-    }
-    if (intrinsics) GOF_CUDA_OK(cudaMemsetAsync(dL_dtan_fov, 0, 2 * sizeof(float), (cudaStream_t)stream));
-    return GOF_OK;
-  }
-  if (!radii || !geom_buffer || !image_buffer || !dL_dpix || !dL_dmean2D || !dL_dopacity || !dL_dcolor ||
-      !dL_dmean3D || !dL_dview2gaussian || (num_rendered > 0 && !binning_buffer)) {
-    gof_set_error("backward: NULL argument");
+  const size_t need = gof_rasterize_backward_scratch_bytes(s->P, s->width, s->height, camera, intrinsics);
+  if ((camera || intrinsics) && o.scratch_bytes < need) {
+    gof_set_error("backward: %s scratch of %zu bytes, %zu needed (gof_rasterize_backward_scratch_bytes)",
+                  intrinsics ? "intrinsics" : "camera", o.scratch_bytes, need);
     return GOF_E_INVALID;
   }
-  if (s->shs && !dL_dsh && !(sh_rgb && sh_hdr)) { gof_set_error("backward: dL_dsh (or sh_rgb + sh_hdr) required with SHs"); return GOF_E_INVALID; }
-  if ((sh_rgb != nullptr) != (sh_hdr != nullptr) || (sh_rgb && !s->shs)) {
-    gof_set_error("backward: sh_rgb and sh_hdr come together and need SHs");
-    return GOF_E_INVALID;
-  }
-  if (s->scales && s->rotations && (!dL_dscale || !dL_drot)) {
-    gof_set_error("backward: dL_dscale / dL_drot required");
+  if ((camera || intrinsics) && s->P > 0 && !o.scratch) {
+    gof_set_error("backward: %s scratch is NULL", intrinsics ? "intrinsics" : "camera");
     return GOF_E_INVALID;
   }
   cudaStream_t st = (cudaStream_t)stream;
+  if (s->P == 0) {   // rasterize_points.cu:172; the camera and focal-length gradients of no Gaussians are zero
+    if (camera) {
+      GOF_CUDA_OK(cudaMemsetAsync(o.dL_dviewmatrix, 0, 16 * sizeof(float), st));
+      GOF_CUDA_OK(cudaMemsetAsync(o.dL_dcampos, 0, 3 * sizeof(float), st));
+    }
+    if (intrinsics) GOF_CUDA_OK(cudaMemsetAsync(o.dL_dtan_fov, 0, 2 * sizeof(float), st));
+    return GOF_OK;
+  }
+  if (!radii || !geom_buffer || !image_buffer || !dL_dpix || !o.dL_dmean2D || !o.dL_dopacity || !o.dL_dcolor ||
+      !o.dL_dmean3D || !o.dL_dview2gaussian || (num_rendered > 0 && !binning_buffer)) {
+    gof_set_error("backward: NULL argument");
+    return GOF_E_INVALID;
+  }
+  if (s->shs && !o.dL_dsh && !(o.sh_rgb && o.sh_hdr)) {
+    gof_set_error("backward: dL_dsh (or sh_rgb + sh_hdr) required with SHs");
+    return GOF_E_INVALID;
+  }
+  if ((o.sh_rgb != nullptr) != (o.sh_hdr != nullptr) || (o.sh_rgb && !s->shs)) {
+    gof_set_error("backward: sh_rgb and sh_hdr come together and need SHs");
+    return GOF_E_INVALID;
+  }
+  if (s->scales && s->rotations && (!o.dL_dscale || !o.dL_drot)) {
+    gof_set_error("backward: dL_dscale / dL_drot required");
+    return GOF_E_INVALID;
+  }
   const GofView v = gof_make_view(s);
   const GofGeomLayout GL = gof_geom_layout((size_t)s->P);
   const GofImageLayout IL = gof_image_layout(s->width, s->height);
@@ -391,56 +374,31 @@ static int rasterize_backward(const gof_scene_t* s, int num_rendered, const int*
   // The geometry buffer is the caller's scratch for this view: its last section holds the blend kernel's 64-byte
   // per-Gaussian accumulator rows, zeroed and filled by every backward call (the forward state in it is only read).
   char* geom = static_cast<char*>(geom_buffer);
+  double* rays = intrinsics ? reinterpret_cast<double*>(static_cast<char*>(o.scratch) + intrinsics_camera_bytes(s->P)) : nullptr;
   if ((rc = gof_launch_render_backward(s, v, geom, GL, (const char*)binning_buffer, BL, (const char*)image_buffer, IL, dL_dpix,
-                                       rays, dL_dtan_fov, st)) != GOF_OK)
+                                       rays, o.dL_dtan_fov, st)) != GOF_OK)
     return rc;
-  return gof_launch_preprocess_backward(s, v, geom, GL, radii, dL_dmean2D, dL_dopacity, dL_dcolor, dL_dview2gaussian, dL_dmean3D,
-                                        dL_dsh, dL_dscale, dL_drot, dL_dcov3D, dens_sum, dens_max, sh_rgb, sh_hdr, dL_dviewmatrix,
-                                        dL_dcampos, cam_scratch, st);
+  return gof_launch_preprocess_backward(s, v, geom, GL, radii, o.dL_dmean2D, o.dL_dopacity, o.dL_dcolor, o.dL_dview2gaussian,
+                                        o.dL_dmean3D, o.dL_dsh, o.dL_dscale, o.dL_drot, o.dL_dcov3D, o.dens_sum, o.dens_max, o.sh_rgb,
+                                        o.sh_hdr, o.dL_dviewmatrix, o.dL_dcampos, o.scratch, st);
 }
 
-extern "C" int gof_rasterize_backward_dp(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
-                                         const void* binning_buffer, const void* image_buffer, const float* dL_dpix,
-                                         float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                         float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-                                         float* dL_dview2gaussian, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
-                                         void* stream) {
+extern "C" int gof_rasterize_backward(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
+                                      const void* binning_buffer, const void* image_buffer, const float* dL_dpix, float* dL_dmean2D,
+                                      float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                                      float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, void* stream) {
   (void)dL_dconic;
-  return rasterize_backward(s, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dopacity,
-                            dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dview2gaussian, dens_sum, dens_max, sh_rgb,
-                            sh_hdr, nullptr, nullptr, nullptr, 0, nullptr, stream);
-}
-
-extern "C" size_t gof_rasterize_backward_camera_scratch_bytes(int P) { return gof_camera_grad_scratch_bytes(P); }
-
-extern "C" int gof_rasterize_backward_camera(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
-                                             const void* binning_buffer, const void* image_buffer, const float* dL_dpix,
-                                             float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                             float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-                                             float* dL_dview2gaussian, float* dens_sum, float* dens_max, float* dL_dviewmatrix,
-                                             float* dL_dcampos, void* scratch, size_t scratch_bytes, void* stream) {
-  (void)dL_dconic;
-  return rasterize_backward(s, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dopacity,
-                            dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dview2gaussian, dens_sum, dens_max, nullptr,
-                            nullptr, dL_dviewmatrix, dL_dcampos, scratch, scratch_bytes, nullptr, stream);
-}
-
-extern "C" size_t gof_rasterize_backward_intrinsics_scratch_bytes(int P, int width, int height) {
-  return P > 0 && width > 0 && height > 0 ? intrinsics_camera_bytes(P) + gof_ray_grad_scratch_bytes(width, height) : 0;
-}
-
-extern "C" int gof_rasterize_backward_intrinsics(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
-                                                 const void* binning_buffer, const void* image_buffer, const float* dL_dpix,
-                                                 float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                                 float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-                                                 float* dL_dview2gaussian, float* dens_sum, float* dens_max, float* dL_dviewmatrix,
-                                                 float* dL_dcampos, float* dL_dtan_fov, void* scratch, size_t scratch_bytes,
-                                                 void* stream) {
-  (void)dL_dconic;
-  if (!dL_dtan_fov) { gof_set_error("backward: dL_dtan_fov is NULL"); return GOF_E_INVALID; }
-  return rasterize_backward(s, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dopacity,
-                            dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dview2gaussian, dens_sum, dens_max, nullptr,
-                            nullptr, dL_dviewmatrix, dL_dcampos, scratch, scratch_bytes, dL_dtan_fov, stream);
+  gof_backward_out_t o{};
+  o.dL_dmean2D = dL_dmean2D;
+  o.dL_dopacity = dL_dopacity;
+  o.dL_dcolor = dL_dcolor;
+  o.dL_dmean3D = dL_dmean3D;
+  o.dL_dcov3D = dL_dcov3D;
+  o.dL_dsh = dL_dsh;
+  o.dL_dscale = dL_dscale;
+  o.dL_drot = dL_drot;
+  o.dL_dview2gaussian = dL_dview2gaussian;
+  return gof_rasterize_backward_ex(s, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, &o, stream);
 }
 
 extern "C" int gof_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
@@ -554,12 +512,12 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
 }
 
 // One view of the multi-view opacity field (DESIGN.md 4.12): gof_integrate's Gaussian and point sides, then k_integrate<true>
-// folds each projecting point's alpha into alpha_min / argmin instead of writing the query's outputs.
-// with_color: gof_integrate_min_color, k_integrate<true, true> also writes the winner's colour to color_min (DESIGN.md 4.13)
-static int integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc, void* geom_user,
-                         gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc, void* image_user,
-                         gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc, void* point_binning_user,
-                         int* radii, float* alpha_min, int* argmin, bool with_color, float* color_min, void* stream) {
+// folds each projecting point's alpha into alpha_min / argmin instead of writing the query's outputs.  With color_min,
+// k_integrate<true, true> also writes the winner's colour there (DESIGN.md 4.13).
+extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
+                                 void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
+                                 void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
+                                 void* point_binning_user, int* radii, float* alpha_min, int* argmin, float* color_min, void* stream) {
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
   if (!geom_alloc || !binning_alloc || !image_alloc || !point_alloc || !point_binning_alloc) {
@@ -571,7 +529,7 @@ static int integrate_min(const gof_scene_t* s, int PN, const float* points3D, in
     return GOF_E_INVALID;
   }
   if (s->P == 0 || PN <= 0) return GOF_OK;
-  if (!points3D || !radii || !alpha_min || !argmin || (with_color && !color_min)) {
+  if (!points3D || !radii || !alpha_min || !argmin) {
     gof_set_error("integrate_min: NULL argument");
     return GOF_E_INVALID;
   }
@@ -582,39 +540,23 @@ static int integrate_min(const gof_scene_t* s, int PN, const float* points3D, in
   if ((rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.5f, false,
                           &num_rendered, st, g)) != GOF_OK)
     return rc;
-  const GofIntMin mn{alpha_min, argmin, view, with_color ? color_min : nullptr};
+  const GofIntMin mn{alpha_min, argmin, view, color_min};
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
                     g.IL, point_alloc, point_user, point_binning_alloc, point_binning_user, nullptr, nullptr, nullptr, &mn, st);
 }
 
-extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
-                                 void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
-                                 void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
-                                 void* point_binning_user, int* radii, float* alpha_min, int* argmin, void* stream) {
-  return integrate_min(s, PN, points3D, view, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, point_alloc,
-                       point_user, point_binning_alloc, point_binning_user, radii, alpha_min, argmin, false, nullptr, stream);
-}
-
-extern "C" int gof_integrate_min_color(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
-                                       void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
-                                       void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
-                                       void* point_binning_user, int* radii, float* alpha_min, int* argmin, float* color_min,
-                                       void* stream) {
-  return integrate_min(s, PN, points3D, view, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, point_alloc,
-                       point_user, point_binning_alloc, point_binning_user, radii, alpha_min, argmin, true, color_min, stream);
-}
-
 extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
 
-// with_color: gof_integrate_backward_color (DESIGN.md 4.13): dL_dalpha and dL_dcolor_int may be NULL, dL_dcolors is required and
-// dL_dsh too with SHs
-static int integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
-                              void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
-                              void* point_binning_buffer, const float* dL_dalpha, const float* dL_dcolor_int, float* dL_dpoints3D,
-                              float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian,
-                              float* dL_dcov3D, bool with_color, float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes,
-                              void* stream) {
+// Colour mode (DESIGN.md 4.13), with dL_dcolor_int or dL_dcolors given: dL_dalpha and dL_dcolor_int may be NULL, dL_dcolors is
+// required and dL_dsh too with SHs.  Alpha mode reads neither dL_dcolors nor dL_dsh.
+extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
+                                      void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
+                                      void* point_binning_buffer, const float* dL_dalpha, const float* dL_dcolor_int, float* dL_dpoints3D,
+                                      float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian,
+                                      float* dL_dcov3D, float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes,
+                                      void* stream) {
+  const bool with_color = dL_dcolor_int || dL_dcolors;
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
   if (PN < 0) { gof_set_error("integrate_backward: PN < 0"); return GOF_E_INVALID; }
@@ -675,29 +617,7 @@ static int integrate_backward(const gof_scene_t* s, int PN, const float* points3
                                        reinterpret_cast<const uint2*>(static_cast<const char*>(image_buffer) + IL.ranges),
                                        static_cast<const char*>(point_buffer), PL, static_cast<char*>(point_binning_buffer), PBL,
                                        dL_dalpha, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale, dL_drot, dL_dview2gaussian,
-                                       dL_dcov3D, with_color ? dL_dcolor_int : nullptr, with_color ? dL_dcolors : nullptr,
-                                       with_color ? dL_dsh : nullptr, scratch, st);
-}
-
-extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
-                                      void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
-                                      void* point_binning_buffer, const float* dL_dalpha, float* dL_dpoints3D, float* dL_dopacity,
-                                      float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
-                                      void* scratch, size_t scratch_bytes, void* stream) {
-  return integrate_backward(s, PN, points3D, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, point_buffer,
-                            point_binning_buffer, dL_dalpha, nullptr, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale, dL_drot,
-                            dL_dview2gaussian, dL_dcov3D, false, nullptr, nullptr, scratch, scratch_bytes, stream);
-}
-
-extern "C" int gof_integrate_backward_color(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
-                                            void* geom_buffer, const void* binning_buffer, const void* image_buffer,
-                                            const void* point_buffer, void* point_binning_buffer, const float* dL_dalpha,
-                                            const float* dL_dcolor_integrated, float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D,
-                                            float* dL_dscale, float* dL_drot, float* dL_dview2gaussian, float* dL_dcov3D,
-                                            float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes, void* stream) {
-  return integrate_backward(s, PN, points3D, num_rendered, radii, geom_buffer, binning_buffer, image_buffer, point_buffer,
-                            point_binning_buffer, dL_dalpha, dL_dcolor_integrated, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale,
-                            dL_drot, dL_dview2gaussian, dL_dcov3D, true, dL_dcolors, dL_dsh, scratch, scratch_bytes, stream);
+                                       dL_dcov3D, dL_dcolor_int, dL_dcolors, with_color ? dL_dsh : nullptr, scratch, st);
 }
 
 // ---- the Gaussian side of the query, once per view --------------------------------------------------------------

@@ -239,7 +239,7 @@ struct PreBwdArgs {
   float* dL_dscale;
   float* dL_drot;
   float* dL_dcov3D;         // optional [P][6]: written as zeros
-  float* dens_sum;          // optional [P][3]: |dL_dmean2D.xy|, |dL_dmean2D.z|, 1 for visible Gaussians (gof_rasterize_backward_stats)
+  float* dens_sum;          // optional [P][3]: |dL_dmean2D.xy|, |dL_dmean2D.z|, 1 for visible Gaussians (gof_backward_out_t::dens_sum)
   float* dens_max;          // optional [P][2]: |dL_dmean2D.z|, radius
   float* sh_rgb;            // optional [3][GOF_SH_PLANE(P)] planes: the clamp-masked dL_dRGB the SH gradient is the outer product of
   float* sh_hdr;            //   (view-parallel exchange, csrc/sh_views.cu); sh_hdr[0..3] = camera centre, active degree.  dL_dsh may be NULL.

@@ -40,6 +40,14 @@ class _Scene(ctypes.Structure):
     ]
 
 
+class _BackwardOut(ctypes.Structure):
+    """gof_backward_out_t: the outputs of gof_rasterize_backward_ex."""
+    _fields_ = [(n, _fp) for n in (
+        "dL_dmean2D", "dL_dopacity", "dL_dcolor", "dL_dmean3D", "dL_dcov3D", "dL_dsh", "dL_dscale", "dL_drot", "dL_dview2gaussian",
+        "dens_sum", "dens_max", "sh_rgb", "sh_hdr", "dL_dviewmatrix", "dL_dcampos", "dL_dtan_fov", "scratch")] + \
+        [("scratch_bytes", ctypes.c_size_t)]
+
+
 class _StateView(ctypes.Structure):
     _fields_ = [(n, _fp) for n in (
         "depths", "means2D", "conic_opacity", "rgb", "view2gaussian", "clamped", "tiles_touched",
@@ -51,20 +59,11 @@ _lib.gof_rasterize_forward.restype = ctypes.c_int
 _lib.gof_rasterize_forward.argtypes = [
     ctypes.POINTER(_Scene), _ALLOC_FN, ctypes.c_void_p, _ALLOC_FN, ctypes.c_void_p, _ALLOC_FN, ctypes.c_void_p,
     _fp, _fp, ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
-_lib.gof_rasterize_backward.restype = ctypes.c_int
-_lib.gof_rasterize_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 15 + [ctypes.c_void_p]
-_lib.gof_rasterize_backward_stats.restype = ctypes.c_int
-_lib.gof_rasterize_backward_stats.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 17 + [ctypes.c_void_p]
-_lib.gof_rasterize_backward_dp.restype = ctypes.c_int
-_lib.gof_rasterize_backward_dp.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 19 + [ctypes.c_void_p]
-_lib.gof_rasterize_backward_camera_scratch_bytes.restype = ctypes.c_size_t
-_lib.gof_rasterize_backward_camera_scratch_bytes.argtypes = [ctypes.c_int]
-_lib.gof_rasterize_backward_camera.restype = ctypes.c_int
-_lib.gof_rasterize_backward_camera.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 20 + [ctypes.c_size_t, ctypes.c_void_p]
-_lib.gof_rasterize_backward_intrinsics_scratch_bytes.restype = ctypes.c_size_t
-_lib.gof_rasterize_backward_intrinsics_scratch_bytes.argtypes = [ctypes.c_int] * 3
-_lib.gof_rasterize_backward_intrinsics.restype = ctypes.c_int
-_lib.gof_rasterize_backward_intrinsics.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [_fp] * 21 + [ctypes.c_size_t, ctypes.c_void_p]
+_lib.gof_rasterize_backward_scratch_bytes.restype = ctypes.c_size_t
+_lib.gof_rasterize_backward_scratch_bytes.argtypes = [ctypes.c_int] * 5
+_lib.gof_rasterize_backward_ex.restype = ctypes.c_int
+_lib.gof_rasterize_backward_ex.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, _fp, _fp, _fp, _fp, ctypes.POINTER(_BackwardOut),
+                                           ctypes.c_void_p]
 _lib.gof_sh_grad_from_views.restype = ctypes.c_int
 _lib.gof_sh_grad_from_views.argtypes = [ctypes.c_int] * 3 + [_fp, ctypes.c_void_p, _fp, ctypes.c_void_p]
 _lib.gof_mark_visible.restype = ctypes.c_int
@@ -260,9 +259,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  binningBuffer, imageBuffer, debug, _out=None, _camera=False, _intrinsics=False, _ray_map=False):
     """RasterizeGaussiansBackwardCUDA (rasterize_points.cu:124-211).  Returns, in the reference's order
     (:210): (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
-    dL_drotations, dL_dview2gaussian).  `_camera=True` (extension, gof_rasterize_backward_camera) appends
+    dL_drotations, dL_dview2gaussian).  `_camera=True` (extension, gof_backward_out_t.dL_dviewmatrix / dL_dcampos) appends
     dL_dviewmatrix and dL_dcampos, shaped like viewmatrix and campos.  `_intrinsics=True` (extension,
-    gof_rasterize_backward_intrinsics) then appends dL_dtanfovx and dL_dtanfovy, 0-dim float32 tensors on the device.
+    gof_backward_out_t.dL_dtan_fov) then appends dL_dtanfovx and dL_dtanfovy, 0-dim float32 tensors on the device.
     `_ray_map=True` (tests only; needs _intrinsics) appends the per-pixel float64 [2,H,W] dL/drx, dL/dry of the call."""
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
@@ -346,7 +345,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         dL_dviewmatrix, dL_dcampos = cam_out[:16], cam_out[16:]
     if _intrinsics:
         fov_out = torch.empty(2, dtype=torch.float32, device=means3D.device)
-    if P != 0 or _camera or _intrinsics:   # with P == 0 the camera and intrinsics entry points write zeros
+    if P != 0 or _camera or _intrinsics:   # with P == 0 the library writes the camera and focal-length gradients as zeros
         g = dL_dout_color.contiguous()
         rad = radii.contiguous()
         with torch.cuda.device(means3D.device):
@@ -358,34 +357,28 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             if ds is not None and not (ds.is_contiguous() and dm.is_contiguous() and tuple(ds.shape) == (P, 3) and tuple(dm.shape) == (P, 2)
                                        and ds.dtype == torch.float32 and dm.dtype == torch.float32):
                 raise RuntimeError("gof_b200: dens_sum must be a contiguous float32 (P,3) and dens_max (P,2) tensor")
-            common = (ctypes.byref(s), int(R), _ptr(rad, torch.int32), _ptr(geomBuffer, torch.uint8),
-                      _ptr(binningBuffer, torch.uint8), _ptr(imageBuffer, torch.uint8), _ptr(g),
-                      dL_dmeans2D.data_ptr(), None, dL_dopacity.data_ptr(), dL_dcolors.data_ptr(),
-                      dL_dmeans3D.data_ptr(), dL_dcov3D.data_ptr(),
-                      (_ptr(full_t) if full_t is not None else None) if factored else _ptr(dL_dsh),
-                      dL_dscales.data_ptr(), dL_drotations.data_ptr(), dL_dv2g.data_ptr(),
-                      ds.data_ptr() if ds is not None else None, dm.data_ptr() if dm is not None else None)
-            if _intrinsics:
-                nbytes = int(_lib.gof_rasterize_backward_intrinsics_scratch_bytes(P, W, H))
-                scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=means3D.device)
-                _check(_lib.gof_rasterize_backward_intrinsics(*common, dL_dviewmatrix.data_ptr() if _camera else None,
-                                                              dL_dcampos.data_ptr() if _camera else None, fov_out.data_ptr(),
-                                                              scratch.data_ptr() if nbytes else None, nbytes, _stream()))
-            elif _camera:
-                nbytes = int(_lib.gof_rasterize_backward_camera_scratch_bytes(P))
-                scratch = torch.empty(nbytes, dtype=torch.uint8, device=means3D.device)
-                _check(_lib.gof_rasterize_backward_camera(*common, dL_dviewmatrix.data_ptr(), dL_dcampos.data_ptr(),
-                                                          scratch.data_ptr(), nbytes, _stream()))
-            else:
-                _check(_lib.gof_rasterize_backward_dp(*common, rgb_t.data_ptr() if factored else None,
-                                                      hdr_t.data_ptr() if factored else None, _stream()))
+            nbytes = int(_lib.gof_rasterize_backward_scratch_bytes(P, W, H, int(_camera), int(_intrinsics)))
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=means3D.device) if nbytes else None
+            o = _BackwardOut(
+                dL_dmean2D=dL_dmeans2D.data_ptr(), dL_dopacity=dL_dopacity.data_ptr(), dL_dcolor=dL_dcolors.data_ptr(),
+                dL_dmean3D=dL_dmeans3D.data_ptr(), dL_dcov3D=dL_dcov3D.data_ptr(),
+                dL_dsh=(_ptr(full_t) if full_t is not None else None) if factored else _ptr(dL_dsh),
+                dL_dscale=dL_dscales.data_ptr(), dL_drot=dL_drotations.data_ptr(), dL_dview2gaussian=dL_dv2g.data_ptr(),
+                dens_sum=ds.data_ptr() if ds is not None else None, dens_max=dm.data_ptr() if dm is not None else None,
+                sh_rgb=rgb_t.data_ptr() if factored else None, sh_hdr=hdr_t.data_ptr() if factored else None,
+                dL_dviewmatrix=dL_dviewmatrix.data_ptr() if _camera else None, dL_dcampos=dL_dcampos.data_ptr() if _camera else None,
+                dL_dtan_fov=fov_out.data_ptr() if _intrinsics else None,
+                scratch=scratch.data_ptr() if nbytes else None, scratch_bytes=nbytes)
+            _check(_lib.gof_rasterize_backward_ex(ctypes.byref(s), int(R), _ptr(rad, torch.int32), _ptr(geomBuffer, torch.uint8),
+                                                  _ptr(binningBuffer, torch.uint8), _ptr(imageBuffer, torch.uint8), _ptr(g),
+                                                  ctypes.byref(o), _stream()))
     grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations, dL_dv2g)
     if _camera:
         grads += (dL_dviewmatrix.view(viewmatrix.shape), dL_dcampos.view(campos.shape))
     if _intrinsics:
         grads += (fov_out[0], fov_out[1])
     if _ray_map:
-        # the per-pixel [2][H][W] doubles follow the camera pass's rows in the scratch (api.cu, intrinsics_camera_bytes)
+        # the per-pixel [2][H][W] doubles follow the camera pass's rows in the scratch (gof_backward_out_t.scratch)
         if P == 0:
             grads += (torch.zeros((2, H, W), dtype=torch.float64, device=means3D.device),)
         else:
@@ -454,10 +447,7 @@ def _integrate(background, points3D, means3D, colors, opacity, scales, rotations
 
 _lib.gof_integrate_min.restype = ctypes.c_int
 _lib.gof_integrate_min.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_ALLOC_FN, ctypes.c_void_p] * 5 + \
-    [_fp, _fp, _fp, ctypes.c_void_p]
-_lib.gof_integrate_min_color.restype = ctypes.c_int
-_lib.gof_integrate_min_color.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + \
-    [_ALLOC_FN, ctypes.c_void_p] * 5 + [_fp, _fp, _fp, _fp, ctypes.c_void_p]
+    [_fp, _fp, _fp, _fp, ctypes.c_void_p]
 
 
 def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier,
@@ -467,7 +457,7 @@ def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opa
     """gof_integrate_min (extension, DESIGN.md 4.12): integrate_gaussians_to_points for view index `view`, folded into the running
     minimum over views in place: where a point's alpha_integrated < alpha_min, alpha_min takes it and argmin takes `view`.
     alpha_min (float32 [PN], start at 1) and argmin (int32 [PN], start at 2^30) must be contiguous.  With color_min (float32
-    [PN,3], contiguous; gof_integrate_min_color, DESIGN.md 4.13) the same update also stores the point's color_integrated of
+    [PN,3], contiguous; DESIGN.md 4.13) the same update also stores the point's color_integrated of
     that view.  Returns radii [P]."""
     if points3D.ndimension() != 2 or points3D.size(1) != 3:
         raise RuntimeError("points3D must have dimensions (num_points, 3)")
@@ -491,23 +481,16 @@ def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opa
         p3 = points3D.contiguous()
         allocs = (geom.cb, None, binning.cb, None, img.cb, None, pts.cb, None, pbin.cb, None)
         with torch.cuda.device(dev):
-            if color_min is None:
-                _check(_lib.gof_integrate_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), *allocs, radii.data_ptr(),
-                                              _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev), _stream()))
-            else:
-                _check(_lib.gof_integrate_min_color(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), *allocs, radii.data_ptr(),
-                                                    _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev),
-                                                    _ptr(color_min, device=dev), _stream()))
+            _check(_lib.gof_integrate_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), *allocs, radii.data_ptr(),
+                                          _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev),
+                                          _ptr(color_min, device=dev), _stream()))
     return radii
 
 
 _lib.gof_integrate_backward_scratch_bytes.restype = ctypes.c_size_t
 _lib.gof_integrate_backward_scratch_bytes.argtypes = [ctypes.c_int]
 _lib.gof_integrate_backward.restype = ctypes.c_int
-_lib.gof_integrate_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 15 + \
-    [ctypes.c_size_t, ctypes.c_void_p]
-_lib.gof_integrate_backward_color.restype = ctypes.c_int
-_lib.gof_integrate_backward_color.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 18 + \
+_lib.gof_integrate_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 18 + \
     [ctypes.c_size_t, ctypes.c_void_p]
 
 
@@ -519,7 +502,7 @@ def integrate_gaussians_to_points_backward(background, points3D, means3D, radii,
     """gof_integrate_backward (extension, DESIGN.md 4.11): the gradient dL_dalpha [PN] of out_alpha_integrated ->
     (dL_dpoints3D [PN,3] or None, dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drotations [P,4],
     dL_dcov3D [P,6], dL_dview2gaussian [P,10]).  The state is what integrate_gaussians_to_points_state returned.
-    With dL_dcolor [PN,3], the gradient of out_color_integrated (gof_integrate_backward_color, DESIGN.md 4.13), dL_dalpha may be
+    With dL_dcolor [PN,3], the gradient of out_color_integrated (colour mode, DESIGN.md 4.13), dL_dalpha may be
     None, and two more outputs follow: dL_dcolors [P,3] and dL_dsh [P,M,3] (None without SHs)."""
     P, PN = means3D.size(0), points3D.size(0)
     keep = []
@@ -545,26 +528,21 @@ def integrate_gaussians_to_points_backward(background, points3D, means3D, radii,
     if g is not None and g.numel() != PN:
         raise RuntimeError(f"gof_b200: dL_dalpha has {g.numel()} elements, expected {PN}")
     has_sr = s.scales is not None and s.rotations is not None
-    buf = lambda t: t.data_ptr() if t is not None and t.numel() else None   # noqa: E731
-    head = (ctypes.byref(s), PN, _ptr(p3, device=dev), int(num_rendered), _ptr(radii.contiguous(), torch.int32), buf(geomBuffer),
-            buf(binningBuffer), buf(imgBuffer), buf(pointBuffer), buf(pointBinningBuffer), None if g is None else _ptr(g, device=dev))
-    grads = (dpts.data_ptr() if dpts is not None and PN else None, out["dopacity"].data_ptr() if P else None,
-             out["dmeans3D"].data_ptr() if P else None, out["dscales"].data_ptr() if P and has_sr else None,
-             out["drot"].data_ptr() if P and has_sr else None, out["dv2g"].data_ptr() if P else None,
-             out["dcov3D"].data_ptr() if P else None)
-    tail = (scratch.data_ptr() if nbytes else None, nbytes, _stream())
-    if not color:
-        with torch.cuda.device(dev):
-            _check(_lib.gof_integrate_backward(*head, *grads, *tail))
-    else:
+    gc = dcolors = dsh = None
+    if color:
         gc = _c(dL_dcolor)
         if gc.numel() != 3 * PN:
             raise RuntimeError(f"gof_b200: dL_dcolor has {gc.numel()} elements, expected {3 * PN}")
         dcolors = torch.empty((P, 3), dtype=torch.float32, device=dev)
         dsh = torch.empty((P, s.M, 3), dtype=torch.float32, device=dev) if s.M > 0 else None
-        with torch.cuda.device(dev):
-            _check(_lib.gof_integrate_backward_color(*head, _ptr(gc, device=dev), *grads, dcolors.data_ptr() if P else None,
-                                                     dsh.data_ptr() if dsh is not None and dsh.numel() else None, *tail))
+    buf = lambda t: t.data_ptr() if t is not None and t.numel() else None   # noqa: E731
+    with torch.cuda.device(dev):
+        _check(_lib.gof_integrate_backward(
+            ctypes.byref(s), PN, _ptr(p3, device=dev), int(num_rendered), _ptr(radii.contiguous(), torch.int32), buf(geomBuffer),
+            buf(binningBuffer), buf(imgBuffer), buf(pointBuffer), buf(pointBinningBuffer), _ptr(g, device=dev), _ptr(gc, device=dev),
+            buf(dpts), buf(out["dopacity"]), buf(out["dmeans3D"]), buf(out["dscales"]) if has_sr else None,
+            buf(out["drot"]) if has_sr else None, buf(out["dv2g"]), buf(out["dcov3D"]), buf(dcolors), buf(dsh),
+            scratch.data_ptr() if nbytes else None, nbytes, _stream()))
     if P and not has_sr:
         out["dscales"].zero_()
         out["drot"].zero_()

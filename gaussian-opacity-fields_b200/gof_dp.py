@@ -22,7 +22,7 @@ need each other's clamp-masked dL_dRGB -- 3 floats per Gaussian and view -- and 
 NVLink by the expansion kernel (peer-memory / NVLS exchange) or all-gathered (NCCL / gloo).
 
 The bucket also carries this view's densification statistics (written by the rasterizer backward itself, see
-gof_rasterize_backward_stats): `dens_sum` (P,3) = (|dL_dmean2D.xy|, |dL_dmean2D.z|, visible) reduced with SUM and `dens_max`
+gof_backward_out_t.dens_sum / dens_max): `dens_sum` (P,3) = (|dL_dmean2D.xy|, |dL_dmean2D.z|, visible) reduced with SUM and `dens_max`
 (P,2) = (|dL_dmean2D.z|, radius) reduced with MAX -- what GaussianModel.add_densification_stats and train.py:255 accumulate.
 """
 import ctypes

@@ -1,21 +1,15 @@
-"""CPU: the float64 camera-gradient oracle (tests/_camera_oracle.py) against central differences, and the C ABI of
-gof_rasterize_backward_camera.
+"""CPU: the float64 camera-gradient oracle (tests/_camera_oracle.py) against central differences (the C ABI's checks are in
+test_backward_abi.py).
 
 The oracle's camera terms are Jacobian-vector products of the loss L = sum_g <dL_dv2g_g, view2gaussian_g(vm)> +
 <dL_dRGB_g, rgb_g(campos)> (dL_dRGB masked by the clamp flags), so for any direction u, <dL_dvm, u> and <dL_dcampos, u>
 must match (L(x + h u) - L(x - h u)) / 2h of a float64 evaluation of view2gaussian and of the SH colour."""
-import ctypes
-import os
-
 import numpy as np
 import pytest
 
 import _camera_oracle as co
 import gof_oracle
 import gof_synth
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "gaussian-opacity-fields_b200", "diff_gaussian_rasterization", "libgof_b200.so")
 
 
 def _scene(D, precomp=None, seed=0, P=96):
@@ -114,77 +108,3 @@ def test_sh_rgb_restatement_matches_the_oracle_forward():
     rgb = np.maximum(co.sh_rgb(a["means3D"][vis], a["cam_pos"], a["shs"][vis], 3), 0.0)
     assert np.allclose(rgb, g["rgb"][vis], rtol=0, atol=1e-5)
 
-
-# ---- the C ABI ----------------------------------------------------------------------------------------------------------
-
-class _Scene(ctypes.Structure):
-    _fields_ = [("P", ctypes.c_int), ("D", ctypes.c_int), ("M", ctypes.c_int), ("width", ctypes.c_int), ("height", ctypes.c_int),
-                ("tan_fovx", ctypes.c_float), ("tan_fovy", ctypes.c_float), ("kernel_size", ctypes.c_float),
-                ("scale_modifier", ctypes.c_float)] + [(n, ctypes.c_void_p) for n in (
-                    "background", "means3D", "shs", "colors_precomp", "opacities", "scales", "rotations", "cov3D_precomp",
-                    "view2gaussian_precomp", "viewmatrix", "projmatrix", "cam_pos", "subpixel_offset")] + \
-               [("prefiltered", ctypes.c_int), ("debug", ctypes.c_int)]
-
-
-def _lib():
-    assert os.path.exists(LIB), "build the library first: python gaussian-opacity-fields_b200/build.py"
-    lib = ctypes.CDLL(LIB)
-    lib.gof_rasterize_backward_camera_scratch_bytes.restype = ctypes.c_size_t
-    lib.gof_rasterize_backward_camera_scratch_bytes.argtypes = [ctypes.c_int]
-    fp = ctypes.c_void_p
-    lib.gof_rasterize_backward_camera.restype = ctypes.c_int
-    lib.gof_rasterize_backward_camera.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [fp] * 20 + [ctypes.c_size_t, fp]
-    lib.gof_rasterize_backward_stats.restype = ctypes.c_int
-    lib.gof_rasterize_backward_stats.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [fp] * 17 + [fp]
-    lib.gof_last_error.restype = ctypes.c_char_p
-    return lib
-
-
-def test_camera_entry_point_is_exported():
-    lib = _lib()
-    assert hasattr(lib, "gof_rasterize_backward_camera") and hasattr(lib, "gof_rasterize_backward_camera_scratch_bytes")
-
-
-@pytest.mark.parametrize("P,rows", [(-1, 0), (0, 0), (1, 1), (127, 1), (128, 1), (129, 2), (1_000_000, 7813)])
-def test_scratch_query_is_one_row_of_16_doubles_per_128_gaussians(P, rows):
-    assert _lib().gof_rasterize_backward_camera_scratch_bytes(P) == rows * 16 * 8
-
-
-def _fake_scene(P):
-    """A scene whose pointers pass validation; the calls below fail before any of them is dereferenced."""
-    s = _Scene()
-    s.P, s.D, s.M, s.width, s.height = P, 3, 16, 64, 48
-    s.tan_fovx = s.tan_fovy = 0.5
-    s.scale_modifier = 1.0
-    for n in ("background", "means3D", "shs", "opacities", "scales", "rotations", "viewmatrix", "projmatrix", "cam_pos"):
-        setattr(s, n, 256)
-    return s
-
-
-def test_both_null_is_the_stats_entry_point():
-    """With dL_dviewmatrix = dL_dcampos = NULL the call is gof_rasterize_backward_stats: the same checks, the same errors
-    (only argument errors here, found before anything is launched; the outputs are compared on the GPU)."""
-    lib = _lib()
-    s = _fake_scene(300)
-    for missing in (2, 7, 10):   # radii, dL_dmean2D, dL_dcolor
-        base = [ctypes.byref(s), 0, 256, 256, None, 256, 256, 256, None, 256, 256, 256, None, 256, 256, 256, 256]
-        base[missing] = None
-        rc_s = lib.gof_rasterize_backward_stats(*base, None, None, None)
-        err_s = lib.gof_last_error()
-        rc_c = lib.gof_rasterize_backward_camera(*base, None, None, None, None, None, 0, None)
-        err_c = lib.gof_last_error()
-        assert rc_s == rc_c == -1 and err_s == err_c == b"backward: NULL argument"
-
-
-def test_camera_arguments_are_checked():
-    lib = _lib()
-    s = _fake_scene(300)
-    base = [ctypes.byref(s), 0, 256, 256, None, 256, 256, 256, None, 256, 256, 256, None, 256, 256, 256, 256, None, None]
-    need = int(lib.gof_rasterize_backward_camera_scratch_bytes(300))
-    assert lib.gof_rasterize_backward_camera(*base, 256, None, 256, need, None) == -1
-    assert b"come together" in lib.gof_last_error()
-    assert lib.gof_rasterize_backward_camera(*base, None, 256, 256, need, None) == -1
-    assert lib.gof_rasterize_backward_camera(*base, 256, 512, 256, need - 1, None) == -1
-    assert b"scratch" in lib.gof_last_error()
-    assert lib.gof_rasterize_backward_camera(*base, 256, 512, None, need, None) == -1
-    assert b"scratch" in lib.gof_last_error()

@@ -1,5 +1,5 @@
-"""CPU: the float64 ray-gradient oracle (tests/focal_oracle/focal_oracle.c) against a complex-step derivative, and the C ABI of
-gof_rasterize_backward_intrinsics.
+"""CPU: the float64 ray-gradient oracle (tests/focal_oracle/focal_oracle.c) against a complex-step derivative (the C ABI's checks
+are in test_backward_abi.py).
 
 The oracle's per-pixel dL/drx, dL/dry (DESIGN.md 4.10) is checked against an independent float64 restatement of one pixel's
 compositing, differentiated by the complex step Im L(rx + ih) / h, which has no cancellation.  The restatement keeps the pixel's
@@ -8,8 +8,6 @@ the power <= 0 clamp subtract a real constant (the backward differentiates opaci
 T alpha and the pixel's final A and D are constants, and channel 7 is ignored.  Branches (the clamps, and through the fixed
 list the 1/255 and near-plane gates) are taken on the real part."""
 import cmath
-import ctypes
-import os
 
 import numpy as np
 import pytest
@@ -18,8 +16,6 @@ import _focal_oracle as fo
 import gof_oracle
 import gof_synth
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "gaussian-opacity-fields_b200", "diff_gaussian_rasterization", "libgof_b200.so")
 ALPHA_MAX = float(np.float32(0.99))
 H_STEP = 1e-30
 
@@ -130,90 +126,3 @@ def test_oracle_matches_the_complex_step(seed, view):
     f = fo.rays(sc.W, sc.H, sc.tan_fovx, sc.tan_fovy, st, sc.arr["background"], dL, float_geometry=True)
     assert np.allclose(f["drays"], d["drays"], rtol=0, atol=float(1e-3 * d["mag"].max()))
 
-
-# ---- the C ABI ----------------------------------------------------------------------------------------------------------
-
-class _Scene(ctypes.Structure):
-    _fields_ = [("P", ctypes.c_int), ("D", ctypes.c_int), ("M", ctypes.c_int), ("width", ctypes.c_int), ("height", ctypes.c_int),
-                ("tan_fovx", ctypes.c_float), ("tan_fovy", ctypes.c_float), ("kernel_size", ctypes.c_float),
-                ("scale_modifier", ctypes.c_float)] + [(n, ctypes.c_void_p) for n in (
-                    "background", "means3D", "shs", "colors_precomp", "opacities", "scales", "rotations", "cov3D_precomp",
-                    "view2gaussian_precomp", "viewmatrix", "projmatrix", "cam_pos", "subpixel_offset")] + \
-               [("prefiltered", ctypes.c_int), ("debug", ctypes.c_int)]
-
-
-def _lib():
-    assert os.path.exists(LIB), "build the library first: python gaussian-opacity-fields_b200/build.py"
-    lib = ctypes.CDLL(LIB)
-    fp = ctypes.c_void_p
-    lib.gof_rasterize_backward_intrinsics_scratch_bytes.restype = ctypes.c_size_t
-    lib.gof_rasterize_backward_intrinsics_scratch_bytes.argtypes = [ctypes.c_int] * 3
-    lib.gof_rasterize_backward_intrinsics.restype = ctypes.c_int
-    lib.gof_rasterize_backward_intrinsics.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [fp] * 21 + [ctypes.c_size_t, fp]
-    lib.gof_rasterize_backward_stats.restype = ctypes.c_int
-    lib.gof_rasterize_backward_stats.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int] + [fp] * 17 + [fp]
-    lib.gof_last_error.restype = ctypes.c_char_p
-    return lib
-
-
-def test_intrinsics_entry_point_is_exported():
-    lib = _lib()
-    assert hasattr(lib, "gof_rasterize_backward_intrinsics") and hasattr(lib, "gof_rasterize_backward_intrinsics_scratch_bytes")
-
-
-@pytest.mark.parametrize("P,W,H", [(-1, 64, 48), (0, 64, 48), (5, 0, 48), (5, 64, -1), (1, 16, 16), (129, 203, 117),
-                                   (1_000_000, 1920, 1080)])
-def test_scratch_query_is_16_bytes_per_pixel_plus_the_camera_rows(P, W, H):
-    """The camera pass's rows (one row of 16 doubles per 128 Gaussians, padded to 256 bytes), then [2][H][W] doubles of dL/dr
-    and [tiles][2] doubles of tile sums; zero when there is nothing to render."""
-    got = _lib().gof_rasterize_backward_intrinsics_scratch_bytes(P, W, H)
-    if P <= 0 or W <= 0 or H <= 0:
-        assert got == 0
-        return
-    cam = -(-((P + 127) // 128 * 128) // 256) * 256
-    tiles = ((W + 15) // 16) * ((H + 15) // 16)
-    assert got == cam + 16 * W * H + 16 * tiles
-
-
-def _fake_scene(P):
-    """A scene whose pointers pass validation; the calls below fail before any of them is dereferenced."""
-    s = _Scene()
-    s.P, s.D, s.M, s.width, s.height = P, 3, 16, 64, 48
-    s.tan_fovx = s.tan_fovy = 0.5
-    s.scale_modifier = 1.0
-    for n in ("background", "means3D", "shs", "opacities", "scales", "rotations", "viewmatrix", "projmatrix", "cam_pos"):
-        setattr(s, n, 256)
-    return s
-
-
-def _base(s):
-    return [ctypes.byref(s), 0, 256, 256, None, 256, 256, 256, None, 256, 256, 256, None, 256, 256, 256, 256, None, None]
-
-
-def test_intrinsics_arguments_are_checked():
-    lib = _lib()
-    s = _fake_scene(300)
-    need = int(lib.gof_rasterize_backward_intrinsics_scratch_bytes(300, 64, 48))
-    base = _base(s)
-    assert lib.gof_rasterize_backward_intrinsics(*base, None, None, None, 256, need, None) == -1
-    assert b"dL_dtan_fov" in lib.gof_last_error()
-    assert lib.gof_rasterize_backward_intrinsics(*base, 256, None, 512, 256, need, None) == -1
-    assert b"come together" in lib.gof_last_error()
-    assert lib.gof_rasterize_backward_intrinsics(*base, None, None, 512, 256, need - 1, None) == -1
-    assert b"scratch" in lib.gof_last_error()
-    assert lib.gof_rasterize_backward_intrinsics(*base, 256, 512, 768, None, need, None) == -1
-    assert b"scratch" in lib.gof_last_error()
-
-
-def test_other_arguments_are_checked_like_the_stats_entry_point():
-    lib = _lib()
-    s = _fake_scene(300)
-    need = int(lib.gof_rasterize_backward_intrinsics_scratch_bytes(300, 64, 48))
-    for missing in (2, 7, 10):   # radii, dL_dmean2D, dL_dcolor
-        base = _base(s)[:17]
-        base[missing] = None
-        rc_s = lib.gof_rasterize_backward_stats(*base, None, None, None)
-        err_s = lib.gof_last_error()
-        rc_i = lib.gof_rasterize_backward_intrinsics(*base, None, None, None, None, 512, 1024, need, None)
-        err_i = lib.gof_last_error()
-        assert rc_s == rc_i == -1 and err_s == err_i == b"backward: NULL argument"

@@ -1,4 +1,4 @@
-"""GPU: the camera gradient of the backward (gof_rasterize_backward_camera, DESIGN.md 4.9).
+"""GPU: the camera gradient of the backward (gof_backward_out_t.dL_dviewmatrix / dL_dcampos, DESIGN.md 4.9).
 
 (a) The 19 values against the float64 oracle (tests/_camera_oracle.py) fed with this backward's own dL_dview2gaussian and
     dL_dcolors, as test_gpu_grad_stagewise feeds the preprocess backward.  The allowance of each value is the sum over the

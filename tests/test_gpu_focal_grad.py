@@ -1,4 +1,4 @@
-"""GPU: the focal-length gradient of the backward (gof_rasterize_backward_intrinsics, DESIGN.md 4.10).
+"""GPU: the focal-length gradient of the backward (gof_backward_out_t.dL_dtan_fov, DESIGN.md 4.10).
 
 (a) Every pixel's dL/drx, dL/dry (the [2,H,W] map the call leaves in its scratch) against the float64 oracle
     (tests/focal_oracle/focal_oracle.c) run from this library's own forward state with the same dL_dpix:

@@ -1,6 +1,6 @@
 """CPU: the float64 oracle of the query's colour backward (tests/integrate_grad_oracle/integrate_color_oracle.c, DESIGN.md 4.13) against central
 differences of a float64 restatement of one pixel's compositing with its blended set held fixed, and the argument checks of
-gof_integrate_backward_color and gof_integrate_min_color through the built library (decided before any device work)."""
+gof_integrate_backward and gof_integrate_min with the colour through the built library (decided before any device work)."""
 import ctypes
 
 import numpy as np
@@ -120,7 +120,7 @@ def test_transmittance_skip_is_followed_by_accepted_pairs():
     assert np.all(o["dcol"][2] == 0) and np.all(o["dv2g"][2] == 0) and np.all(o["dcol"][3] != 0)
 
 
-# ---------------- argument checks of the two C entries ----------------
+# ---------------- argument checks of the two C entries with the colour ----------------
 FAKE = 0x1000
 
 
@@ -148,10 +148,9 @@ def _bwd(_C, s, PN=4, scratch=FAKE, nbytes=10 ** 6, **kw):
     a = dict(points=FAKE, radii=FAKE, geom=FAKE, binning=FAKE, image=FAKE, pts=FAKE, pbin=FAKE, dalpha=FAKE, dcolor=FAKE,
              dpts=FAKE, dop=FAKE, dmean=FAKE, dscale=FAKE, drot=FAKE, dv2g=FAKE, dcov=FAKE, dcolors=FAKE, dsh=FAKE)
     a.update(kw)
-    return _C._lib.gof_integrate_backward_color(ctypes.byref(s), PN, a["points"], 1, a["radii"], a["geom"], a["binning"], a["image"],
-                                                a["pts"], a["pbin"], a["dalpha"], a["dcolor"], a["dpts"], a["dop"], a["dmean"],
-                                                a["dscale"], a["drot"], a["dv2g"], a["dcov"], a["dcolors"], a["dsh"], scratch, nbytes,
-                                                None)
+    return _C._lib.gof_integrate_backward(ctypes.byref(s), PN, a["points"], 1, a["radii"], a["geom"], a["binning"], a["image"],
+                                          a["pts"], a["pbin"], a["dalpha"], a["dcolor"], a["dpts"], a["dop"], a["dmean"], a["dscale"],
+                                          a["drot"], a["dv2g"], a["dcov"], a["dcolors"], a["dsh"], scratch, nbytes, None)
 
 
 def test_backward_color_refusals():
@@ -172,7 +171,7 @@ def test_backward_color_refusals():
     bad = _scene(_C)
     bad.P = -1
     assert _bwd(_C, bad) == -1
-    assert _C._lib.gof_integrate_backward_color(None, 4, *[FAKE] * 2, 1, *[FAKE] * 18, FAKE, 10 ** 6, None) == -1
+    assert _C._lib.gof_integrate_backward(None, 4, *[FAKE] * 2, 1, *[FAKE] * 18, FAKE, 10 ** 6, None) == -1
 
 
 def test_min_color_refusals():
@@ -183,8 +182,8 @@ def test_min_color_refusals():
 
     def call(PN=4, view=0, allocs=None, points=FAKE, radii=FAKE, amin=FAKE, argmin=FAKE, cmin=FAKE):
         allocs = allocs if allocs is not None else m._Allocs(_C)
-        return _C._lib.gof_integrate_min_color(ctypes.byref(s), PN, points, view, *allocs.args(), radii, amin, argmin, cmin, None)
-    for kw in (dict(points=None), dict(radii=None), dict(amin=None), dict(argmin=None), dict(cmin=None)):
+        return _C._lib.gof_integrate_min(ctypes.byref(s), PN, points, view, *allocs.args(), radii, amin, argmin, cmin, None)
+    for kw in (dict(points=None), dict(radii=None), dict(amin=None), dict(argmin=None)):
         assert call(**kw) == -1 and b"NULL" in err(), kw
     for view in (-1, 2 ** 30):
         assert call(view=view) == -1 and b"view" in err()

@@ -1,5 +1,5 @@
 """CPU: the float64 oracle of the opacity-field query's backward (DESIGN.md 4.11) against central differences of a float64
-restatement of one point's integration, and the argument checks of gof_integrate_backward.
+restatement of one point's integration, and the argument checks of gof_integrate_backward in alpha mode.
 
 The restatement holds the contributor list, the rejects and both clamps fixed, as the definition does; each case is built so
 that no decision lies within the finite-difference step of its threshold."""
@@ -158,7 +158,8 @@ def test_argument_checks():
     fake = ctypes.c_void_p(0x1000)
     for name in ("means3D", "opacities", "viewmatrix", "projmatrix", "background", "colors_precomp", "scales", "rotations"):
         setattr(s, name, fake.value)
-    args = [ctypes.byref(s), 4, fake.value, 1] + [fake.value] * 6 + [fake.value] * 8
+    # forward state; dL_dalpha, no dL_dcolor_integrated; the seven outputs; no dL_dcolors / dL_dsh (alpha mode)
+    args = [ctypes.byref(s), 4, fake.value, 1] + [fake.value] * 6 + [fake.value, None] + [fake.value] * 7 + [None, None]
     # a NULL or short scratch is refused before any work
     rc_null = _C._lib.gof_integrate_backward(*args, None, 10 ** 6, None)
     rc_short = _C._lib.gof_integrate_backward(*args, fake.value, 16, None)
@@ -177,6 +178,6 @@ def test_misaligned_rotation_gradient_is_refused():
     for name in ("means3D", "opacities", "viewmatrix", "projmatrix", "background", "colors_precomp", "scales", "rotations"):
         setattr(s, name, fake)
     drot = fake + 4
-    args = [ctypes.byref(s), 4, fake, 1] + [fake] * 6 + [fake] * 5 + [drot, fake, fake]
+    args = [ctypes.byref(s), 4, fake, 1] + [fake] * 6 + [fake, None] + [fake] * 4 + [drot, fake, fake] + [None, None]
     assert _C._lib.gof_integrate_backward(*args, fake, 10 ** 6, None) == -1
     assert b"aligned" in _C._lib.gof_last_error()

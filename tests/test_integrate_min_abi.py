@@ -45,9 +45,9 @@ class _Allocs:
         return out
 
 
-def _call(_C, s, PN=4, points=FAKE, view=0, allocs=None, radii=FAKE, alpha_min=FAKE, argmin=FAKE):
+def _call(_C, s, PN=4, points=FAKE, view=0, allocs=None, radii=FAKE, alpha_min=FAKE, argmin=FAKE, color_min=None):
     allocs = allocs if allocs is not None else _Allocs(_C)
-    return _C._lib.gof_integrate_min(ctypes.byref(s), PN, points, view, *allocs.args(), radii, alpha_min, argmin, None)
+    return _C._lib.gof_integrate_min(ctypes.byref(s), PN, points, view, *allocs.args(), radii, alpha_min, argmin, color_min, None)
 
 
 def test_null_buffers_are_refused():
@@ -103,7 +103,7 @@ def test_bad_scene_is_refused():
     s = _scene(_C)
     s.colors_precomp = None   # neither SHs nor colours
     assert _call(_C, s) == GOF_E_INVALID
-    assert _C._lib.gof_integrate_min(None, 4, FAKE, 0, *_Allocs(_C).args(), FAKE, FAKE, FAKE, None) == GOF_E_INVALID
+    assert _C._lib.gof_integrate_min(None, 4, FAKE, 0, *_Allocs(_C).args(), FAKE, FAKE, FAKE, None, None) == GOF_E_INVALID
 
 
 def test_binding_checks_the_running_minimum_tensors():

@@ -1,6 +1,6 @@
 """Cost of the camera gradient: the backward of one C3 view (1 M Gaussians, 1920x1080) with and without the camera outputs
-(`_C.rasterize_gaussians_backward(..., _camera=True)`, gof_rasterize_backward_camera), alternating calls over one forward
-state after warm-up.  CUDA events around single calls; medians and spreads are reported, plus the per-kernel split of the
+(`_C.rasterize_gaussians_backward(..., _camera=True)`, gof_rasterize_backward_ex with dL_dviewmatrix / dL_dcampos), alternating
+calls over one forward state after warm-up.  CUDA events around single calls; medians and spreads are reported, plus the per-kernel split of the
 library's event brackets (preprocess_bwd vs preprocess_bwd_camera + camera_grad_sum).
 
 Checks that the parameter gradients of the two variants are bit-identical wherever the blend stage (whose double atomics

@@ -1,5 +1,5 @@
 """Cost of the focal-length gradient: the backward of one C3 view (1 M Gaussians, 1920x1080) with and without the intrinsics
-outputs (`_C.rasterize_gaussians_backward(..., _intrinsics=True)`, gof_rasterize_backward_intrinsics), alternating calls over
+outputs (`_C.rasterize_gaussians_backward(..., _intrinsics=True)`, gof_rasterize_backward_ex with dL_dtan_fov), alternating calls over
 one forward state after warm-up.  CUDA events around single calls; medians and spreads are reported, plus the per-kernel split
 of the library's event brackets (render_bwd vs render_bwd_rays + focal_grad_sum).
 

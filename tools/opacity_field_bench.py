@@ -3,7 +3,7 @@
 
 Times, with CUDA events after warm-up, alternating: the plain multi-view query (`evaluate_alpha` over
 `GaussianRasterizer.integrate`, one call per view), the forward of `gof_extract.opacity_field` (one `gof_integrate_min` per
-view), the same forward with `return_color=True` (one `gof_integrate_min_color` per view, DESIGN.md 4.13) and the backward.  Reports ms per view for both forwards, the backward's ms in all and per winning view, and the
+view), the same forward with `return_color=True` (one `gof_integrate_min` with `color_min` per view, DESIGN.md 4.13) and the backward.  Reports ms per view for both forwards, the backward's ms in all and per winning view, and the
 per-kernel split of the library's event brackets.  Then the peak `torch.cuda.max_memory_allocated` growth over forward and
 backward of `opacity_field` against the naive composition (per-view `integrate_gaussians` kept by autograd, torch.min).  Checks
 that the field equals evaluate_alpha bit for bit and that the point gradients of two backward calls are bit-identical.
