@@ -196,7 +196,7 @@ void gof_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* gof_last_error(void) { return g_err; }
-extern "C" int gof_version(void) { return 101; }
+extern "C" int gof_version(void) { return 102; }
 
 static int validate_scene(const gof_scene_t* s) {
   if (!s) { gof_set_error("scene is NULL"); return GOF_E_INVALID; }
@@ -314,6 +314,17 @@ extern "C" size_t gof_rasterize_backward_scratch_bytes(int P, int width, int hei
   return camera ? gof_camera_grad_scratch_bytes(P) : 0;
 }
 
+// The checks of the Gaussian gradients that both backwards hand to k_preprocess_backward, which stores dL_drot as float4, and
+// dL_dsh too at M == 16 and degree 3.
+static int check_gaussian_grads(const char* who, const gof_scene_t* s, const gof_backward_out_t& o) {
+  const char* err = nullptr;
+  if (s->P > 0 && s->scales && s->rotations && (!o.dL_dscale || !o.dL_drot)) err = "dL_dscale / dL_drot required";
+  else if (reinterpret_cast<uintptr_t>(o.dL_drot) & 15) err = "dL_drot must be 16-byte aligned";
+  else if (s->shs && s->M == 16 && s->D == 3 && (reinterpret_cast<uintptr_t>(o.dL_dsh) & 15)) err = "dL_dsh must be 16-byte aligned";
+  if (err) gof_set_error("%s: %s", who, err);
+  return err ? GOF_E_INVALID : GOF_OK;
+}
+
 extern "C" int gof_rasterize_backward_ex(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
                                          const void* binning_buffer, const void* image_buffer, const float* dL_dpix,
                                          const gof_backward_out_t* out, void* stream) {
@@ -363,10 +374,7 @@ extern "C" int gof_rasterize_backward_ex(const gof_scene_t* s, int num_rendered,
     gof_set_error("backward: sh_rgb and sh_hdr come together and need SHs");
     return GOF_E_INVALID;
   }
-  if (s->scales && s->rotations && (!o.dL_dscale || !o.dL_drot)) {
-    gof_set_error("backward: dL_dscale / dL_drot required");
-    return GOF_E_INVALID;
-  }
+  if ((rc = check_gaussian_grads("backward", s, o)) != GOF_OK) return rc;
   const GofView v = gof_make_view(s);
   const GofGeomLayout GL = gof_geom_layout((size_t)s->P);
   const GofImageLayout IL = gof_image_layout(s->width, s->height);
@@ -378,9 +386,7 @@ extern "C" int gof_rasterize_backward_ex(const gof_scene_t* s, int num_rendered,
   if ((rc = gof_launch_render_backward(s, v, geom, GL, (const char*)binning_buffer, BL, (const char*)image_buffer, IL, dL_dpix,
                                        rays, o.dL_dtan_fov, st)) != GOF_OK)
     return rc;
-  return gof_launch_preprocess_backward(s, v, geom, GL, radii, o.dL_dmean2D, o.dL_dopacity, o.dL_dcolor, o.dL_dview2gaussian,
-                                        o.dL_dmean3D, o.dL_dsh, o.dL_dscale, o.dL_drot, o.dL_dcov3D, o.dens_sum, o.dens_max, o.sh_rgb,
-                                        o.sh_hdr, o.dL_dviewmatrix, o.dL_dcampos, o.scratch, st);
+  return gof_launch_preprocess_backward(s, geom, GL, radii, o, st);
 }
 
 extern "C" int gof_rasterize_backward(const gof_scene_t* s, int num_rendered, const int* radii, void* geom_buffer,
@@ -548,55 +554,49 @@ extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* poin
 
 extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
 
-// Colour mode (DESIGN.md 4.13), with dL_dcolor_int or dL_dcolors given: dL_dalpha and dL_dcolor_int may be NULL, dL_dcolors is
-// required and dL_dsh too with SHs.  Alpha mode reads neither dL_dcolors nor dL_dsh.
 extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float* points3D, int num_rendered, const int* radii,
                                       void* geom_buffer, const void* binning_buffer, const void* image_buffer, const void* point_buffer,
                                       void* point_binning_buffer, const float* dL_dalpha, const float* dL_dcolor_int, float* dL_dpoints3D,
-                                      float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot, float* dL_dview2gaussian,
-                                      float* dL_dcov3D, float* dL_dcolors, float* dL_dsh, void* scratch, size_t scratch_bytes,
-                                      void* stream) {
-  const bool with_color = dL_dcolor_int || dL_dcolors;
+                                      const gof_backward_out_t* out, void* stream) {
+  if (!out) { gof_set_error("integrate_backward: out is NULL"); return GOF_E_INVALID; }
+  const struct { const void* p; const char* name; } not_produced[] = {
+      {out->dL_dmean2D, "dL_dmean2D"}, {out->dens_sum, "dens_sum"}, {out->dens_max, "dens_max"}, {out->sh_rgb, "sh_rgb"},
+      {out->sh_hdr, "sh_hdr"}, {out->dL_dviewmatrix, "dL_dviewmatrix"}, {out->dL_dcampos, "dL_dcampos"}, {out->dL_dtan_fov, "dL_dtan_fov"}};
+  for (const auto& f : not_produced)
+    if (f.p) { gof_set_error("integrate_backward: out->%s must be NULL (not an output of this backward)", f.name); return GOF_E_INVALID; }
+  gof_backward_out_t o = *out;
+  const bool with_color = dL_dcolor_int || o.dL_dcolor;   // colour mode (DESIGN.md 4.13)
+  if (!with_color) o.dL_dsh = nullptr;                    // alpha mode does not read it
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
   if (PN < 0) { gof_set_error("integrate_backward: PN < 0"); return GOF_E_INVALID; }
   const size_t need = gof_integrate_backward_scratch(s->P);
-  if (scratch_bytes < need) {
-    gof_set_error("integrate_backward: scratch of %zu bytes, %zu needed (gof_integrate_backward_scratch_bytes)", scratch_bytes, need);
+  if (o.scratch_bytes < need) {
+    gof_set_error("integrate_backward: scratch of %zu bytes, %zu needed (gof_integrate_backward_scratch_bytes)", o.scratch_bytes, need);
     return GOF_E_INVALID;
   }
-  if (s->P > 0 && !scratch) { gof_set_error("integrate_backward: scratch is NULL"); return GOF_E_INVALID; }
+  if (s->P > 0 && !o.scratch) { gof_set_error("integrate_backward: scratch is NULL"); return GOF_E_INVALID; }
   const size_t P = (size_t)s->P;
-  if ((PN > 0 && !dL_dalpha && !with_color) || (P > 0 && (!dL_dopacity || !dL_dmean3D || !dL_dview2gaussian)) ||
-      (with_color && P > 0 && !dL_dcolors)) {
+  if ((PN > 0 && !dL_dalpha && !with_color) || (P > 0 && (!o.dL_dopacity || !o.dL_dmean3D || !o.dL_dview2gaussian)) ||
+      (with_color && P > 0 && !o.dL_dcolor)) {
     gof_set_error("integrate_backward: NULL argument");
     return GOF_E_INVALID;
   }
-  if (with_color && s->shs && P > 0 && !dL_dsh) {
-    gof_set_error("integrate_backward: dL_dsh required with SHs");
-    return GOF_E_INVALID;
-  }
-  if (s->scales && s->rotations && P > 0 && (!dL_dscale || !dL_drot)) {
-    gof_set_error("integrate_backward: dL_dscale / dL_drot required");
-    return GOF_E_INVALID;
-  }
-  if (reinterpret_cast<uintptr_t>(dL_drot) & 15) {   // k_preprocess_backward writes each rotation gradient as one float4
-    gof_set_error("integrate_backward: dL_drot must be 16-byte aligned");
-    return GOF_E_INVALID;
-  }
+  if (with_color && s->shs && P > 0 && !o.dL_dsh) { gof_set_error("integrate_backward: dL_dsh required with SHs"); return GOF_E_INVALID; }
+  if ((rc = check_gaussian_grads("integrate_backward", s, o)) != GOF_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   // P == 0 or PN == 0: gof_integrate ran nothing, no output depends on anything; likewise with no loss at all
   if (P == 0 || PN == 0 || (!dL_dalpha && !dL_dcolor_int)) {
     if (dL_dpoints3D && PN > 0) GOF_CUDA_OK(cudaMemsetAsync(dL_dpoints3D, 0, (size_t)PN * 12, st));
     if (P > 0) {
-      if (with_color) GOF_CUDA_OK(cudaMemsetAsync(dL_dcolors, 0, P * 12, st));
-      if (with_color && s->shs) GOF_CUDA_OK(cudaMemsetAsync(dL_dsh, 0, P * (size_t)s->M * 12, st));
-      GOF_CUDA_OK(cudaMemsetAsync(dL_dopacity, 0, P * 4, st));
-      GOF_CUDA_OK(cudaMemsetAsync(dL_dmean3D, 0, P * 12, st));
-      GOF_CUDA_OK(cudaMemsetAsync(dL_dview2gaussian, 0, P * 40, st));
-      if (dL_dscale) GOF_CUDA_OK(cudaMemsetAsync(dL_dscale, 0, P * 12, st));
-      if (dL_drot) GOF_CUDA_OK(cudaMemsetAsync(dL_drot, 0, P * 16, st));
-      if (dL_dcov3D) GOF_CUDA_OK(cudaMemsetAsync(dL_dcov3D, 0, P * 24, st));
+      if (with_color) GOF_CUDA_OK(cudaMemsetAsync(o.dL_dcolor, 0, P * 12, st));
+      if (with_color && s->shs) GOF_CUDA_OK(cudaMemsetAsync(o.dL_dsh, 0, P * (size_t)s->M * 12, st));
+      GOF_CUDA_OK(cudaMemsetAsync(o.dL_dopacity, 0, P * 4, st));
+      GOF_CUDA_OK(cudaMemsetAsync(o.dL_dmean3D, 0, P * 12, st));
+      GOF_CUDA_OK(cudaMemsetAsync(o.dL_dview2gaussian, 0, P * 40, st));
+      if (o.dL_dscale) GOF_CUDA_OK(cudaMemsetAsync(o.dL_dscale, 0, P * 12, st));
+      if (o.dL_drot) GOF_CUDA_OK(cudaMemsetAsync(o.dL_drot, 0, P * 16, st));
+      if (o.dL_dcov3D) GOF_CUDA_OK(cudaMemsetAsync(o.dL_dcov3D, 0, P * 24, st));
     }
     return GOF_OK;
   }
@@ -616,8 +616,7 @@ extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float*
                                        reinterpret_cast<const uint32_t*>(static_cast<const char*>(binning_buffer) + BL.point_list),
                                        reinterpret_cast<const uint2*>(static_cast<const char*>(image_buffer) + IL.ranges),
                                        static_cast<const char*>(point_buffer), PL, static_cast<char*>(point_binning_buffer), PBL,
-                                       dL_dalpha, dL_dpoints3D, dL_dopacity, dL_dmean3D, dL_dscale, dL_drot, dL_dview2gaussian,
-                                       dL_dcov3D, dL_dcolor_int, dL_dcolors, with_color ? dL_dsh : nullptr, scratch, st);
+                                       dL_dalpha, dL_dcolor_int, dL_dpoints3D, o, st);
 }
 
 // ---- the Gaussian side of the query, once per view --------------------------------------------------------------

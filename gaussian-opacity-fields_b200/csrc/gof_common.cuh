@@ -347,12 +347,10 @@ static inline GofView gof_make_view(const gof_scene_t* s) {
 // box_margin: see gof_cull_bbox (0 when the records feed the blend kernels, 0.5 when they feed k_integrate)
 int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, const GofGeomLayout& L,
                           int* radii, float box_margin, cudaStream_t st);
-int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const char* geom,
-                                   const GofGeomLayout& L, const int* radii, float* dL_dmean2D, float* dL_dopacity,
-                                   float* dL_dcolor, float* dL_dv2g, float* dL_dmean3D, float* dL_dsh, float* dL_dscale,
-                                   float* dL_drot, float* dL_dcov3D, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
-                                   float* dL_dviewmatrix, float* dL_dcampos, void* cam_scratch, cudaStream_t st);
-// bytes of cam_scratch: the camera-gradient pass (dL_dviewmatrix non-NULL) leaves one partial row per CTA there
+// The accumulator rows in geom -> the outputs in o (checked by the caller)
+int gof_launch_preprocess_backward(const gof_scene_t* s, const char* geom, const GofGeomLayout& L, const int* radii,
+                                   const gof_backward_out_t& o, cudaStream_t st);
+// bytes of o.scratch for the camera-gradient pass (o.dL_dviewmatrix non-NULL): it leaves one partial row per CTA there
 size_t gof_camera_grad_scratch_bytes(int P);
 int gof_launch_mark_visible(int P, const float* means3D, const float* vm, unsigned char* present,
                             cudaStream_t st);
@@ -422,16 +420,14 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
                          float* out_color_int, const GofIntMin* mn, cudaStream_t st);
 // The backward of the query (DESIGN.md 4.11) from the state gof_launch_integrate left in geom / pts / pbin: dL_dalpha [PN] ->
 // dL_dpoints3D [PN][3] (optional) and, through the accumulator rows and k_preprocess_backward, the Gaussian gradients.  The
-// contributor slab in pbin and the accumulator rows in geom are rewritten.  scratch: gof_integrate_backward_scratch(P) bytes.
-// dL_dcolors NULL: the alpha-only backward (no SH chain).  Otherwise (DESIGN.md 4.13) dL_dcolor_int [PN][3] (NULL: no colour
-// loss) also goes through the colour walk, dL_dalpha may be NULL, and dL_dcolors [P][3] / dL_dsh receive the colour's chain.
+// contributor slab in pbin and the accumulator rows in geom are rewritten.  o.scratch: gof_integrate_backward_scratch(P) bytes.
+// o.dL_dcolor NULL: the alpha-only backward (no SH chain).  Otherwise (DESIGN.md 4.13) dL_dcolor_int [PN][3] (NULL: no colour
+// loss) also goes through the colour walk, dL_dalpha may be NULL, and o.dL_dcolor [P][3] / o.dL_dsh receive the colour's chain.
 size_t gof_integrate_backward_scratch(int P);
 int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const int* radii,
                                   char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
                                   const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
-                                  float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot,
-                                  float* dL_dv2g, float* dL_dcov3D, const float* dL_dcolor_int, float* dL_dcolors, float* dL_dsh,
-                                  void* scratch, cudaStream_t st);
+                                  const float* dL_dcolor_int, float* dL_dpoints3D, const gof_backward_out_t& o, cudaStream_t st);
 
 // Per-view cache of the Gaussian side of the opacity-field query (gof_integrate_prepare / gof_integrate_cached): the records,
 // the tile ranges and the per-tile Gaussian lists are all a query needs, and they do not depend on the query points.

@@ -767,9 +767,7 @@ size_t gof_integrate_backward_scratch(int P) { return P > 0 ? 2 * gof_align_up((
 int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const int* radii,
                                   char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
                                   const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
-                                  float* dL_dpoints3D, float* dL_dopacity, float* dL_dmean3D, float* dL_dscale, float* dL_drot,
-                                  float* dL_dv2g, float* dL_dcov3D, const float* dL_dcolor_int, float* dL_dcolors, float* dL_dsh,
-                                  void* scratch, cudaStream_t st) {
+                                  const float* dL_dcolor_int, float* dL_dpoints3D, const gof_backward_out_t& o, cudaStream_t st) {
   const bool debug = s->debug != 0;
   IntBwdColorArgs a{};
   a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.tiles = v.tiles; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
@@ -792,13 +790,12 @@ int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN
   else
     GOF_LAUNCH("integrate_bwd", st, k_integrate_backward<false><<<grid, GOF_BLOCK_SIZE, 0, st>>>(static_cast<const IntBwdArgs&>(a)));
   GOF_LAUNCH_CHECK(debug, st);
-  // the accumulator rows -> the Gaussian parameters, exactly as after the blend backward.  Without dL_dcolors (the alpha-only
-  // entry) the scene goes in without SHs, and dL_dcolor / dL_dmean2D (zero rows) land in the scratch; with it, rows 10..12 go
-  // through the SH (or colors_precomp) backward as after the blend.
+  // the accumulator rows -> the Gaussian parameters, exactly as after the blend backward.  dL_dmean2D (zero rows) lands in the
+  // scratch.  Without o.dL_dcolor (alpha mode) the scene goes in without SHs, and dL_dcolor lands in the scratch too; with it,
+  // rows 10..12 go through the SH (or colors_precomp) backward as after the blend.
   gof_scene_t sg = *s;
-  if (!dL_dcolors) sg.shs = nullptr;
-  float* dcolor = dL_dcolors ? dL_dcolors : static_cast<float*>(scratch);
-  float* dmean2D = reinterpret_cast<float*>(static_cast<char*>(scratch) + gof_align_up((size_t)s->P * 12, 256));
-  return gof_launch_preprocess_backward(&sg, v, geom, GL, radii, dmean2D, dL_dopacity, dcolor, dL_dv2g, dL_dmean3D, dL_dcolors ? dL_dsh : nullptr,
-                                        dL_dscale, dL_drot, dL_dcov3D, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, st);
+  gof_backward_out_t po = o;
+  po.dL_dmean2D = reinterpret_cast<float*>(static_cast<char*>(o.scratch) + gof_align_up((size_t)s->P * 12, 256));
+  if (!o.dL_dcolor) { sg.shs = nullptr; po.dL_dcolor = static_cast<float*>(o.scratch); po.dL_dsh = nullptr; }
+  return gof_launch_preprocess_backward(&sg, geom, GL, radii, po, st);
 }

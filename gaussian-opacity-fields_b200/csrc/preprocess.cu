@@ -721,12 +721,8 @@ int gof_launch_preprocess(const gof_scene_t* s, const GofView& v, char* geom, co
   return GOF_OK;
 }
 
-int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const char* geom,
-                                   const GofGeomLayout& L, const int* radii, float* dL_dmean2D, float* dL_dopacity,
-                                   float* dL_dcolor, float* dL_dv2g, float* dL_dmean3D, float* dL_dsh, float* dL_dscale,
-                                   float* dL_drot, float* dL_dcov3D, float* dens_sum, float* dens_max, float* sh_rgb, float* sh_hdr,
-                                   float* dL_dviewmatrix, float* dL_dcampos, void* cam_scratch, cudaStream_t st) {
-  (void)v;
+int gof_launch_preprocess_backward(const gof_scene_t* s, const char* geom, const GofGeomLayout& L, const int* radii,
+                                   const gof_backward_out_t& o, cudaStream_t st) {
   PreBwdArgs a{};
   a.P = s->P; a.D = s->D; a.M = s->M;
   a.means3D = s->means3D; a.radii = radii; a.shs = s->shs;
@@ -734,22 +730,23 @@ int gof_launch_preprocess_backward(const gof_scene_t* s, const GofView& v, const
   a.scales = s->scales; a.rotations = s->rotations; a.viewmatrix = s->viewmatrix; a.cam_pos = s->cam_pos;
   a.grad_acc = reinterpret_cast<const double2*>(geom + L.grad_acc);
   a.splat = reinterpret_cast<const GofSplat*>(geom + L.splat);
-  a.dL_dmean2D = dL_dmean2D; a.dL_dopacity = dL_dopacity;
-  a.dL_dcolor = dL_dcolor; a.dL_dv2g = dL_dv2g; a.dL_dmean3D = dL_dmean3D; a.dL_dsh = dL_dsh;
-  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot; a.dL_dcov3D = dL_dcov3D;
-  a.dens_sum = (dens_sum && dens_max) ? dens_sum : nullptr; a.dens_max = a.dens_sum ? dens_max : nullptr;
-  a.sh_rgb = s->shs ? sh_rgb : nullptr; a.sh_hdr = a.sh_rgb ? sh_hdr : nullptr; a.sh_plane = GOF_SH_PLANE(s->P);
+  a.dL_dmean2D = o.dL_dmean2D; a.dL_dopacity = o.dL_dopacity;
+  a.dL_dcolor = o.dL_dcolor; a.dL_dv2g = o.dL_dview2gaussian; a.dL_dmean3D = o.dL_dmean3D; a.dL_dsh = o.dL_dsh;
+  a.dL_dscale = o.dL_dscale; a.dL_drot = o.dL_drot; a.dL_dcov3D = o.dL_dcov3D;
+  a.dens_sum = (o.dens_sum && o.dens_max) ? o.dens_sum : nullptr; a.dens_max = a.dens_sum ? o.dens_max : nullptr;
+  a.sh_rgb = s->shs ? o.sh_rgb : nullptr; a.sh_hdr = a.sh_rgb ? o.sh_hdr : nullptr; a.sh_plane = GOF_SH_PLANE(s->P);
   const int blocks = (s->P + K8_THREADS - 1) / K8_THREADS;
-  if (dL_dviewmatrix == nullptr) {
+  if (o.dL_dviewmatrix == nullptr) {
     GOF_LAUNCH("preprocess_bwd", st, k_preprocess_backward<false><<<blocks, K8_THREADS, 0, st>>>(a));
     GOF_LAUNCH_CHECK(s->debug, st);
     return GOF_OK;
   }
-  a.cam_partial = static_cast<double*>(cam_scratch);
+  a.cam_partial = static_cast<double*>(o.scratch);
   a.cam_vm = s->view2gaussian_precomp == nullptr;
   GOF_LAUNCH("preprocess_bwd_camera", st, k_preprocess_backward<true><<<blocks, K8_THREADS, 0, st>>>(a));
   GOF_LAUNCH_CHECK(s->debug, st);
-  GOF_LAUNCH("camera_grad_sum", st, k_camera_grad_sum<<<1, CAM_SUM_THREADS, 0, st>>>(blocks, a.cam_partial, dL_dviewmatrix, dL_dcampos));
+  GOF_LAUNCH("camera_grad_sum", st, k_camera_grad_sum<<<1, CAM_SUM_THREADS, 0, st>>>(blocks, a.cam_partial, o.dL_dviewmatrix,
+                                                                                       o.dL_dcampos));
   GOF_LAUNCH_CHECK(s->debug, st);
   return GOF_OK;
 }

@@ -41,7 +41,7 @@ class _Scene(ctypes.Structure):
 
 
 class _BackwardOut(ctypes.Structure):
-    """gof_backward_out_t: the outputs of gof_rasterize_backward_ex."""
+    """gof_backward_out_t: the outputs of gof_rasterize_backward_ex and of gof_integrate_backward."""
     _fields_ = [(n, _fp) for n in (
         "dL_dmean2D", "dL_dopacity", "dL_dcolor", "dL_dmean3D", "dL_dcov3D", "dL_dsh", "dL_dscale", "dL_drot", "dL_dview2gaussian",
         "dens_sum", "dens_max", "sh_rgb", "sh_hdr", "dL_dviewmatrix", "dL_dcampos", "dL_dtan_fov", "scratch")] + \
@@ -490,8 +490,8 @@ def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opa
 _lib.gof_integrate_backward_scratch_bytes.restype = ctypes.c_size_t
 _lib.gof_integrate_backward_scratch_bytes.argtypes = [ctypes.c_int]
 _lib.gof_integrate_backward.restype = ctypes.c_int
-_lib.gof_integrate_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 18 + \
-    [ctypes.c_size_t, ctypes.c_void_p]
+_lib.gof_integrate_backward.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_fp] * 9 + \
+    [ctypes.POINTER(_BackwardOut), ctypes.c_void_p]
 
 
 def integrate_gaussians_to_points_backward(background, points3D, means3D, radii, colors, scales, rotations, scale_modifier,
@@ -501,9 +501,9 @@ def integrate_gaussians_to_points_backward(background, points3D, means3D, radii,
                                            pointBinningBuffer, debug, points_grad=True, dL_dcolor=None):
     """gof_integrate_backward (extension, DESIGN.md 4.11): the gradient dL_dalpha [PN] of out_alpha_integrated ->
     (dL_dpoints3D [PN,3] or None, dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drotations [P,4],
-    dL_dcov3D [P,6], dL_dview2gaussian [P,10]).  The state is what integrate_gaussians_to_points_state returned.
-    With dL_dcolor [PN,3], the gradient of out_color_integrated (colour mode, DESIGN.md 4.13), dL_dalpha may be
-    None, and two more outputs follow: dL_dcolors [P,3] and dL_dsh [P,M,3] (None without SHs)."""
+    dL_dcov3D [P,6], dL_dview2gaussian [P,10], dL_dcolors, dL_dsh).  The state is what integrate_gaussians_to_points_state
+    returned.  With dL_dcolor [PN,3], the gradient of out_color_integrated (colour mode, DESIGN.md 4.13), dL_dalpha may be
+    None, and dL_dcolors [P,3] and dL_dsh [P,M,3] (None without SHs) are computed; without it both are None."""
     P, PN = means3D.size(0), points3D.size(0)
     keep = []
     s = _scene(keep, background, means3D, colors, means3D, scales, rotations, scale_modifier, cov3D_precomp,
@@ -536,18 +536,18 @@ def integrate_gaussians_to_points_backward(background, points3D, means3D, radii,
         dcolors = torch.empty((P, 3), dtype=torch.float32, device=dev)
         dsh = torch.empty((P, s.M, 3), dtype=torch.float32, device=dev) if s.M > 0 else None
     buf = lambda t: t.data_ptr() if t is not None and t.numel() else None   # noqa: E731
+    o = _BackwardOut(dL_dopacity=buf(out["dopacity"]), dL_dmean3D=buf(out["dmeans3D"]), dL_dscale=buf(out["dscales"]) if has_sr else None,
+                     dL_drot=buf(out["drot"]) if has_sr else None, dL_dview2gaussian=buf(out["dv2g"]), dL_dcov3D=buf(out["dcov3D"]),
+                     dL_dcolor=buf(dcolors), dL_dsh=buf(dsh), scratch=scratch.data_ptr() if nbytes else None, scratch_bytes=nbytes)
     with torch.cuda.device(dev):
         _check(_lib.gof_integrate_backward(
             ctypes.byref(s), PN, _ptr(p3, device=dev), int(num_rendered), _ptr(radii.contiguous(), torch.int32), buf(geomBuffer),
             buf(binningBuffer), buf(imgBuffer), buf(pointBuffer), buf(pointBinningBuffer), _ptr(g, device=dev), _ptr(gc, device=dev),
-            buf(dpts), buf(out["dopacity"]), buf(out["dmeans3D"]), buf(out["dscales"]) if has_sr else None,
-            buf(out["drot"]) if has_sr else None, buf(out["dv2g"]), buf(out["dcov3D"]), buf(dcolors), buf(dsh),
-            scratch.data_ptr() if nbytes else None, nbytes, _stream()))
+            buf(dpts), ctypes.byref(o), _stream()))
     if P and not has_sr:
         out["dscales"].zero_()
         out["drot"].zero_()
-    res = (dpts, out["dopacity"], out["dmeans3D"], out["dscales"], out["drot"], out["dcov3D"], out["dv2g"])
-    return res + (dcolors, dsh) if color else res
+    return dpts, out["dopacity"], out["dmeans3D"], out["dscales"], out["drot"], out["dcov3D"], out["dv2g"], dcolors, dsh
 
 
 _lib.gof_integrate_cache_bytes.restype = ctypes.c_size_t

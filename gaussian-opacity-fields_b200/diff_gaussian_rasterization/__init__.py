@@ -198,15 +198,9 @@ class _IntegrateGaussians(torch.autograd.Function):
             grad_alpha = torch.zeros(points3D.size(0), dtype=torch.float32, device=points3D.device)
         args = _integrate_backward_args(rs, points3D, means3D, radii, colors_precomp, scales, rotations, cov3D_precomp,
                                         view2gaussian_precomp, shs, grad_alpha, ctx.num_rendered, geom, binning, img, pts, pbin)
-        g_colors = g_sh = None
-        if grad_color_integrated is None:
-            g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g = _call_native(
-                _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
-                points_grad=ctx.needs_input_grad[0])
-        else:
-            g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g, g_colors, g_sh = _call_native(
-                _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
-                points_grad=ctx.needs_input_grad[0], dL_dcolor=grad_color_integrated)
+        g_pts, g_opacity, g_means3D, g_scales, g_rot, g_cov3D, g_v2g, g_colors, g_sh = _call_native(
+            _C.integrate_gaussians_to_points_backward, args, rs.debug, "snapshot_bw.dump", "backward",
+            points_grad=ctx.needs_input_grad[0], dL_dcolor=grad_color_integrated)
         need = ctx.needs_input_grad
         pick = lambda g, i: g if need[i] else None   # noqa: E731
         return (pick(g_pts, 0), pick(g_means3D, 1), None, pick(g_opacity, 3), pick(g_sh, 4), pick(g_colors, 5), pick(g_scales, 6),
@@ -289,10 +283,8 @@ class GaussianRasterizer(nn.Module):
         rs = self.raster_settings
         shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp = _normalise_optionals(
             shs, colors_precomp, scales, rotations, cov3D_precomp, view2gaussian_precomp)
-        args = (rs.bg, points3D, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
-                cov3D_precomp, view2gaussian_precomp) + _camera_args(rs) + (rs.image_height, rs.image_width, shs,
-                                                                            rs.sh_degree, rs.campos, rs.prefiltered,
-                                                                            rs.debug)
+        args = _integrate_args(rs, points3D, means3D, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+                               view2gaussian_precomp, shs)
         (_num_rendered, color, alpha_integrated, color_integrated, radii, _g, _b, _i) = _call_native(
             _C.integrate_gaussians_to_points, args, rs.debug, "snapshot_fw.dump", "forward")
         return color, alpha_integrated, color_integrated, radii

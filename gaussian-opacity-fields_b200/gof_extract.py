@@ -203,17 +203,12 @@ class _OpacityField(torch.autograd.Function):
                 bargs = dgr._integrate_backward_args(rs, p, means3D, radii, colors, scales_, rotations_, cov3D, v2g, shs_, dA[sel], R,
                                                      geom, binning, img, pts, pbin)
                 del geom, binning, img, pts, pbin
-                if with_color:
-                    dp, dop, dm, dsc, drot, _dcov, _dv2g, _dcol, dsh = dgr._call_native(
-                        _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward",
-                        points_grad=need[0], dL_dcolor=dC[sel])
-                    if n_sh:
-                        g_sh += dsh.view(-1)
-                else:
-                    dp, dop, dm, dsc, drot, _dcov, _dv2g = dgr._call_native(
-                        _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward",
-                        points_grad=need[0])
+                dp, dop, dm, dsc, drot, _dcov, _dv2g, _dcol, dsh = dgr._call_native(
+                    _C.integrate_gaussians_to_points_backward, bargs, rs.debug, "snapshot_bw.dump", "backward",
+                    points_grad=need[0], dL_dcolor=dC[sel] if with_color else None)
                 del bargs   # the state goes back to the scratch pool before the next view
+                if n_sh:
+                    g_sh += dsh.view(-1)
                 if dp is not None:
                     g_pts[sel] = dp
                 if gaussians:

@@ -50,6 +50,19 @@ def _call(s, out, radii=FAKE):
     return rc, _C._lib.gof_last_error()
 
 
+def _positional(s, radii=FAKE, **kw):
+    """The positional gof_rasterize_backward with the arguments of _call and _out's gradients, updated by `kw`."""
+    lib = _C._lib
+    lib.gof_rasterize_backward.restype = ctypes.c_int
+    lib.gof_rasterize_backward.argtypes = [ctypes.POINTER(_C._Scene), ctypes.c_int] + [ctypes.c_void_p] * 16
+    g = {n: getattr(_out(**kw), n) for n in ("dL_dmean2D", "dL_dopacity", "dL_dcolor", "dL_dmean3D", "dL_dsh", "dL_dscale", "dL_drot",
+                                             "dL_dview2gaussian")}
+    rc = lib.gof_rasterize_backward(ctypes.byref(s), 0, radii, FAKE, None, FAKE, FAKE, g["dL_dmean2D"], None, g["dL_dopacity"],
+                                    g["dL_dcolor"], g["dL_dmean3D"], None, g["dL_dsh"], g["dL_dscale"], g["dL_drot"],
+                                    g["dL_dview2gaussian"], None)
+    return rc, lib.gof_last_error()
+
+
 def test_backward_entry_points_are_exported():
     for name in ("gof_rasterize_backward", "gof_rasterize_backward_ex", "gof_rasterize_backward_scratch_bytes"):
         assert hasattr(_C._lib, name), name
@@ -85,19 +98,23 @@ def test_null_out_is_refused():
 def test_missing_gradients_are_refused_with_or_without_camera_and_focal_length():
     """radii, dL_dmean2D or dL_dcolor missing: the plain call, the camera request, the focal-length request and the positional
     gof_rasterize_backward all fail with the same error."""
-    lib = _C._lib
-    lib.gof_rasterize_backward.restype = ctypes.c_int
-    lib.gof_rasterize_backward.argtypes = [ctypes.POINTER(_C._Scene), ctypes.c_int] + [ctypes.c_void_p] * 16
     s = _fake_scene(300)
     for missing in ("radii", "dL_dmean2D", "dL_dcolor"):
         field = {} if missing == "radii" else {missing: None}
         radii = None if missing == "radii" else FAKE
         for out in (_out(**field), _camera(**field), _intrinsics(**field)):
             assert _call(s, out, radii=radii) == (-1, b"backward: NULL argument"), missing
-        g = {**dict(radii=radii, dL_dmean2D=FAKE, dL_dcolor=FAKE), **field}
-        rc = lib.gof_rasterize_backward(ctypes.byref(s), 0, g["radii"], FAKE, None, FAKE, FAKE, g["dL_dmean2D"], None, FAKE,
-                                        g["dL_dcolor"], FAKE, None, FAKE, FAKE, FAKE, FAKE, None)
-        assert (rc, lib.gof_last_error()) == (-1, b"backward: NULL argument"), missing
+        assert _positional(s, radii=radii, **field) == (-1, b"backward: NULL argument"), missing
+
+
+def test_misaligned_rotation_and_sh_gradients_are_refused():
+    """dL_drot, and dL_dsh with M = 16 and degree 3, are written with 16-byte stores: a pointer that is not 16-byte aligned fails
+    with GOF_E_INVALID before any work, through gof_rasterize_backward_ex and the positional gof_rasterize_backward."""
+    s = _fake_scene(300)
+    assert (s.M, s.D) == (16, 3)
+    for field in ("dL_drot", "dL_dsh"):
+        for rc, err in (_call(s, _out(**{field: 0x1004})), _positional(s, **{field: 0x1004})):
+            assert rc == -1 and f"{field} must be 16-byte aligned".encode() in err, field
 
 
 def _check_request(request_):

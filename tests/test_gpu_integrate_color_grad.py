@@ -45,10 +45,9 @@ def _backward(ia, state, dL_dalpha, dL_dcolor, points_grad=True):
     from diff_gaussian_rasterization import _C
     (bg, p3, m3, col, op, sc, rot, sm, cov, v2g, vm, pm, tfx, tfy, ks, sub, H, W, sh, deg, cp, _pf, dbg) = ia
     R, _color, _a, _c, radii, geom, binning, img, pts, pbin = state
-    kw = {} if dL_dcolor is None else dict(dL_dcolor=dL_dcolor)
     return _C.integrate_gaussians_to_points_backward(bg, p3, m3, radii, col, sc, rot, sm, cov, v2g, vm, pm, tfx, tfy, ks, sub, H, W,
                                                      sh, deg, cp, dL_dalpha, R, geom, binning, img, pts, pbin, dbg,
-                                                     points_grad=points_grad, **kw)
+                                                     points_grad=points_grad, dL_dcolor=dL_dcolor)
 
 
 def run(cam, gs, pts, seed=0, kernel_size=0.0):

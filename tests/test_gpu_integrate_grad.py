@@ -63,7 +63,8 @@ def run(cam, gs, pts, seed=0, kernel_size=0.0):
     dL = torch.randn(PN, generator=torch.Generator().manual_seed(seed))
     g = _backward(ia, state, dL.to(dev))
     torch.cuda.synchronize()
-    got = dict(zip(("dpts", "dopacity", "dmeans3D", "dscales", "drot", "dcov3D", "dv2g"), (t.cpu().numpy() for t in g)))
+    assert g[7:] == (None, None)   # alpha mode: no dL_dcolors, no dL_dsh
+    got = dict(zip(("dpts", "dopacity", "dmeans3D", "dscales", "drot", "dcov3D", "dv2g"), (t.cpu().numpy() for t in g[:7])))
     R, _color, alpha, _ci, radii, geom, binning, img, _pts, _pbin = state
     sc = gof_oracle.Scene(W, H, cam.tanfovx, cam.tanfovy, cam.world_view_transform, cam.full_proj_transform, cam.camera_center,
                           gs["means3D"], gs["opacities"], scales=gs["scales"], rotations=gs["rotations"], shs=gs["shs"],

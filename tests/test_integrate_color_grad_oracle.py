@@ -148,12 +148,14 @@ def _bwd(_C, s, PN=4, scratch=FAKE, nbytes=10 ** 6, **kw):
     a = dict(points=FAKE, radii=FAKE, geom=FAKE, binning=FAKE, image=FAKE, pts=FAKE, pbin=FAKE, dalpha=FAKE, dcolor=FAKE,
              dpts=FAKE, dop=FAKE, dmean=FAKE, dscale=FAKE, drot=FAKE, dv2g=FAKE, dcov=FAKE, dcolors=FAKE, dsh=FAKE)
     a.update(kw)
+    o = _C._BackwardOut(dL_dopacity=a["dop"], dL_dmean3D=a["dmean"], dL_dscale=a["dscale"], dL_drot=a["drot"],
+                        dL_dview2gaussian=a["dv2g"], dL_dcov3D=a["dcov"], dL_dcolor=a["dcolors"], dL_dsh=a["dsh"], scratch=scratch,
+                        scratch_bytes=nbytes)
     return _C._lib.gof_integrate_backward(ctypes.byref(s), PN, a["points"], 1, a["radii"], a["geom"], a["binning"], a["image"],
-                                          a["pts"], a["pbin"], a["dalpha"], a["dcolor"], a["dpts"], a["dop"], a["dmean"], a["dscale"],
-                                          a["drot"], a["dv2g"], a["dcov"], a["dcolors"], a["dsh"], scratch, nbytes, None)
+                                          a["pts"], a["pbin"], a["dalpha"], a["dcolor"], a["dpts"], ctypes.byref(o), None)
 
 
-def test_backward_color_refusals():
+def test_backward_color_refusals_with_out():
     _C = _abi()
     err = _C._lib.gof_last_error
     s = _scene(_C)
@@ -165,13 +167,16 @@ def test_backward_color_refusals():
         assert _bwd(_C, s, **{k: None}) == -1 and b"dL_dscale / dL_drot" in err(), k
     assert _bwd(_C, s, drot=FAKE + 4) == -1 and b"aligned" in err()
     assert _bwd(_C, _scene(_C, shs=True), dsh=None) == -1 and b"dL_dsh" in err()
+    # M = 16 and degree 3: dL_dsh is written with 16-byte stores
+    assert _bwd(_C, _scene(_C, shs=True), dsh=FAKE + 4) == -1 and b"dL_dsh must be 16-byte aligned" in err()
     assert _bwd(_C, s, PN=-1) == -1 and b"PN" in err()
     for k in ("points", "radii", "geom", "image", "pts", "pbin"):
         assert _bwd(_C, s, **{k: None}) == -1 and b"forward state" in err(), k
     bad = _scene(_C)
     bad.P = -1
     assert _bwd(_C, bad) == -1
-    assert _C._lib.gof_integrate_backward(None, 4, *[FAKE] * 2, 1, *[FAKE] * 18, FAKE, 10 ** 6, None) == -1
+    o = _C._BackwardOut(dL_dopacity=FAKE, dL_dmean3D=FAKE, dL_dview2gaussian=FAKE, dL_dcolor=FAKE, scratch=FAKE, scratch_bytes=10 ** 6)
+    assert _C._lib.gof_integrate_backward(None, 4, FAKE, 1, *[FAKE] * 9, ctypes.byref(o), None) == -1
 
 
 def test_min_color_refusals():

@@ -151,33 +151,52 @@ def test_scratch_bytes():
     assert f(1000) == 2 * ((12000 + 255) // 256 * 256)
 
 
-def test_argument_checks():
-    _C = _abi()
+FAKE = 0x1000
+
+
+def _alpha_call(_C, s, **out):
+    """gof_integrate_backward in alpha mode (dL_dalpha, no dL_dcolor_integrated) with the forward state at FAKE and the Gaussian
+    gradients and a large scratch at FAKE, updated by `out` (field name -> pointer or None)."""
+    o = dict(dL_dopacity=FAKE, dL_dmean3D=FAKE, dL_dscale=FAKE, dL_drot=FAKE, dL_dview2gaussian=FAKE, dL_dcov3D=FAKE,
+             scratch=FAKE, scratch_bytes=10 ** 6)
+    o.update(out)
+    o = _C._BackwardOut(**o)
+    return _C._lib.gof_integrate_backward(ctypes.byref(s), 4, FAKE, 1, *[FAKE] * 6, FAKE, None, FAKE, ctypes.byref(o), None)
+
+
+def _alpha_scene(_C):
     s = _C._Scene()
     s.P, s.width, s.height, s.tan_fovx, s.tan_fovy = 10, 32, 32, 0.5, 0.5
-    fake = ctypes.c_void_p(0x1000)
     for name in ("means3D", "opacities", "viewmatrix", "projmatrix", "background", "colors_precomp", "scales", "rotations"):
-        setattr(s, name, fake.value)
-    # forward state; dL_dalpha, no dL_dcolor_integrated; the seven outputs; no dL_dcolors / dL_dsh (alpha mode)
-    args = [ctypes.byref(s), 4, fake.value, 1] + [fake.value] * 6 + [fake.value, None] + [fake.value] * 7 + [None, None]
+        setattr(s, name, FAKE)
+    return s
+
+
+def test_scratch_in_out_and_scene_are_checked():
+    _C = _abi()
+    s = _alpha_scene(_C)
     # a NULL or short scratch is refused before any work
-    rc_null = _C._lib.gof_integrate_backward(*args, None, 10 ** 6, None)
-    rc_short = _C._lib.gof_integrate_backward(*args, fake.value, 16, None)
+    rc_null = _alpha_call(_C, s, scratch=None)
+    rc_short = _alpha_call(_C, s, scratch_bytes=16)
     assert rc_null == rc_short == -1   # GOF_E_INVALID
     assert b"scratch" in _C._lib.gof_last_error()
     s.P = -1
-    assert _C._lib.gof_integrate_backward(*args, fake.value, 10 ** 6, None) != 0
+    assert _alpha_call(_C, s) != 0
 
 
-def test_misaligned_rotation_gradient_is_refused():
+def test_misaligned_rotation_gradient_in_out_is_refused():
     """dL_drot is written with 16-byte stores: a pointer that is not 16-byte aligned fails with GOF_E_INVALID before any work."""
     _C = _abi()
-    s = _C._Scene()
-    s.P, s.width, s.height, s.tan_fovx, s.tan_fovy = 10, 32, 32, 0.5, 0.5
-    fake = 0x1000
-    for name in ("means3D", "opacities", "viewmatrix", "projmatrix", "background", "colors_precomp", "scales", "rotations"):
-        setattr(s, name, fake)
-    drot = fake + 4
-    args = [ctypes.byref(s), 4, fake, 1] + [fake] * 6 + [fake, None] + [fake] * 4 + [drot, fake, fake] + [None, None]
-    assert _C._lib.gof_integrate_backward(*args, fake, 10 ** 6, None) == -1
+    assert _alpha_call(_C, _alpha_scene(_C), dL_drot=FAKE + 4) == -1
     assert b"aligned" in _C._lib.gof_last_error()
+
+
+def test_out_is_checked():
+    """A NULL out, and any output this backward cannot produce, fail with GOF_E_INVALID and the field's name."""
+    _C = _abi()
+    s = _alpha_scene(_C)
+    assert _C._lib.gof_integrate_backward(ctypes.byref(s), 4, FAKE, 1, *[FAKE] * 6, FAKE, None, FAKE, None, None) == -1
+    assert b"out is NULL" in _C._lib.gof_last_error()
+    for name in ("dL_dmean2D", "dens_sum", "dens_max", "sh_rgb", "sh_hdr", "dL_dviewmatrix", "dL_dcampos", "dL_dtan_fov"):
+        assert _alpha_call(_C, s, **{name: FAKE}) == -1, name
+        assert f"out->{name} must be NULL".encode() in _C._lib.gof_last_error(), name

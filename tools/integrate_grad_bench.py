@@ -63,9 +63,8 @@ def main():
         R, _c, _a, _ci, radii, geom, binning, img, pt, pbin = state
         (bg, p3, m3, col, op, sc, rot, sm, cov, v2g, vm, pm, tfx, tfy, ks, sub, H_, W_, sh, deg, cp, _pf, dbg) = ia
         da, dc = losses[mode]
-        kw = {} if dc is None else dict(dL_dcolor=dc)
         return _C.integrate_gaussians_to_points_backward(bg, p3, m3, radii, col, sc, rot, sm, cov, v2g, vm, pm, tfx, tfy, ks, sub, H_,
-                                                         W_, sh, deg, cp, da, R, geom, binning, img, pt, pbin, dbg, **kw)
+                                                         W_, sh, deg, cp, da, R, geom, binning, img, pt, pbin, dbg, dL_dcolor=dc)
 
     def timed(fn):
         s, t = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
