@@ -4,6 +4,7 @@
 #include <stdlib.h>
 
 #include "gof_common.cuh"
+#include "gof_math.cuh"
 
 // ---- launch counter + optional per-kernel event timing ----------------------------------------------------
 #include <map>
@@ -271,16 +272,14 @@ static int gaussian_side(const gof_scene_t* s, const GofView& v, gof_alloc_fn ge
 // The point side of the query, against the Gaussian side of gaussian_side or of a gof_integrate_prepare cache (img: the
 // image scratch, NULL if its allocator failed).
 static int point_side(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
-                      const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, gof_alloc_fn point_alloc,
-                      void* point_user, gof_alloc_fn point_binning_alloc, void* point_binning_user, float* out_color,
-                      float* out_alpha_integrated, float* out_color_integrated, const GofIntMin* mn, cudaStream_t st) {
-  const GofPointLayout PL = gof_point_layout((size_t)PN);
-  const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count());
-  char* pts = (char*)point_alloc(point_user, PL.bytes);
-  char* pbin = (char*)point_binning_alloc(point_binning_user, PBL.bytes);
+                      const uint32_t* point_list, const uint2* ranges, char* img, gof_alloc_fn point_alloc, void* point_user,
+                      gof_alloc_fn point_binning_alloc, void* point_binning_user, float* out_color, float* out_alpha_integrated,
+                      float* out_color_integrated, const GofIntMin* mn, cudaStream_t st) {
+  char* pts = (char*)point_alloc(point_user, gof_point_layout((size_t)PN).bytes);
+  char* pbin = (char*)point_binning_alloc(point_binning_user, gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count()).bytes);
   if (!img || !pts || !pbin) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
-  return gof_launch_integrate(s, v, PN, points3D, splat, point_list, ranges, img, IL, pts, PL, pbin, PBL, out_color,
-                              out_alpha_integrated, out_color_integrated, mn, st);
+  return gof_launch_integrate(s, v, PN, points3D, splat, point_list, ranges, img, pts, pbin, out_color, out_alpha_integrated,
+                              out_color_integrated, mn, st);
 }
 
 extern "C" int gof_rasterize_forward(const gof_scene_t* s, gof_alloc_fn geom_alloc, void* geom_user,
@@ -444,9 +443,7 @@ __global__ void k_export_image(int W, int H, int grid_x, size_t plane, const flo
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= W || y >= H) return;
   const int tile = (y / 16) * grid_x + (x / 16);
-  const int lx = x & 15, ly = y & 15;
-  const int warp = (ly / 4) * 2 + (lx / 8), lane = (ly & 3) * 8 + (lx & 7);
-  const size_t slot = (size_t)tile * 256 + warp * 32 + lane;
+  const size_t slot = (size_t)tile * 256 + gof_pixel_slot(x & 15, y & 15);
   const size_t HW = (size_t)W * H, pid = (size_t)y * W + x;
   if (o.accum_alpha) for (int k = 0; k < 4; ++k) o.accum_alpha[k * HW + pid] = accum[k * plane + slot];
   if (o.n_contrib) for (int k = 0; k < 2; ++k) o.n_contrib[k * HW + pid] = nc[k * plane + slot];
@@ -513,7 +510,7 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
     return rc;
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
-                    g.IL, point_alloc, point_user, point_binning_alloc, point_binning_user, out_color, out_alpha_integrated,
+                    point_alloc, point_user, point_binning_alloc, point_binning_user, out_color, out_alpha_integrated,
                     out_color_integrated, nullptr, st);
 }
 
@@ -549,7 +546,7 @@ extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* poin
   const GofIntMin mn{alpha_min, argmin, view, color_min};
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
-                    g.IL, point_alloc, point_user, point_binning_alloc, point_binning_user, nullptr, nullptr, nullptr, &mn, st);
+                    point_alloc, point_user, point_binning_alloc, point_binning_user, nullptr, nullptr, nullptr, &mn, st);
 }
 
 extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
@@ -609,14 +606,12 @@ extern "C" int gof_integrate_backward(const gof_scene_t* s, int PN, const float*
   const GofGeomLayout GL = gof_geom_layout(P);
   const GofImageLayout IL = gof_image_layout(s->width, s->height);
   const GofBinLayout BL = gof_bin_layout((size_t)num_rendered, s->width, s->height, false);
-  const GofPointLayout PL = gof_point_layout((size_t)PN);
-  const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count());
   char* geom = static_cast<char*>(geom_buffer);
   return gof_launch_integrate_backward(s, v, PN, points3D, radii, geom, GL,
                                        reinterpret_cast<const uint32_t*>(static_cast<const char*>(binning_buffer) + BL.point_list),
                                        reinterpret_cast<const uint2*>(static_cast<const char*>(image_buffer) + IL.ranges),
-                                       static_cast<const char*>(point_buffer), PL, static_cast<char*>(point_binning_buffer), PBL,
-                                       dL_dalpha, dL_dcolor_int, dL_dpoints3D, o, st);
+                                       static_cast<const char*>(point_buffer), static_cast<char*>(point_binning_buffer), dL_dalpha,
+                                       dL_dcolor_int, dL_dpoints3D, o, st);
 }
 
 // ---- the Gaussian side of the query, once per view --------------------------------------------------------------
@@ -677,6 +672,6 @@ extern "C" int gof_integrate_cached(const gof_scene_t* s, int PN, const float* p
   char* img = (char*)image_alloc(image_user, IL.bytes);
   const char* c = (const char*)cache;
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(c + CL.splat), reinterpret_cast<const uint32_t*>(c + CL.point_list),
-                    reinterpret_cast<const uint2*>(c + CL.ranges), img, IL, point_alloc, point_user, point_binning_alloc,
+                    reinterpret_cast<const uint2*>(c + CL.ranges), img, point_alloc, point_user, point_binning_alloc,
                     point_binning_user, out_color, out_alpha_integrated, out_color_integrated, nullptr, st);
 }

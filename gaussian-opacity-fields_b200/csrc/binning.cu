@@ -521,13 +521,13 @@ int gof_depth_sort(int P, char* geom, const GofGeomLayout& L, bool debug, cudaSt
 // key_shift; the bits below it order the points of a tile by pixel), then the per-tile ranges of the first ids < num_tiles (ranges must hold num_tiles + 1 uint2; the last slot absorbs the
 // sentinel id given to points outside the image).  Buffers: keys/vals ping-pong (u32), scratch as in gof_sort_scratch_bytes.
 int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist,
-                            uint2* ranges, int num_tiles, bool debug, cudaStream_t st, int* result_in_b) {
+                            uint2* ranges, int num_tiles, bool debug, cudaStream_t st) {
   GOF_CUDA_OK(cudaMemsetAsync(ranges, 0, (size_t)(num_tiles + 1) * sizeof(uint2), st));
-  *result_in_b = 0;
   if (n == 0) return GOF_OK;
-  const int rc = sort_pairs<uint32_t>(ka, kb, va, vb, hist, n, nbits, debug, st, result_in_b);
+  int in_b = 0;
+  const int rc = sort_pairs<uint32_t>(ka, kb, va, vb, hist, n, nbits, debug, st, &in_b);
   if (rc != GOF_OK) return rc;
-  const uint32_t* sorted = *result_in_b ? kb : ka;
+  const uint32_t* sorted = in_b ? kb : ka;
   GOF_LAUNCH("tile_ranges", st, k_tile_ranges<uint32_t><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, sorted, ranges, key_shift));
   GOF_LAUNCH_CHECK(debug, st);
   return GOF_OK;

@@ -382,7 +382,7 @@ int gof_depth_sort(int P, char* geom, const GofGeomLayout& L, bool debug, cudaSt
 int gof_bin_tiles(int P, size_t R, const GofView& v, char* geom, const GofGeomLayout& GL, char* bin,
                   const GofBinLayout& BL, char* img, const GofImageLayout& IL, bool debug, cudaStream_t st);
 int gof_sort_points_by_tile(size_t n, int nbits, int key_shift, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint32_t* hist,
-                            uint2* ranges, int num_tiles, bool debug, cudaStream_t st, int* result_in_b);
+                            uint2* ranges, int num_tiles, bool debug, cudaStream_t st);
 // *result_in_b of a radix sort of n > 0 pairs over nbits key bits (gof_sort_points_by_tile, gof_bin_tiles): 1 when the sorted pairs
 // end in the b buffers
 int gof_radix_result_in_b(int nbits);
@@ -415,9 +415,8 @@ struct GofIntMin {
   float* color_min;   // [PN][3] or NULL: also the winning view's colour (gof_integrate_min's color_min, DESIGN.md 4.13)
 };
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
-                         const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, char* pts,
-                         const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, float* out_color, float* out_alpha,
-                         float* out_color_int, const GofIntMin* mn, cudaStream_t st);
+                         const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin, float* out_color,
+                         float* out_alpha, float* out_color_int, const GofIntMin* mn, cudaStream_t st);
 // The backward of the query (DESIGN.md 4.11) from the state gof_launch_integrate left in geom / pts / pbin: dL_dalpha [PN] ->
 // dL_dpoints3D [PN][3] (optional) and, through the accumulator rows and k_preprocess_backward, the Gaussian gradients.  The
 // contributor slab in pbin and the accumulator rows in geom are rewritten.  o.scratch: gof_integrate_backward_scratch(P) bytes.
@@ -426,8 +425,8 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
 size_t gof_integrate_backward_scratch(int P);
 int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const int* radii,
                                   char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
-                                  const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
-                                  const float* dL_dcolor_int, float* dL_dpoints3D, const gof_backward_out_t& o, cudaStream_t st);
+                                  char* pbin, const float* dL_dalpha, const float* dL_dcolor_int, float* dL_dpoints3D,
+                                  const gof_backward_out_t& o, cudaStream_t st);
 
 // Per-view cache of the Gaussian side of the opacity-field query (gof_integrate_prepare / gof_integrate_cached): the records,
 // the tile ranges and the per-tile Gaussian lists are all a query needs, and they do not depend on the query points.

@@ -57,29 +57,31 @@ __global__ void __launch_bounds__(256) k_preprocess_points(const PtArgs a) {
       int cx = gof_f2i_rz(x * 0.0625f), cy = gof_f2i_rz(y * 0.0625f);
       cx = min(a.grid_x - 1, max(0, cx));
       cy = min(a.grid_y - 1, max(0, cy));
-      // the thread slot of the pixel the point falls in (same mapping as k_integrate's pass 2): sorting on it makes the points
-      // of one pixel -- which replay the SAME contributor list -- neighbours, so a warp's record gathers coincide
-      int lx = gof_f2i_rz(x) - cx * 16, ly = gof_f2i_rz(y) - cy * 16;
-      lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
-      key = ((uint32_t)(cy * a.grid_x + cx) << PT_KEY_SHIFT) | (uint32_t)(((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7));
+      // the thread slot of the pixel the point falls in, as pass 2 finds it: sorting on it makes the points of one pixel --
+      // which replay the SAME contributor list -- neighbours, so a warp's record gathers coincide
+      key = ((uint32_t)(cy * a.grid_x + cx) << PT_KEY_SHIFT) | (uint32_t)gof_point_slot(x, y, cx, cy);
     }
   }
   a.key[idx] = key;
   a.val[idx] = (uint32_t)idx;
 }
 
-struct IntArgs {
+// One view's query state, read by the forward and the backward alike (int_query fills it)
+struct IntQuery {
   int W, H, grid_x, tiles;
   float focal_x, focal_y;
-  const uint2* ranges;
+  const uint2* ranges;          // per tile: its Gaussian list in point_list
   const uint32_t* point_list;
   const GofSplat* splat;
-  const uint2* pranges;
-  const uint32_t* pt_list;
+  const uint2* pranges;         // per tile: its points in pt_list
+  const uint32_t* pt_list;      // point ids sorted by tile and pixel slot
   const float2* pt_xy;
   const float* pt_depth;
+  uint16_t* ids;                // [gridDim][256][1024] contributor slab
+};
+
+struct IntArgs : IntQuery {
   const float* bg;
-  uint16_t* ids;        // [gridDim][256][1024]
   float* final_T;       // tile-major plane 0 of the image state
   uint32_t* ncontrib;   // tile-major planes 0 (last contributor) and 1 (contributors recorded, for export_state)
   float* out_color;     // [9][H][W]
@@ -93,12 +95,6 @@ struct IntArgs {
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
-
-__device__ __forceinline__ bool box_hits(uint32_t lo, uint32_t hi, int wx0, int wy0, int wx1, int wy1) {
-  const int x0 = (int)(short)(lo & 0xffffu), y0 = (int)(short)(lo >> 16);
-  const int x1 = (int)(short)(hi & 0xffffu), y1 = (int)(short)(hi >> 16);
-  return x0 <= wx1 && x1 >= wx0 && y0 <= wy1 && y1 >= wy0;
-}
 
 // forward.cu:919-930: the five rays (k = 0 centre, 1..4 corners) with the reference's per-ray fusion pattern
 template <int K>
@@ -119,11 +115,16 @@ __device__ __forceinline__ void pair_geom_k(const float* v, float rx, float ry, 
   *BB = F_ADD(bh, bh);
 }
 
-// one ray of pass 1 (forward.cu:931-975): true when the Gaussian is blended on this ray; then *alpha / *test_T hold the
-// blend weight and the transmittance after it, and tmax has been raised to t (forward.cu:965-967)
+struct RayHit {
+  float alpha, test_T;   // the blend weight and the transmittance after it
+  float t;               // the stationary point -BB / (2 AA), where the ray meets the Gaussian
+  bool free;             // power <= 0 and op * exp(power) <= GOF_ALPHA_MAX: alpha carries a derivative
+};
+
+// one ray of pass 1 (forward.cu:931-975): true when the Gaussian is blended on this ray; then *h holds the hit, and tmax has
+// been raised to t (forward.cu:965-967)
 template <int K>
-__device__ __forceinline__ bool ray_step(const float* v, float op, float thr, float rx, float ry, float Tk, float& tmax,
-                                         float* alpha, float* test_T) {
+__device__ __forceinline__ bool ray_step(const float* v, float op, float thr, float rx, float ry, float Tk, float& tmax, RayHit* h) {
   float AA, BB;
   pair_geom_k<K>(v, rx, ry, &AA, &BB);
   {
@@ -139,14 +140,15 @@ __device__ __forceinline__ bool ray_step(const float* v, float op, float thr, fl
   if (GOF_T_BEHIND_NEAR(t)) return false;
   const double mv = D_FMA((double)F_DIV(-BB, AA), D_MUL((double)BB, 0.25), (double)v[9]);
   float power = (float)D_MUL(mv, -0.5);
+  const bool unclamped = power <= 0.0f;
   if (power > 0.0f) power = 0.0f;
-  const float al = fminf(F_MUL(op, F_EXP(power)), GOF_ALPHA_MAX);
+  const float raw = F_MUL(op, F_EXP(power));
+  const float al = fminf(raw, GOF_ALPHA_MAX);
   if (al < GOF_ALPHA_MIN) return false;
   const float tt = F_MUL(Tk, F_SUB(1.0f, al));
   if (tt < GOF_T_EPS) return false;
   if (t > tmax) tmax = t;
-  *alpha = al;
-  *test_T = tt;
+  *h = RayHit{al, tt, t, unclamped && raw <= GOF_ALPHA_MAX};
   return true;
 }
 
@@ -160,11 +162,10 @@ struct Pass1 {
 };
 
 // One batch of the tile list into shared memory: the record and the reject threshold of ray_step (pass 1 and the colour walk)
-__device__ __forceinline__ void int_load_batch(const uint32_t* __restrict__ point_list, const GofSplat* __restrict__ splat,
-                                               float4 (*s_rec)[5], uint2 range, int progress, int total) {
+__device__ __forceinline__ void int_load_batch(const IntQuery& q, float4 (*s_rec)[5], uint2 range, int progress, int total) {
   if (progress < total) {
-    const uint32_t g = point_list[range.x + progress];
-    const float4* src = reinterpret_cast<const float4*>(splat + g);
+    const uint32_t g = q.point_list[range.x + progress];
+    const float4* src = reinterpret_cast<const float4*>(q.splat + g);
     const float4 r2 = __ldg(src + 2);
     s_rec[threadIdx.x][0] = __ldg(src); s_rec[threadIdx.x][1] = __ldg(src + 1);
     s_rec[threadIdx.x][2] = r2; s_rec[threadIdx.x][3] = __ldg(src + 3);
@@ -176,24 +177,18 @@ __device__ __forceinline__ void int_load_batch(const uint32_t* __restrict__ poin
 // CTOT: also sum the centre ray's blend in double, ctot = (T, C_0, C_1, C_2) with C = sum_j T_j alpha_j c_j (the colour walk's
 // totals, DESIGN.md 4.13); the float state is the same either way
 template <bool CTOT = false>
-__device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
-                                           const GofSplat* __restrict__ splat, float4 (*s_rec)[5], uint32_t s_base, int tile, int wx0,
-                                           int wy0, uint32_t pix_x, uint32_t pix_y, bool inside, int W, int H, float focal_x,
-                                           float focal_y, uint16_t* my_ids, double* ctot = nullptr) {
+__device__ __forceinline__ Pass1 int_pass1(const IntQuery& q, float4 (*s_rec)[5], uint32_t s_base, int tile, const GofWarpBlock& blk,
+                                           bool inside, uint16_t* my_ids, double* ctot = nullptr) {
   const int lane = threadIdx.x & 31;
   bool done = !inside;
 
   // forward.cu:920: ((pixf + offset) - S/2.) / focal, offsets 0 / -0.5 / +0.5
-  const float pfx = F_ADD((float)pix_x, 0.5f), pfy = F_ADD((float)pix_y, 0.5f);
-  const double hw = D_MUL((double)W, 0.5), hh = D_MUL((double)H, 0.5);
-  const float rx0 = (float)D_DIV(D_SUB((double)pfx, hw), (double)focal_x);
-  const float ry0 = (float)D_DIV(D_SUB((double)pfy, hh), (double)focal_y);
-  const float rxm = (float)D_DIV(D_SUB((double)F_ADD(pfx, -0.5f), hw), (double)focal_x);
-  const float rxp = (float)D_DIV(D_SUB((double)F_ADD(pfx, 0.5f), hw), (double)focal_x);
-  const float rym = (float)D_DIV(D_SUB((double)F_ADD(pfy, -0.5f), hh), (double)focal_y);
-  const float ryp = (float)D_DIV(D_SUB((double)F_ADD(pfy, 0.5f), hh), (double)focal_y);
+  const float pfx = F_ADD((float)blk.pix_x, 0.5f), pfy = F_ADD((float)blk.pix_y, 0.5f);
+  const float rx0 = gof_ray_at(pfx, q.W, q.focal_x), ry0 = gof_ray_at(pfy, q.H, q.focal_y);
+  const float rxm = gof_ray_at(F_ADD(pfx, -0.5f), q.W, q.focal_x), rxp = gof_ray_at(F_ADD(pfx, 0.5f), q.W, q.focal_x);
+  const float rym = gof_ray_at(F_ADD(pfy, -0.5f), q.H, q.focal_y), ryp = gof_ray_at(F_ADD(pfy, 0.5f), q.H, q.focal_y);
 
-  const uint2 range = ranges[tile];
+  const uint2 range = q.ranges[tile];
   const int total = (int)(range.y - range.x);
   const int rounds = (total + BATCH - 1) / BATCH;
 
@@ -203,7 +198,7 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
 
   for (int i = 0; i < rounds; ++i) {
     __syncthreads();
-    int_load_batch(point_list, splat, s_rec, range, i * BATCH + (int)threadIdx.x, total);
+    int_load_batch(q, s_rec, range, i * BATCH + (int)threadIdx.x, total);
     __syncthreads();
     const int nb = min(BATCH, total - i * BATCH);
 #pragma unroll 1
@@ -214,7 +209,8 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
       // The box holds every pixel at which one of the five rays can pass the alpha test (the half pixel of the corner
       // rays is inside it, added before the rounding to integers), so it is tested against the warp's 8x4 pixels as they
       // are: a Gaussian skipped here would be rejected by all five ray_step calls of all 32 lanes.
-      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
+      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && gof_box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), blk.wx0, blk.wy0,
+                                                                      blk.wx0 + 7, blk.wy0 + 3));
       while (m) {
         const int j = k * 32 + __ffs(m) - 1;
         m &= m - 1;
@@ -225,25 +221,25 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
         const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
         const float op = q2.z;
         const float thr = gof_lds32<64>(row);
-        float al, tt;
+        RayHit h;
         bool used = false;
-        if (ray_step<0>(v, op, thr, rx0, ry0, T0, tmax, &al, &tt)) {
+        if (ray_step<0>(v, op, thr, rx0, ry0, T0, tmax, &h)) {
           const float2 q3 = gof_lds64<48>(row);
-          C0 = F_FMA(T0, F_MUL(al, q2.w), C0);
-          C1 = F_FMA(T0, F_MUL(al, q3.x), C1);
-          C2 = F_FMA(T0, F_MUL(al, q3.y), C2);
-          Aacc = F_FMA(T0, al, Aacc);
+          C0 = F_FMA(T0, F_MUL(h.alpha, q2.w), C0);
+          C1 = F_FMA(T0, F_MUL(h.alpha, q3.x), C1);
+          C2 = F_FMA(T0, F_MUL(h.alpha, q3.y), C2);
+          Aacc = F_FMA(T0, h.alpha, Aacc);
           if constexpr (CTOT) {
-            const double w = ctot[0] * (double)al;
+            const double w = ctot[0] * (double)h.alpha;
             ctot[1] += w * (double)q2.w; ctot[2] += w * (double)q3.x; ctot[3] += w * (double)q3.y;
-            ctot[0] *= 1.0 - (double)al;
+            ctot[0] *= 1.0 - (double)h.alpha;
           }
-          T0 = tt; used = true;
+          T0 = h.test_T; used = true;
         }
-        if (ray_step<1>(v, op, thr, rxm, rym, T1, tmax, &al, &tt)) { T1 = tt; used = true; }
-        if (ray_step<2>(v, op, thr, rxp, rym, T2, tmax, &al, &tt)) { T2 = tt; used = true; }
-        if (ray_step<3>(v, op, thr, rxm, ryp, T3, tmax, &al, &tt)) { T3 = tt; used = true; }
-        if (ray_step<4>(v, op, thr, rxp, ryp, T4, tmax, &al, &tt)) { T4 = tt; used = true; }
+        if (ray_step<1>(v, op, thr, rxm, rym, T1, tmax, &h)) { T1 = h.test_T; used = true; }
+        if (ray_step<2>(v, op, thr, rxp, rym, T2, tmax, &h)) { T2 = h.test_T; used = true; }
+        if (ray_step<3>(v, op, thr, rxm, ryp, T3, tmax, &h)) { T3 = h.test_T; used = true; }
+        if (ray_step<4>(v, op, thr, rxp, ryp, T4, tmax, &h)) { T4 = h.test_T; used = true; }
         if (used) {
           last_contributor = contributor;
           my_ids[n_local] = (uint16_t)contributor;    // uint16 truncation as in forward.cu:983
@@ -254,6 +250,35 @@ __device__ __forceinline__ Pass1 int_pass1(const uint2* __restrict__ ranges, con
     }
   }
   return Pass1{range, T0, C0, C1, C2, tmax, Aacc, last_contributor, n_local};
+}
+
+// The quadric v[10] and the opacity of record g, read from global memory (pass 2 and the backward's walks)
+__device__ __forceinline__ float load_rec(const GofSplat* __restrict__ splat, uint32_t g, float* v) {
+  const float4* src = reinterpret_cast<const float4*>(splat + g);
+  const float4 q0 = __ldg(src), q1 = __ldg(src + 1), q2 = __ldg(src + 2);
+  v[0] = q0.x; v[1] = q0.y; v[2] = q0.z; v[3] = q0.w; v[4] = q1.x; v[5] = q1.y; v[6] = q1.z; v[7] = q1.w; v[8] = q2.x; v[9] = q2.y;
+  return q2.z;
+}
+
+// One pair of pass 2 and of the backward's walks 1 and 2 (forward.cu:1158-1190): the float alpha and what its derivative needs
+struct PairEval {
+  float al;       // alpha after the clamp; < GOF_ALPHA_MIN: rejected
+  bool free;      // op * exp(power) <= GOF_ALPHA_MAX: alpha carries a derivative
+  bool clamped;   // t was clamped to the point's depth
+  float t;
+};
+__device__ __forceinline__ PairEval pair_eval(const float* v, float op, float rx, float ry, float ray_depth) {
+  const GofPair p = gof_pair_geom(v, rx, ry);
+  PairEval e;
+  float t = F_DIV(-p.BB, F_ADD(p.AA, p.AA));
+  e.clamped = t > ray_depth;
+  if (e.clamped) t = ray_depth;
+  const float power = F_MUL(F_ADD(v[9], F_FMA(p.BB, t, F_MUL(t, F_MUL(p.AA, t)))), -0.5f);
+  const float raw = F_MUL(op, F_EXP(power));
+  e.al = fminf(raw, GOF_ALPHA_MAX);
+  e.free = raw <= GOF_ALPHA_MAX;
+  e.t = t;
+  return e;
 }
 
 // MIN_UPDATE: the query of one view of the multi-view opacity field (DESIGN.md 4.12).  Each point that projects folds its alpha
@@ -275,31 +300,28 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
 
   for (int tile = blockIdx.x; tile < a.tiles; tile += gridDim.x) {
     const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
-    const int wx0 = tile_x * 16 + (warp & 1) * 8, wy0 = tile_y * 16 + (warp >> 1) * 4;
-    const uint32_t pix_x = wx0 + (lane & 7), pix_y = wy0 + (lane >> 3);
-    const bool inside = pix_x < (uint32_t)a.W && pix_y < (uint32_t)a.H;
+    const GofWarpBlock blk = gof_warp_block(tile_x, tile_y, warp, lane);
+    const bool inside = blk.pix_x < (uint32_t)a.W && blk.pix_y < (uint32_t)a.H;
 
     // ---------------- pass 1 (forward.cu:886-993) ----------------
-    const Pass1 p1 = int_pass1(a.ranges, a.point_list, a.splat, s_rec, s_base, tile, wx0, wy0, pix_x, pix_y, inside, a.W, a.H,
-                               a.focal_x, a.focal_y, my_ids);
+    const Pass1 p1 = int_pass1(a, s_rec, s_base, tile, blk, inside, my_ids);
     const uint2 range = p1.range;
     const float T0 = p1.T0, C0 = p1.C0, C1 = p1.C1, C2 = p1.C2, tmax = p1.tmax, Aacc = p1.Aacc;
     const uint32_t last_contributor = p1.last_contributor, n_local = p1.n_local;
 
     // forward.cu:997-1008
-    float col0 = 0.f, col1 = 0.f, col2 = 0.f;
     if constexpr (!MIN_UPDATE) {
       const size_t slot = (size_t)tile * 256 + threadIdx.x;
       a.final_T[slot] = T0;
       a.ncontrib[slot] = last_contributor;
       a.ncontrib[(size_t)a.tiles * 256 + slot] = n_local;
-      col0 = F_FMA(T0, a.bg[0], C0); col1 = F_FMA(T0, a.bg[1], C1); col2 = F_FMA(T0, a.bg[2], C2);
     }
-    if constexpr (MIN_COLOR) { col0 = F_FMA(T0, a.bg[0], C0); col1 = F_FMA(T0, a.bg[1], C1); col2 = F_FMA(T0, a.bg[2], C2); }
-    s_cnt[threadIdx.x] = n_local;
+    float col0 = 0.f, col1 = 0.f, col2 = 0.f;   // the pixel colour C + T*bg
     if constexpr (!MIN_UPDATE || MIN_COLOR) {
+      col0 = F_FMA(T0, a.bg[0], C0); col1 = F_FMA(T0, a.bg[1], C1); col2 = F_FMA(T0, a.bg[2], C2);
       s_col[threadIdx.x][0] = col0; s_col[threadIdx.x][1] = col1; s_col[threadIdx.x][2] = col2;
     }
+    s_cnt[threadIdx.x] = n_local;
     if constexpr (!MIN_UPDATE) s_proj[threadIdx.x] = 0u;
     __threadfence_block();
     __syncthreads();
@@ -312,13 +334,9 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
         const uint32_t id = a.pt_list[q];
         const float2 xy = a.pt_xy[id];
         const float ray_depth = a.pt_depth[id];
-        // the pixel (thread slot) this point belongs to: pix <= xy < pix + 1 (forward.cu:1071-1072)
-        int lx = gof_f2i_rz(xy.x) - tile_x * 16, ly = gof_f2i_rz(xy.y) - tile_y * 16;
-        lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
-        const int pslot = ((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7);
+        const int pslot = gof_point_slot(xy.x, xy.y, tile_x, tile_y);
         if constexpr (!MIN_UPDATE) atomicAdd(&s_proj[pslot], 1u);
-        const float rx = (float)D_DIV(D_FMA((double)a.W, -0.5, (double)xy.x), (double)a.focal_x);
-        const float ry = (float)D_DIV(D_FMA((double)a.H, -0.5, (double)xy.y), (double)a.focal_y);
+        const float rx = gof_point_ray(xy.x, a.W, a.focal_x), ry = gof_point_ray(xy.y, a.H, a.focal_y);
         const uint32_t cnt = s_cnt[pslot];
         const uint16_t* ids = slab + (size_t)pslot * GOF_INT_MAX_CONTRIB;
         float point_alpha = 0.f, point_T = 1.f;
@@ -327,15 +345,9 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
           const uint32_t cid = (uint32_t)ids[c];
           if (cid <= prev) break;     // a wrapped uint16 id can never be matched again by the running index (:1141-1149)
           prev = cid;
-          const uint32_t g = a.point_list[range.x + cid - 1];
-          const float4* src = reinterpret_cast<const float4*>(a.splat + g);
-          const float4 q0 = __ldg(src), q1 = __ldg(src + 1), q2 = __ldg(src + 2);
-          const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
-          const GofPair p = gof_pair_geom(v, rx, ry);
-          float t = F_DIV(-p.BB, F_ADD(p.AA, p.AA));
-          if (t > ray_depth) t = ray_depth;
-          const float power = F_MUL(F_ADD(v[9], F_FMA(p.BB, t, F_MUL(t, F_MUL(p.AA, t)))), -0.5f);
-          const float al = fminf(F_MUL(q2.z, F_EXP(power)), GOF_ALPHA_MAX);
+          float v[10];
+          const float op = load_rec(a.splat, a.point_list[range.x + cid - 1], v);
+          const float al = pair_eval(v, op, rx, ry, ray_depth).al;
           if (al < GOF_ALPHA_MIN) continue;
           point_alpha = F_FMA(al, point_T, point_alpha);
           point_T = F_MUL(point_T, F_SUB(1.0f, al));
@@ -360,7 +372,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
     }
     __syncthreads();
     if (!MIN_UPDATE && inside) {
-      const size_t pid = (size_t)pix_y * a.W + pix_x;
+      const size_t pid = (size_t)blk.pix_y * a.W + blk.pix_x;
       a.out_color[0 * HW + pid] = col0;
       a.out_color[1 * HW + pid] = col1;
       a.out_color[2 * HW + pid] = col2;
@@ -376,20 +388,10 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
 // A = sum_j alpha_j T_j over the point's contributors is 1 - prod_j (1 - alpha_j), so with the list, the rejects and the clamps
 // held fixed dA/dalpha_j = T / (1 - alpha_j), T = prod_i (1 - alpha_i) the point's final transmittance.  Walk 1 forms T and the
 // point's own gradient; walk 2 (which needs T) hands each pair's dL/dview2gaussian to its Gaussian's accumulator row.
-struct IntBwdArgs {
-  int W, H, grid_x, tiles;
-  float focal_x, focal_y;
-  const uint2* ranges;
-  const uint32_t* point_list;
-  const GofSplat* splat;
-  const uint2* pranges;
-  const uint32_t* pt_list;
-  const float2* pt_xy;
-  const float* pt_depth;
+struct IntBwdArgs : IntQuery {   // ids: the forward's slab, rewritten
   const float* points3D;
   const float* vm;
   const float* dL_dalpha;   // [PN]
-  uint16_t* ids;            // [gridDim][256][1024] (the forward's slab, rewritten)
   double* grad_acc;         // [P][16]: dL_dview2gaussian[10] of every pair lands in 0..9 (zeroed by the launcher)
   float* dL_dpoints3D;      // [PN][3] or NULL (zeroed by the launcher: points that do not project keep the zeros)
 };
@@ -400,26 +402,13 @@ struct IntBwdColorArgs : IntBwdArgs {
   const float* bg;          // [3]
 };
 
-// One pair of walk 1 / walk 2: the forward's float alpha (same operations as k_integrate's pass 2) and what its derivative needs.
-struct PairEval {
-  float al;       // alpha after the clamp; < GOF_ALPHA_MIN: rejected
-  bool free;      // op * exp(power) <= GOF_ALPHA_MAX: alpha carries a derivative
-  bool clamped;   // t was clamped to the point's depth
-  float t;
-};
-__device__ __forceinline__ PairEval pair_eval(const float* v, float op, float rx, float ry, float ray_depth, GofPair* pp) {
-  const GofPair p = gof_pair_geom(v, rx, ry);
-  PairEval e;
-  float t = F_DIV(-p.BB, F_ADD(p.AA, p.AA));
-  e.clamped = t > ray_depth;
-  if (e.clamped) t = ray_depth;
-  const float power = F_MUL(F_ADD(v[9], F_FMA(p.BB, t, F_MUL(t, F_MUL(p.AA, t)))), -0.5f);
-  const float raw = F_MUL(op, F_EXP(power));
-  e.al = fminf(raw, GOF_ALPHA_MAX);
-  e.free = raw <= GOF_ALPHA_MAX;
-  e.t = t;
-  *pp = p;
-  return e;
+// A pair's dL/dview2gaussian rows from f = dL/dCC, at depth t on the ray (x, y, 1): power = -1/2 (AA t^2 + BB t + CC) with t held
+// fixed, AA = r^T Sigma r and BB = 2 b.r, the off-diagonal entries of Sigma counted twice (walk 2 and the colour walk)
+__device__ __forceinline__ void v2g_rows(double f, double t, double x, double y, double* d) {
+  const double ft2 = f * t * t, ft = f * t;
+  d[0] = ft2 * x * x; d[1] = 2.0 * ft2 * x * y; d[2] = 2.0 * ft2 * x;
+  d[3] = ft2 * y * y; d[4] = 2.0 * ft2 * y; d[5] = ft2;
+  d[6] = 2.0 * ft * x; d[7] = 2.0 * ft * y; d[8] = 2.0 * ft; d[9] = f;
 }
 
 // 94 registers: two CTAs per SM (the query's three do not fit), and the grid is that many, so no CTA waits for a second wave
@@ -432,9 +421,9 @@ constexpr int INT_BWD_CTAS_PER_SM = 2;
 // (the recorded uint16 ids wrap past 65 535).  With T_j, the suffix S_j = tot - sum_{i<=j} T_i alpha_i c_i (tot from pass 1, in
 // double):  dL/dc_j = T_j alpha_j dL/dC  and  dL/dalpha_j = dL/dC . (T_j c_j - S_j / (1 - alpha_j)).  A warp visits its candidate
 // Gaussians in step, so each pair's 13 rows are summed over the warp and sent by one lane.
-__device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 (*s_rec)[5], uint32_t s_base, uint2 range, int wx0,
-                                               int wy0, uint32_t pix_x, uint32_t pix_y, const double* dC, const double* tot,
-                                               uint32_t last, uint32_t* s_last) {
+__device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 (*s_rec)[5], uint32_t s_base, uint2 range,
+                                               const GofWarpBlock& blk, const double* dC, const double* tot, uint32_t last,
+                                               uint32_t* s_last) {
   const int lane = threadIdx.x & 31;
   const bool want = last > 0 && (dC[0] != 0.0 || dC[1] != 0.0 || dC[2] != 0.0);
   if (threadIdx.x == 0) *s_last = 0u;
@@ -446,15 +435,13 @@ __device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 
   const bool warp_wants = __any_sync(0xffffffffu, want);
   const uint32_t warp_last = __reduce_max_sync(0xffffffffu, want ? last : 0u);
 
-  const float pfx = F_ADD((float)pix_x, 0.5f), pfy = F_ADD((float)pix_y, 0.5f);
-  const float rx0 = (float)D_DIV(D_SUB((double)pfx, D_MUL((double)a.W, 0.5)), (double)a.focal_x);
-  const float ry0 = (float)D_DIV(D_SUB((double)pfy, D_MUL((double)a.H, 0.5)), (double)a.focal_y);
+  const float rx0 = gof_ray(blk.pix_x, a.W, a.focal_x), ry0 = gof_ray(blk.pix_y, a.H, a.focal_y);
   float T0 = 1.f, tmax = 0.f;
   double T = 1.0, pre0 = 0.0, pre1 = 0.0, pre2 = 0.0;
   const int rounds = (total + BATCH - 1) / BATCH;
   for (int i = 0; i < rounds; ++i) {
     __syncthreads();
-    int_load_batch(a.point_list, a.splat, s_rec, range, i * BATCH + (int)threadIdx.x, total);
+    int_load_batch(a, s_rec, range, i * BATCH + (int)threadIdx.x, total);
     __syncthreads();
     if (!warp_wants) continue;
     const int nb = min(BATCH, total - i * BATCH);
@@ -463,7 +450,8 @@ __device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 
       if (k * 32 >= nb || (uint32_t)(i * BATCH + k * 32) >= warp_last) break;
       const int idx = k * 32 + lane;
       const float4 qb = s_rec[idx][3];
-      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
+      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && gof_box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), blk.wx0, blk.wy0,
+                                                                      blk.wx0 + 7, blk.wy0 + 3));
       while (m) {
         const int j = k * 32 + __ffs(m) - 1;
         m &= m - 1;
@@ -477,13 +465,12 @@ __device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 
           const float4 q0 = gof_lds128<0>(row), q1 = gof_lds128<16>(row), q2 = gof_lds128<32>(row);
           const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
           const float op = q2.z;
-          float al, tt;
-          if (ray_step<0>(v, op, gof_lds32<64>(row), rx0, ry0, T0, tmax, &al, &tt)) {
-            T0 = tt;
-            has = true;
+          RayHit h;
+          if (ray_step<0>(v, op, gof_lds32<64>(row), rx0, ry0, T0, tmax, &h)) {
+            T0 = h.test_T; has = true;
             const float2 q3 = gof_lds64<48>(row);
             const double c[3] = {(double)q2.w, (double)q3.x, (double)q3.y};
-            const double alpha = al, w = T * alpha, om = 1.0 - alpha;
+            const double alpha = h.alpha, w = T * alpha, om = 1.0 - alpha;
             pre0 += w * c[0]; pre1 += w * c[1]; pre2 += w * c[2];
             const double S[3] = {tot[1] - pre0, tot[2] - pre1, tot[3] - pre2};
             double dLdal = 0.0;
@@ -493,18 +480,8 @@ __device__ __forceinline__ void int_color_walk(const IntBwdColorArgs& a, float4 
               dLdal += dC[ch] * (T * c[ch] - S[ch] / om);
             }
             T *= om;
-            // the derivative pieces of ray_step's alpha: power = -1/2 (CC - BB^2 / (4 AA)), stationary in t = -BB / (2 AA)
-            float AA, BB;
-            pair_geom_k<0>(v, rx0, ry0, &AA, &BB);
-            const float t = F_DIV(-BB, F_ADD(AA, AA));
-            const float power = (float)D_MUL(D_FMA((double)F_DIV(-BB, AA), D_MUL((double)BB, 0.25), (double)v[9]), -0.5);
-            if (power <= 0.0f && F_MUL(op, F_EXP(power)) <= GOF_ALPHA_MAX) {
-              const double f = -0.5 * dLdal * alpha;   // dL/dpower times d power / d CC
-              const double x = rx0, y = ry0, td = t, ft2 = f * td * td, ft = f * td;
-              d[0] = ft2 * x * x; d[1] = 2.0 * ft2 * x * y; d[2] = 2.0 * ft2 * x;
-              d[3] = ft2 * y * y; d[4] = 2.0 * ft2 * y; d[5] = ft2;
-              d[6] = 2.0 * ft * x; d[7] = 2.0 * ft * y; d[8] = 2.0 * ft; d[9] = f;
-            }
+            // power = -1/2 (CC - BB^2 / (4 AA)) is stationary in t = -BB / (2 AA), so its derivative is -1/2 (t^2, t, 1)
+            if (h.free) v2g_rows(-0.5 * dLdal * alpha, h.t, rx0, ry0, d);
           }
         }
         const uint32_t with = __ballot_sync(0xffffffffu, has);
@@ -541,13 +518,11 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
     const uint2 pr = a.pranges[tile];
     if (pr.x == pr.y) continue;   // uniform over the CTA: no point here, no list needed
     const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
-    const int wx0 = tile_x * 16 + (warp & 1) * 8, wy0 = tile_y * 16 + (warp >> 1) * 4;
-    const uint32_t pix_x = wx0 + (lane & 7), pix_y = wy0 + (lane >> 3);
-    const bool inside = pix_x < (uint32_t)a.W && pix_y < (uint32_t)a.H;
+    const GofWarpBlock blk = gof_warp_block(tile_x, tile_y, warp, lane);
+    const bool inside = blk.pix_x < (uint32_t)a.W && blk.pix_y < (uint32_t)a.H;
 
     double tot[4] = {1.0, 0.0, 0.0, 0.0};
-    const Pass1 p1 = int_pass1<COLOR>(a.ranges, a.point_list, a.splat, s_rec, s_base, tile, wx0, wy0, pix_x, pix_y, inside, a.W,
-                                      a.H, a.focal_x, a.focal_y, my_ids, COLOR ? tot : nullptr);
+    const Pass1 p1 = int_pass1<COLOR>(a, s_rec, s_base, tile, blk, inside, my_ids, COLOR ? tot : nullptr);
     const uint2 range = p1.range;
     s_cnt[threadIdx.x] = p1.n_local;
     __threadfence_block();
@@ -563,11 +538,8 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
         id = a.pt_list[q];
         const float2 xy = a.pt_xy[id];
         ray_depth = a.pt_depth[id];
-        int lx = gof_f2i_rz(xy.x) - tile_x * 16, ly = gof_f2i_rz(xy.y) - tile_y * 16;
-        lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
-        pslot = ((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7);
-        rx = (float)D_DIV(D_FMA((double)a.W, -0.5, (double)xy.x), (double)a.focal_x);
-        ry = (float)D_DIV(D_FMA((double)a.H, -0.5, (double)xy.y), (double)a.focal_y);
+        pslot = gof_point_slot(xy.x, xy.y, tile_x, tile_y);
+        rx = gof_point_ray(xy.x, a.W, a.focal_x); ry = gof_point_ray(xy.y, a.H, a.focal_y);
       }
       const float dLdA = valid ? a.dL_dalpha[id] : 0.f;
       const uint16_t* ids = slab + (size_t)(pslot & 255) * GOF_INT_MAX_CONTRIB;
@@ -581,12 +553,9 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
         if (cid <= prev) break;   // a wrapped uint16 id ends the list, as in the forward
         prev = cid;
         n_eff = c + 1;
-        const uint32_t g = a.point_list[range.x + cid - 1];
-        const float4* src = reinterpret_cast<const float4*>(a.splat + g);
-        const float4 q0 = __ldg(src), q1 = __ldg(src + 1), q2 = __ldg(src + 2);
-        const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
-        GofPair p;
-        const PairEval e = pair_eval(v, q2.z, rx, ry, ray_depth, &p);
+        float v[10];
+        const float op = load_rec(a.splat, a.point_list[range.x + cid - 1], v);
+        const PairEval e = pair_eval(v, op, rx, ry, ray_depth);
         if (e.al < GOF_ALPHA_MIN) continue;
         const double om = 1.0 - (double)e.al;
         T *= om;
@@ -640,18 +609,12 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
         if (c < n_eff) {
           g = a.point_list[range.x + (uint32_t)ids[c] - 1];
           if (dLdA != 0.f) {
-            const float4* src = reinterpret_cast<const float4*>(a.splat + g);
-            const float4 q0 = __ldg(src), q1 = __ldg(src + 1), q2 = __ldg(src + 2);
-            const float v[10] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y};
-            GofPair p;
-            const PairEval e = pair_eval(v, q2.z, rx, ry, ray_depth, &p);
+            float v[10];
+            const float op = load_rec(a.splat, g, v);
+            const PairEval e = pair_eval(v, op, rx, ry, ray_depth);
             if (e.al >= GOF_ALPHA_MIN && e.free) {
               has = true;
-              const double f = -0.5 * s * (double)e.al / (1.0 - (double)e.al);   // dL/dpower
-              const double t = e.t, x = rx, y = ry, ft2 = f * t * t, ft = f * t;
-              d[0] = ft2 * x * x; d[1] = 2.0 * ft2 * x * y; d[2] = 2.0 * ft2 * x;
-              d[3] = ft2 * y * y; d[4] = 2.0 * ft2 * y; d[5] = ft2;
-              d[6] = 2.0 * ft * x; d[7] = 2.0 * ft * y; d[8] = 2.0 * ft; d[9] = f;
+              v2g_rows(-0.5 * s * (double)e.al / (1.0 - (double)e.al), e.t, rx, ry, d);
             }
           }
         }
@@ -687,9 +650,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
         if (q < pr.y) {
           const uint32_t id = a.pt_list[q];
           const float2 xy = a.pt_xy[id];
-          int lx = gof_f2i_rz(xy.x) - tile_x * 16, ly = gof_f2i_rz(xy.y) - tile_y * 16;
-          lx = min(15, max(0, lx)); ly = min(15, max(0, ly));
-          pslot = ((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7);
+          pslot = gof_point_slot(xy.x, xy.y, tile_x, tile_y);
 #pragma unroll
           for (int ch = 0; ch < 3; ++ch) g[ch] = a.dL_dcolor[3 * (size_t)id + ch];
         }
@@ -709,19 +670,35 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
       __syncthreads();
       const double dC[3] = {s_dC[threadIdx.x][0], s_dC[threadIdx.x][1], s_dC[threadIdx.x][2]};
       tot[1] += tot[0] * (double)a.bg[0]; tot[2] += tot[0] * (double)a.bg[1]; tot[3] += tot[0] * (double)a.bg[2];
-      int_color_walk(a, s_rec, s_base, range, wx0, wy0, pix_x, pix_y, dC, tot, p1.last_contributor, &s_last);
+      int_color_walk(a, s_rec, s_base, range, blk, dC, tot, p1.last_contributor, &s_last);
     }
     __syncthreads();
   }
 }
 
+// The query's state in the caller's buffers.  The point sort of gof_launch_integrate (PN > 0 pairs over pt_key_bits) leaves
+// the sorted ids in val_a or val_b by the parity of its passes.
+IntQuery int_query(const GofView& v, const GofSplat* splat, const uint32_t* point_list, const uint2* ranges, const char* pts,
+                   const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL) {
+  IntQuery q;
+  q.W = v.W; q.H = v.H; q.grid_x = v.grid_x; q.tiles = v.tiles; q.focal_x = v.focal_x; q.focal_y = v.focal_y;
+  q.ranges = ranges; q.point_list = point_list; q.splat = splat;
+  q.pranges = reinterpret_cast<const uint2*>(pbin + PBL.pranges);
+  q.pt_list = reinterpret_cast<const uint32_t*>(pbin + (gof_radix_result_in_b(pt_key_bits(v.tiles)) ? PBL.val_b : PBL.val_a));
+  q.pt_xy = reinterpret_cast<const float2*>(pts + PL.xy); q.pt_depth = reinterpret_cast<const float*>(pts + PL.depth);
+  q.ids = reinterpret_cast<uint16_t*>(pbin + PBL.ids);
+  return q;
+}
+
 }  // namespace
 
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
-                         const uint32_t* point_list, const uint2* ranges, char* img, const GofImageLayout& IL, char* pts,
-                         const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, float* out_color, float* out_alpha,
-                         float* out_color_int, const GofIntMin* mn, cudaStream_t st) {
+                         const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin, float* out_color,
+                         float* out_alpha, float* out_color_int, const GofIntMin* mn, cudaStream_t st) {
   const bool debug = s->debug != 0;
+  const GofImageLayout IL = gof_image_layout(s->width, s->height);
+  const GofPointLayout PL = gof_point_layout((size_t)PN);
+  const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count());
   PtArgs pa{};
   pa.PN = PN; pa.W = v.W; pa.H = v.H; pa.grid_x = v.grid_x; pa.grid_y = v.grid_y; pa.tiles = v.tiles;
   pa.focal_x = v.focal_x; pa.focal_y = v.focal_y; pa.points3D = points3D; pa.vm = s->viewmatrix;
@@ -733,19 +710,14 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
   pa.key = ka; pa.val = va;
   GOF_LAUNCH("preprocess_points", st, k_preprocess_points<<<(PN + 255) / 256, 256, 0, st>>>(pa));
   GOF_LAUNCH_CHECK(debug, st);
-  int in_b = 0;
-  uint2* pranges = reinterpret_cast<uint2*>(pbin + PBL.pranges);
   int rc = gof_sort_points_by_tile((size_t)PN, pt_key_bits(v.tiles), PT_KEY_SHIFT, ka, kb, va, vb,
-                                   reinterpret_cast<uint32_t*>(pbin + PBL.hist), pranges, v.tiles, debug, st, &in_b);
+                                   reinterpret_cast<uint32_t*>(pbin + PBL.hist), reinterpret_cast<uint2*>(pbin + PBL.pranges),
+                                   v.tiles, debug, st);
   if (rc != GOF_OK) return rc;
 
   IntArgs a{};
-  a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.tiles = v.tiles; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
-  a.ranges = ranges;
-  a.point_list = point_list;
-  a.splat = splat;
-  a.pranges = pranges; a.pt_list = in_b ? vb : va; a.pt_xy = pa.xy; a.pt_depth = pa.depth; a.bg = s->background;
-  a.ids = reinterpret_cast<uint16_t*>(pbin + PBL.ids);
+  static_cast<IntQuery&>(a) = int_query(v, splat, point_list, ranges, pts, PL, pbin, PBL);
+  a.bg = s->background;
   a.final_T = reinterpret_cast<float*>(img + IL.accum);
   a.ncontrib = reinterpret_cast<uint32_t*>(img + IL.ncontrib);
   a.out_color = out_color; a.out_alpha = out_alpha; a.out_color_int = out_color_int;
@@ -766,18 +738,14 @@ size_t gof_integrate_backward_scratch(int P) { return P > 0 ? 2 * gof_align_up((
 
 int gof_launch_integrate_backward(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const int* radii,
                                   char* geom, const GofGeomLayout& GL, const uint32_t* point_list, const uint2* ranges, const char* pts,
-                                  const GofPointLayout& PL, char* pbin, const GofPointBinLayout& PBL, const float* dL_dalpha,
-                                  const float* dL_dcolor_int, float* dL_dpoints3D, const gof_backward_out_t& o, cudaStream_t st) {
+                                  char* pbin, const float* dL_dalpha, const float* dL_dcolor_int, float* dL_dpoints3D,
+                                  const gof_backward_out_t& o, cudaStream_t st) {
   const bool debug = s->debug != 0;
+  const GofPointBinLayout PBL = gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count());
   IntBwdColorArgs a{};
-  a.W = v.W; a.H = v.H; a.grid_x = v.grid_x; a.tiles = v.tiles; a.focal_x = v.focal_x; a.focal_y = v.focal_y;
-  a.ranges = ranges; a.point_list = point_list; a.splat = reinterpret_cast<const GofSplat*>(geom + GL.splat);
-  a.pranges = reinterpret_cast<const uint2*>(pbin + PBL.pranges);
-  // where gof_launch_integrate's point sort (PN > 0 pairs, the same key bits) left the sorted ids
-  a.pt_list = reinterpret_cast<const uint32_t*>(pbin + (gof_radix_result_in_b(pt_key_bits(v.tiles)) ? PBL.val_b : PBL.val_a));
-  a.pt_xy = reinterpret_cast<const float2*>(pts + PL.xy); a.pt_depth = reinterpret_cast<const float*>(pts + PL.depth);
+  static_cast<IntQuery&>(a) = int_query(v, reinterpret_cast<const GofSplat*>(geom + GL.splat), point_list, ranges, pts,
+                                        gof_point_layout((size_t)PN), pbin, PBL);
   a.points3D = points3D; a.vm = s->viewmatrix; a.dL_dalpha = dL_dalpha;
-  a.ids = reinterpret_cast<uint16_t*>(pbin + PBL.ids);
   a.grad_acc = reinterpret_cast<double*>(geom + GL.grad_acc);
   a.dL_dpoints3D = dL_dpoints3D;
   a.dL_dcolor = dL_dcolor_int; a.bg = s->background;

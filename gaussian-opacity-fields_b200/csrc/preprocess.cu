@@ -164,8 +164,7 @@ __global__ void __launch_bounds__(256) k_preprocess(const PreArgs a) {
     const GofBox box = a.cull ? gof_cull_bbox(rec.v2g, rec.opacity, lambda_min, a.W, a.H, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy,
                                                 a.box_margin)
                               : gof_full_box();
-    rec.box_lo = ((uint32_t)box.x0 & 0xffffu) | ((uint32_t)box.y0 << 16);
-    rec.box_hi = ((uint32_t)box.x1 & 0xffffu) | ((uint32_t)box.y1 << 16);
+    gof_box_pack(box, &rec.box_lo, &rec.box_hi);
     a.depth[idx] = tz;
     // Constant of the blend kernel's conservative pair reject (render_fwd.cu): with thr = -ln(255 op) - 2e-3 (the margin
     // covers expf and the float rounding of power) a pair is provably below alpha = 1/255 when

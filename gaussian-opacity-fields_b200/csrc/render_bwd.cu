@@ -94,9 +94,8 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_backward(const Bwd
   // this warp's mask slab [GROUPS][32]; its first word also carries the tile's deepest contributor before the first batch
   uint32_t* const s_mask = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(s_dyn) + SMEM_RECORDS) + warp * GROUPS * 32;
   uint32_t* const s_max = s_mask - warp * GROUPS * 32;
-  const int wx0 = tile_x * 16 + (warp & 1) * 8, wy0 = tile_y * 16 + (warp >> 1) * 4;
-  const uint32_t pix_x = wx0 + (lane & 7);
-  const uint32_t pix_y = wy0 + (lane >> 3);
+  const GofWarpBlock blk = gof_warp_block(tile_x, tile_y, warp, lane);
+  const uint32_t pix_x = blk.pix_x, pix_y = blk.pix_y;
   const bool inside = pix_x < (uint32_t)a.W && pix_y < (uint32_t)a.H;
   const float rx = gof_ray(pix_x, a.W, a.focal_x);
   const float ry = gof_ray(pix_y, a.H, a.focal_y);

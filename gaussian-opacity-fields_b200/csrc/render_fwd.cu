@@ -41,12 +41,6 @@ struct FwdArgs {
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
 
-__device__ __forceinline__ bool box_hits(uint32_t lo, uint32_t hi, int wx0, int wy0, int wx1, int wy1) {
-  const int x0 = (int)(short)(lo & 0xffffu), y0 = (int)(short)(lo >> 16);
-  const int x1 = (int)(short)(hi & 0xffffu), y1 = (int)(short)(hi >> 16);
-  return x0 <= wx1 && x1 >= wx0 && y0 <= wy1 && y1 >= wy0;
-}
-
 __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_forward(const FwdArgs a) {
   // Rows of 80 bytes = the 64-byte record of a staged Gaussian + (K', -, -, -), K' = the reject constant (see
   // GofGeomLayout::reject_k).  One row base serves every load of a visit.  Two buffers (40 KB), filled by bulk copies.
@@ -58,9 +52,8 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_forward(const FwdA
   const int tile = blockIdx.x;
   const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int wx0 = tile_x * 16 + (warp & 1) * 8, wy0 = tile_y * 16 + (warp >> 1) * 4;   // this warp's 8x4 pixel block
-  const uint32_t pix_x = wx0 + (lane & 7);
-  const uint32_t pix_y = wy0 + (lane >> 3);
+  const GofWarpBlock blk = gof_warp_block(tile_x, tile_y, warp, lane);   // this warp's 8x4 pixel block and the lane's pixel
+  const uint32_t pix_x = blk.pix_x, pix_y = blk.pix_y;
   const bool inside = pix_x < (uint32_t)a.W && pix_y < (uint32_t)a.H;
   bool done = !inside;
 
@@ -135,7 +128,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 4) k_render_forward(const FwdA
       if (k * 32 >= nb) break;
       const int idx = k * 32 + lane;
       const float4 qb = gof_lds128<48>(buf_base + (uint32_t)idx * 80u);
-      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), wx0, wy0, wx0 + 7, wy0 + 3));
+      uint32_t m = __ballot_sync(0xffffffffu, idx < nb && gof_box_hits(__float_as_uint(qb.z), __float_as_uint(qb.w), blk.wx0, blk.wy0, blk.wx0 + 7, blk.wy0 + 3));
       uint32_t mybits = 0u;   // bit b: this pixel blended entry k*32+b of the batch
       while (m != 0u) {
         const int b = __ffs(m) - 1;

@@ -78,4 +78,31 @@ void hm_bbox(const float* v2g, float opacity, const float* scale, int W, int H, 
 void hm_sh(int deg, const float* mean, const float* campos, const float* sh, float* rgb, unsigned char* clamped) {
   gof_sh_to_rgb(deg, mean[0], mean[1], mean[2], campos, sh, rgb, clamped);
 }
+
+// the pixel of thread (warp, lane) in tile (tile_x, tile_y): out = (wx0, wy0, pix_x, pix_y)
+void hm_warp_block(int tile_x, int tile_y, int warp, int lane, int* out) {
+  const GofWarpBlock b = gof_warp_block(tile_x, tile_y, warp, lane);
+  out[0] = b.wx0; out[1] = b.wy0; out[2] = (int)b.pix_x; out[3] = (int)b.pix_y;
+}
+
+int hm_pixel_slot(int lx, int ly) { return gof_pixel_slot(lx, ly); }
+
+// n points: slot[i] = gof_point_slot(xy[2i], xy[2i+1], tile[2i], tile[2i+1])
+void hm_point_slots(int n, const float* xy, const int* tile, int* slot) {
+  for (int i = 0; i < n; ++i) slot[i] = gof_point_slot(xy[2 * i], xy[2 * i + 1], tile[2 * i], tile[2 * i + 1]);
+}
+
+// n boxes (x0, y0, x1, y1) packed into the record's words, each tested against the 8x4 block at rect (wx0, wy0):
+// words[2i..2i+1] = (lo, hi), hit[i] = gof_box_hits
+void hm_box_hits(int n, const int* box, const int* rect, unsigned* words, int* hit) {
+  for (int i = 0; i < n; ++i) {
+    GofBox b;
+    b.x0 = box[4 * i]; b.y0 = box[4 * i + 1]; b.x1 = box[4 * i + 2]; b.y1 = box[4 * i + 3];
+    uint32_t lo, hi;
+    gof_box_pack(b, &lo, &hi);
+    words[2 * i] = lo; words[2 * i + 1] = hi;
+    const int wx0 = rect[2 * i], wy0 = rect[2 * i + 1];
+    hit[i] = gof_box_hits(lo, hi, wx0, wy0, wx0 + 7, wy0 + 3);
+  }
+}
 }

@@ -103,3 +103,72 @@ def test_pair_math_matches_oracle_render(hm):
         pw = np.float32(-0.5 * (-(np.float64(out[1]) / np.float64(out[0])) * (np.float64(out[1]) / 4.0) + np.float64(v[9])))
         pw = min(pw, np.float32(0.0))
         assert abs(out[3] - pw) <= 1e-6 * max(abs(pw), 1.0)
+
+
+def test_tile_slots_and_box_packing(hm):
+    """The thread <-> pixel map of a 16x16 tile, the pixel slot of a projected point, and the 16-bit box packing with its overlap
+    test against a warp's 8x4 block, checked against plain integer arithmetic."""
+    i32 = ctypes.POINTER(ctypes.c_int)
+    # every thread of a tile gets its own pixel, and gof_pixel_slot maps that pixel back to the thread
+    for tile_x, tile_y in ((0, 0), (3, 1), (119, 67)):
+        seen = set()
+        out = np.zeros(4, np.int32)
+        for t in range(256):
+            warp, lane = t >> 5, t & 31
+            hm.hm_warp_block(tile_x, tile_y, warp, lane, _p(out))
+            wx0, wy0, px, py = (int(v) for v in out)
+            assert (wx0, wy0) == (tile_x * 16 + (warp & 1) * 8, tile_y * 16 + (warp >> 1) * 4)
+            assert wx0 <= px < wx0 + 8 and wy0 <= py < wy0 + 4
+            lx, ly = px - tile_x * 16, py - tile_y * 16
+            assert hm.hm_pixel_slot(lx, ly) == t
+            seen.add((lx, ly))
+        assert len(seen) == 256
+
+    # a point falls in the pixel that contains it (pix <= xy < pix + 1), clamped to its tile
+    rng = np.random.default_rng(5)
+    W, H = 1920, 1080
+    xy = np.concatenate([
+        rng.uniform(0, [W, H], (4000, 2)),
+        np.stack(np.meshgrid(np.arange(0, W + 1, 16.0), [0.0, 15.5, 16.0, H - 1e-3])).reshape(2, -1).T,   # tile edges
+        [[np.nextafter(np.float32(16), 0), 0.0], [np.nextafter(np.float32(W), 0), np.nextafter(np.float32(H), 0)]],
+    ]).astype(np.float32)
+    tile = np.minimum((xy // 16).astype(np.int32), [(W + 15) // 16 - 1, (H + 15) // 16 - 1]).astype(np.int32)
+    # and points the clamp takes to the tile's edge: left of / above it (trunc towards 0), and past its right / lower edge
+    xy = np.concatenate([xy, [[-0.75, -0.25], [5.0, -3.0], [40.0, 3.0], [3.0, 47.9]]]).astype(np.float32)
+    tile = np.concatenate([tile, [[0, 0], [0, 0], [1, 0], [0, 1]]]).astype(np.int32)
+    slots = np.zeros(len(xy), np.int32)
+    hm.hm_point_slots(len(xy), _p(xy), _p(tile), _p(slots))
+    lxy = np.clip(np.trunc(xy).astype(np.int64) - tile * 16, 0, 15)
+    lx, ly = lxy[:, 0], lxy[:, 1]
+    expect = ((ly >> 2) * 2 + (lx >> 3)) * 32 + (ly & 3) * 8 + (lx & 7)
+    np.testing.assert_array_equal(slots, expect)
+    own = (xy >= tile * 16).all(1) & (xy < (tile + 1) * 16).all(1)   # the point lies in its tile: no clamp, the containing pixel
+    assert (~own).sum() == 8   # x = W on the image's right edge (four rows), and the four points placed outside their tile
+    np.testing.assert_array_equal(lxy[own], np.floor(xy[own]).astype(np.int64) - tile[own] * 16)
+
+    # box packing: every bound in [-32768, 32767], the full and the empty box among them
+    lo, hi = -32768, 32767
+    edge = np.array([lo, lo + 1, -8, -1, 0, 1, 7, hi - 7, hi - 1, hi])
+    n = 20000
+    box = rng.integers(lo, hi + 1, (n, 4))
+    pick = rng.random((n, 4)) < 0.3
+    box[pick] = rng.choice(edge, pick.sum())
+    small = rng.random(n) < 0.5   # boxes of a few pixels near the blocks, where the overlap test is decided at the edges
+    box[small, 0:2] = rng.integers(-40, 40, (small.sum(), 2))
+    box[small, 2:4] = box[small, 0:2] + rng.integers(-2, 12, (small.sum(), 2))
+    box = np.concatenate([box, [[lo, lo, hi, hi], [hi, hi, lo, lo]] * 4]).astype(np.int32)
+    rect = rng.integers(-48, 48, (len(box), 2))
+    rect[:n][small] = box[:n][small, 0:2] + rng.integers(-10, 4, (small.sum(), 2))
+    rect[-8:] = [[lo, lo], [lo, lo], [hi - 7, hi - 3], [hi - 7, hi - 3], [0, 0], [0, 0], [-8, -4], [-8, -4]]
+    rect = rect.astype(np.int32)
+    words = np.zeros((len(box), 2), np.uint32)
+    hits = np.zeros(len(box), np.int32)
+    hm.hm_box_hits(len(box), _p(box), _p(rect), _p(words), _p(hits))
+    b = box.astype(np.int64)
+    np.testing.assert_array_equal(words[:, 0], (b[:, 0] & 0xFFFF) | ((b[:, 1] & 0xFFFF) << 16))
+    np.testing.assert_array_equal(words[:, 1], (b[:, 2] & 0xFFFF) | ((b[:, 3] & 0xFFFF) << 16))
+    wx0, wy0 = rect[:, 0].astype(np.int64), rect[:, 1].astype(np.int64)
+    expect = (b[:, 0] <= wx0 + 7) & (b[:, 2] >= wx0) & (b[:, 1] <= wy0 + 3) & (b[:, 3] >= wy0)
+    np.testing.assert_array_equal(hits.astype(bool), expect)
+    assert hits[-8::2].all() and not hits[-7::2].any()   # the full box hits every block, the empty box none
+    assert 0.05 < expect[:n][small].mean() < 0.95
