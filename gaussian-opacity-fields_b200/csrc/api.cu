@@ -630,7 +630,7 @@ extern "C" int gof_integrate_prepare(const gof_scene_t* s, gof_alloc_fn geom_all
                                      void* cache_user, int* radii, int* num_rendered, void* stream) {
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
-  if (!geom_alloc || !binning_alloc || !image_alloc || !cache_alloc || !num_rendered || !radii) {
+  if (!geom_alloc || !binning_alloc || !image_alloc || !cache_alloc || !num_rendered || (!radii && s->P > 0)) {
     gof_set_error("integrate_prepare: NULL argument");
     return GOF_E_INVALID;
   }
@@ -674,4 +674,38 @@ extern "C" int gof_integrate_cached(const gof_scene_t* s, int PN, const float* p
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(c + CL.splat), reinterpret_cast<const uint32_t*>(c + CL.point_list),
                     reinterpret_cast<const uint2*>(c + CL.ranges), img, point_alloc, point_user, point_binning_alloc,
                     point_binning_user, out_color, out_alpha_integrated, out_color_integrated, nullptr, st);
+}
+
+// The multi-view opacity field's running minimum (gof_integrate_min) against a gof_integrate_prepare cache, optionally with the
+// winning view's point gradient, formed in the same pass (k_integrate<true, *, true>, DESIGN.md 4.14).
+extern "C" int gof_integrate_cached_min(const gof_scene_t* s, int PN, const float* points3D, int view, const void* cache,
+                                        int num_rendered, gof_alloc_fn image_alloc, void* image_user, gof_alloc_fn point_alloc,
+                                        void* point_user, gof_alloc_fn point_binning_alloc, void* point_binning_user, float* alpha_min,
+                                        int* argmin, float* color_min, float* grad_min, void* stream) {
+  if (!s || s->P < 0 || s->width <= 0 || s->height <= 0 || !s->viewmatrix || !s->background) {
+    gof_set_error("integrate_cached_min: scene needs P, width, height, tan_fov, viewmatrix, background");
+    return GOF_E_INVALID;
+  }
+  if (!image_alloc || !point_alloc || !point_binning_alloc) {
+    gof_set_error("integrate_cached_min: allocators must be non-NULL");
+    return GOF_E_INVALID;
+  }
+  if (view < 0 || view >= (1 << 30)) {   // 2^30 is argmin's "no view" value
+    gof_set_error("integrate_cached_min: view %d outside [0, 2^30)", view);
+    return GOF_E_INVALID;
+  }
+  if (s->P == 0 || PN <= 0) return GOF_OK;
+  if (!cache || !points3D || !alpha_min || !argmin || num_rendered < 0) {
+    gof_set_error("integrate_cached_min: NULL argument");
+    return GOF_E_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const GofView v = gof_make_view(s);
+  const GofIntCacheLayout CL = gof_int_cache_layout((size_t)s->P, s->width, s->height, (size_t)num_rendered);
+  char* img = (char*)image_alloc(image_user, gof_image_layout(s->width, s->height).bytes);
+  const char* c = (const char*)cache;
+  const GofIntMin mn{alpha_min, argmin, view, color_min, grad_min};
+  return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(c + CL.splat), reinterpret_cast<const uint32_t*>(c + CL.point_list),
+                    reinterpret_cast<const uint2*>(c + CL.ranges), img, point_alloc, point_user, point_binning_alloc,
+                    point_binning_user, nullptr, nullptr, nullptr, &mn, st);
 }

@@ -413,6 +413,7 @@ struct GofIntMin {
   int* argmin;        // [PN]
   int view;
   float* color_min;   // [PN][3] or NULL: also the winning view's colour (gof_integrate_min's color_min, DESIGN.md 4.13)
+  float* grad_min;    // [PN][3] or NULL: also the winning view's d alpha / d point (gof_integrate_cached_min, DESIGN.md 4.14)
 };
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
                          const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin, float* out_color,

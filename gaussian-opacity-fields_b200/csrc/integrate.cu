@@ -92,6 +92,10 @@ struct IntArgs : IntQuery {
   int* argmin;          // [PN]
   int view;
   float* color_min;     // [PN][3], k_integrate<true, true>: the winning view's pixel colour (DESIGN.md 4.13)
+  // k_integrate<true, *, true> (DESIGN.md 4.14): the winning view's d alpha_integrated / d point, world space
+  float* grad_min;      // [PN][3]
+  const float* points3D;
+  const float* vm;
 };
 
 constexpr int BATCH = GOF_BLOCK_SIZE;
@@ -281,12 +285,55 @@ __device__ __forceinline__ PairEval pair_eval(const float* v, float op, float rx
   return e;
 }
 
+// Walk 1's step for one pair that passed the alpha reject (k_integrate_backward, and pass 2 of k_integrate<true, *, true>): T and
+// sum_j alpha_j / (1 - alpha_j) * d power_j / d(rx, ry, depth) over the free pairs
+__device__ __forceinline__ void walk1_step(const float* v, const PairEval& e, float rx, float ry, double& T, double& grx, double& gry,
+                                           double& gdep) {
+  const double om = 1.0 - (double)e.al;
+  T *= om;
+  if (!e.free) return;
+  const double w = (double)e.al / om, t = e.t;
+  // power = -1/2 (AA t^2 + BB t + CC): AA = r^T Sigma r, BB = 2 b.r, r = (rx, ry, 1)
+  const double n0 = (double)v[0] * rx + (double)v[1] * ry + v[2];
+  const double n1 = (double)v[1] * rx + (double)v[3] * ry + v[4];
+  grx -= w * (t * t * n0 + t * v[6]);
+  gry -= w * (t * t * n1 + t * v[7]);
+  if (e.clamped) {
+    const double AA = ((double)v[0] * rx + 2.0 * v[1] * ry + 2.0 * v[2]) * rx + ((double)v[3] * ry + 2.0 * v[4]) * ry + v[5];
+    const double bh = (double)v[6] * rx + (double)v[7] * ry + v[8];
+    gdep -= w * (AA * t + bh);
+  }
+}
+
+// Walk 1's totals (T, grx, gry, gdep) of point id -> dL/dA * d A / d point in world space, rounded to float once into out[3].
+// rx = tx / (tz + 1e-7), ry = ty / (tz + 1e-7), depth = tz; (tx, ty, tz) = the view matrix applied to the point
+__device__ __forceinline__ void walk1_point_grad(const float* points3D, const float* vm_, uint32_t id, float dLdA, double T, double grx,
+                                                 double gry, double gdep, float* out) {
+  const double px = points3D[3 * (size_t)id], py = points3D[3 * (size_t)id + 1], pz = points3D[3 * (size_t)id + 2];
+  double vm[16];
+#pragma unroll
+  for (int k = 0; k < 16; ++k) vm[k] = (double)__ldg(vm_ + k);
+  const double tx = vm[0] * px + vm[4] * py + vm[8] * pz + vm[12];
+  const double ty = vm[1] * px + vm[5] * py + vm[9] * pz + vm[13];
+  const double tz = vm[2] * px + vm[6] * py + vm[10] * pz + vm[14];
+  const double s = (double)dLdA * T, den = tz + 1e-7;
+  const double drx = s * grx, dry = s * gry;
+  const double dtx = drx / den, dty = dry / den, dtz = s * gdep - (drx * tx + dry * ty) / (den * den);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) out[i] = (float)(vm[4 * i] * dtx + vm[4 * i + 1] * dty + vm[4 * i + 2] * dtz);
+}
+
+// k_integrate<true, *, true> carries walk 1's four doubles: two CTAs per SM, and a grid of that many (see the launcher)
+constexpr int INT_GRAD_CTAS_PER_SM = 2;
+
 // MIN_UPDATE: the query of one view of the multi-view opacity field (DESIGN.md 4.12).  Each point that projects folds its alpha
 // into alpha_min / argmin with the strict `<` of evaluate_alpha; views run in stream order and a point is one thread of one call,
 // so no atomics are needed.  Nothing else is written: no image, no point colour, no pixel state.  MIN_COLOR (DESIGN.md 4.13):
-// the same update also writes the point's colour of this view, C + T*bg as k_integrate<false> forms it, to color_min.
-template <bool MIN_UPDATE, bool MIN_COLOR = false>
-__global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a) {
+// the same update also writes the point's colour of this view, C + T*bg as k_integrate<false> forms it, to color_min.  MIN_GRAD
+// (DESIGN.md 4.14): pass 2 also runs walk 1 beside the float alpha, over the same pairs, and the update writes walk 1's
+// d alpha_integrated / d point (dL/dA = 1) to grad_min.
+template <bool MIN_UPDATE, bool MIN_COLOR = false, bool MIN_GRAD = false>
+__global__ void __launch_bounds__(GOF_BLOCK_SIZE, MIN_GRAD ? INT_GRAD_CTAS_PER_SM : 3) k_integrate(const IntArgs a) {
   __shared__ float4 s_rec[BATCH][5];   // 80-byte rows: GofSplat | (thr, -, -, -), see render_fwd.cu
   __shared__ uint32_t s_cnt[256];      // contributors recorded per pixel (slot = thread of that pixel)
   __shared__ float s_col[256][3];      // pixel colour (C + T*bg)
@@ -340,6 +387,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
         const uint32_t cnt = s_cnt[pslot];
         const uint16_t* ids = slab + (size_t)pslot * GOF_INT_MAX_CONTRIB;
         float point_alpha = 0.f, point_T = 1.f;
+        double T = 1.0, grx = 0.0, gry = 0.0, gdep = 0.0;   // walk 1 (MIN_GRAD)
         uint32_t prev = 0;
         for (uint32_t c = 0; c < cnt; ++c) {
           const uint32_t cid = (uint32_t)ids[c];
@@ -347,10 +395,12 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
           prev = cid;
           float v[10];
           const float op = load_rec(a.splat, a.point_list[range.x + cid - 1], v);
-          const float al = pair_eval(v, op, rx, ry, ray_depth).al;
+          const PairEval e = pair_eval(v, op, rx, ry, ray_depth);
+          const float al = e.al;
           if (al < GOF_ALPHA_MIN) continue;
           point_alpha = F_FMA(al, point_T, point_alpha);
           point_T = F_MUL(point_T, F_SUB(1.0f, al));
+          if constexpr (MIN_GRAD) walk1_step(v, e, rx, ry, T, grx, gry, gdep);
         }
         if constexpr (MIN_UPDATE) {
           if (point_alpha < a.alpha_min[id]) {   // evaluate_alpha's update, in view order
@@ -361,6 +411,7 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, 3) k_integrate(const IntArgs a
               a.color_min[3 * (size_t)id + 1] = s_col[pslot][1];
               a.color_min[3 * (size_t)id + 2] = s_col[pslot][2];
             }
+            if constexpr (MIN_GRAD) walk1_point_grad(a.points3D, a.vm, id, 1.f, T, grx, gry, gdep, a.grad_min + 3 * (size_t)id);
           }
         } else {
           a.out_alpha[id] = point_alpha;
@@ -557,37 +608,10 @@ __global__ void __launch_bounds__(GOF_BLOCK_SIZE, INT_BWD_CTAS_PER_SM)
         const float op = load_rec(a.splat, a.point_list[range.x + cid - 1], v);
         const PairEval e = pair_eval(v, op, rx, ry, ray_depth);
         if (e.al < GOF_ALPHA_MIN) continue;
-        const double om = 1.0 - (double)e.al;
-        T *= om;
-        if (!e.free) continue;
-        const double w = (double)e.al / om, t = e.t;
-        // power = -1/2 (AA t^2 + BB t + CC): AA = r^T Sigma r, BB = 2 b.r, r = (rx, ry, 1)
-        const double n0 = (double)v[0] * rx + (double)v[1] * ry + v[2];
-        const double n1 = (double)v[1] * rx + (double)v[3] * ry + v[4];
-        grx -= w * (t * t * n0 + t * v[6]);
-        gry -= w * (t * t * n1 + t * v[7]);
-        if (e.clamped) {
-          const double AA = ((double)v[0] * rx + 2.0 * v[1] * ry + 2.0 * v[2]) * rx + ((double)v[3] * ry + 2.0 * v[4]) * ry + v[5];
-          const double bh = (double)v[6] * rx + (double)v[7] * ry + v[8];
-          gdep -= w * (AA * t + bh);
-        }
+        walk1_step(v, e, rx, ry, T, grx, gry, gdep);
       }
-      if (valid && a.dL_dpoints3D != nullptr) {
-        // rx = tx / (tz + 1e-7), ry = ty / (tz + 1e-7), depth = tz; (tx, ty, tz) = the view matrix applied to the point
-        const double px = a.points3D[3 * (size_t)id], py = a.points3D[3 * (size_t)id + 1], pz = a.points3D[3 * (size_t)id + 2];
-        double vm[16];
-#pragma unroll
-        for (int k = 0; k < 16; ++k) vm[k] = (double)__ldg(a.vm + k);
-        const double tx = vm[0] * px + vm[4] * py + vm[8] * pz + vm[12];
-        const double ty = vm[1] * px + vm[5] * py + vm[9] * pz + vm[13];
-        const double tz = vm[2] * px + vm[6] * py + vm[10] * pz + vm[14];
-        const double s = (double)dLdA * T, den = tz + 1e-7;
-        const double drx = s * grx, dry = s * gry;
-        const double dtx = drx / den, dty = dry / den, dtz = s * gdep - (drx * tx + dry * ty) / (den * den);
-#pragma unroll
-        for (int i = 0; i < 3; ++i)
-          a.dL_dpoints3D[3 * (size_t)id + i] = (float)(vm[4 * i] * dtx + vm[4 * i + 1] * dty + vm[4 * i + 2] * dtz);
-      }
+      if (valid && a.dL_dpoints3D != nullptr)
+        walk1_point_grad(a.points3D, a.vm, id, dLdA, T, grx, gry, gdep, a.dL_dpoints3D + 3 * (size_t)id);
 
       // walk 2: pair j of the point adds dL/dA * T / (1 - alpha_j) * alpha_j * d power_j / d view2gaussian to Gaussian j.  Lanes of
       // one pixel (neighbours: the points are sorted by pixel) walk the same list in step, so each run of them sums its rows with
@@ -723,7 +747,14 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
   a.out_color = out_color; a.out_alpha = out_alpha; a.out_color_int = out_color_int;
   if (mn) {
     a.alpha_min = mn->alpha_min; a.argmin = mn->argmin; a.view = mn->view; a.color_min = mn->color_min;
-    if (mn->color_min)
+    a.grad_min = mn->grad_min; a.points3D = points3D; a.vm = s->viewmatrix;
+    // persistent CTAs stride over the tiles, each with the slab of its blockIdx.x (PBL.nblk slabs exist)
+    const int grad_grid = std::min(PBL.nblk, INT_GRAD_CTAS_PER_SM * gof_sm_count());
+    if (mn->grad_min && mn->color_min)
+      GOF_LAUNCH("integrate_min_color_grad", st, k_integrate<true, true, true><<<grad_grid, GOF_BLOCK_SIZE, 0, st>>>(a));
+    else if (mn->grad_min)
+      GOF_LAUNCH("integrate_min_grad", st, k_integrate<true, false, true><<<grad_grid, GOF_BLOCK_SIZE, 0, st>>>(a));
+    else if (mn->color_min)
       GOF_LAUNCH("integrate_min_color", st, k_integrate<true, true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
     else
       GOF_LAUNCH("integrate_min", st, k_integrate<true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));

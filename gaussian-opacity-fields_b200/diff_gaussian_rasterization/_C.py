@@ -614,6 +614,42 @@ def integrate_points_cached(cache, background, points3D, viewmatrix, tan_fovx, t
     return out_color, alpha_int, color_int
 
 
+_lib.gof_integrate_cached_min.restype = ctypes.c_int
+_lib.gof_integrate_cached_min.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int, _fp, ctypes.c_int] + \
+    [_ALLOC_FN, ctypes.c_void_p] * 3 + [_fp, _fp, _fp, _fp, ctypes.c_void_p]
+
+
+def integrate_points_cached_min(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, view, alpha_min, argmin,
+                                color_min=None, grad_min=None, debug=False):
+    """gof_integrate_cached_min (extension, DESIGN.md 4.14): integrate_points_cached for view index `view`, folded into the
+    running minimum over views in place, as integrate_gaussians_to_points_min folds it (alpha_min float32 [PN] from 1, argmin
+    int32 [PN] from 2^30, color_min float32 [PN,3] or None).  With grad_min (float32 [PN,3]) the same update also stores the
+    winning view's d alpha_integrated / d point in world space; points that no view updates keep what the caller put there."""
+    if points3D.ndimension() != 2 or points3D.size(1) != 3:
+        raise RuntimeError("points3D must have dimensions (num_points, 3)")
+    PN = points3D.size(0)
+    checks = [("alpha_min", alpha_min, torch.float32, (PN,)), ("argmin", argmin, torch.int32, (PN,))]
+    for name, t in (("color_min", color_min), ("grad_min", grad_min)):
+        if t is not None:
+            checks.append((name, t, torch.float32, (PN, 3)))
+    for name, t, dt, shape in checks:
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape {shape}")
+    dev = cache.buffer.device
+    s = _Scene()
+    s.P, s.width, s.height = cache.P, cache.W, cache.H
+    s.tan_fovx, s.tan_fovy = _scalar(tan_fovx), _scalar(tan_fovy)
+    bg, vm, p3 = _c(background), _c(viewmatrix), _c(points3D)
+    s.background, s.viewmatrix, s.debug = _ptr(bg, device=dev), _ptr(vm, device=dev), int(bool(debug))
+    if cache.P != 0 and PN != 0:
+        img, pts, pbin = _Scratch(dev, "image"), _Scratch(dev, "points"), _Scratch(dev, "point_binning")
+        with torch.cuda.device(dev):
+            _check(_lib.gof_integrate_cached_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), cache.buffer.data_ptr(),
+                                                 cache.num_rendered, img.cb, None, pts.cb, None, pbin.cb, None,
+                                                 _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev),
+                                                 _ptr(color_min, device=dev), _ptr(grad_min, device=dev), _stream()))
+
+
 def export_state(P, W, H, num_rendered, geomBuffer, binningBuffer, imgBuffer, radii, masks=False):
     """Parity-test helper (gof_export_state): this library's scratch buffers in the reference's field layout.  masks=True
     (buffers of a forward only) adds "blend_masks", int32 [8, num_rendered + 32 * tiles]: the masks the forward leaves for the

@@ -13,6 +13,8 @@ reference's extract_mesh.py, restated with view sharding over the GPUs of one bo
                        gof_tetmesh.marching_tetrahedra.
 * make_integrate_fn == gaussian_renderer.integrate (gaussian_renderer/__init__.py:118-218) for plain tensors.
 * CachedIntegrator  -- the same, with the Gaussian side of every view prepared once and reused by all passes (SURVEY 8(f) rank 3).
+* field_gradient    -- evaluate_alpha over a CachedIntegrator together with the field's point gradient, formed in the query's
+                       own pass (DESIGN §4.14); extract_level_set(return_normals=True) turns it into vertex normals.
 * marching_tetrahedra_sharded / merge_tet_shards -- utils/tetmesh.py's chunk loop (:55-95) spread over ranks (SURVEY 8(e)).
 * extract_level_set -- marching_tetrahedra_with_binary_search (extract_mesh.py:37-120) up to the mesh arrays.
 * get_tetra_points  == GaussianModel.get_tetra_points (scene/gaussian_model.py:433-463), get_frustum_mask == its module-level
@@ -282,12 +284,56 @@ class CachedIntegrator:
                                                                                 rs.debug)
         return alpha_integrated, color_integrated
 
+    def min_update(self, points, view, vi, alpha_min, argmin, color_min=None, grad_min=None):
+        """Folds view `view` (index vi) into the running minimum over views in place (_C.integrate_points_cached_min)."""
+        from diff_gaussian_rasterization import _C
+        _view, rs, c = self.prepare(view)
+        _C.integrate_points_cached_min(c, rs.bg, points, rs.viewmatrix, rs.tanfovx, rs.tanfovy, vi, alpha_min, argmin,
+                                       color_min=color_min, grad_min=grad_min, debug=rs.debug)
+
     @property
     def cached_bytes(self):
         return sum(c.nbytes for _v, _rs, c in self._cache.values())
 
     def clear(self):
         self._cache.clear()
+
+
+@torch.no_grad()
+def field_gradient(points, views, integrate_fn, return_color=False, group=None):
+    """evaluate_alpha's field and its gradient with respect to the points, in one pass over the cached views (DESIGN.md 4.14).
+    integrate_fn must be a CachedIntegrator.  Returns (alpha [N], grad [N,3]) or, with return_color, (alpha, grad, colour [N,3]):
+    alpha and colour are evaluate_alpha(points, views, integrate_fn, return_color=...)'s, bit for bit; grad is d alpha / d point
+    through the winning view (the lowest view index on a tie), the points.grad that opacity_field(points, ...).sum().backward()
+    leaves, bit for bit.  A point that no view lowers below 1 gets zeros.  With torch.distributed initialised each rank folds
+    views[rank::world], and the ranks merge as evaluate_alpha does; the winner's rank contributes the gradient and colour rows."""
+    if not isinstance(integrate_fn, CachedIntegrator):
+        raise TypeError(f"field_gradient: integrate_fn must be a CachedIntegrator, got {type(integrate_fn).__name__}")
+    rank, world = _world(group)
+    n, dev = points.shape[0], points.device
+    alpha_min = torch.ones(n, dtype=torch.float32, device=dev)
+    argmin = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev)
+    grad_min = torch.zeros(n, 3, dtype=torch.float32, device=dev)
+    color = torch.ones(n, 3, dtype=torch.float32, device=dev) if return_color else None
+    views = list(views)
+    for vi in range(rank, len(views), world):
+        integrate_fn.min_update(points, views[vi], vi, alpha_min, argmin, color_min=color, grad_min=grad_min)
+    if world > 1:
+        local = alpha_min.clone()
+        dist.all_reduce(alpha_min, op=dist.ReduceOp.MIN, group=group)
+        cand = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
+        argmin = cand.clone()
+        dist.all_reduce(argmin, op=dist.ReduceOp.MIN, group=group)
+        won = argmin < _NO_VIEW
+        # the winner's gradient and colour rows in one [N,6] block, summed in a single all-reduce
+        rows = torch.cat([grad_min, color], 1) if return_color else grad_min
+        rows = torch.where(((cand == argmin) & won).reshape(-1, 1), rows, torch.zeros_like(rows))
+        dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=group)
+        grad_min = rows[:, :3]
+        if return_color:
+            color = torch.where(won.reshape(-1, 1), rows[:, 3:], torch.ones_like(color))
+    alpha, grad = 1 - alpha_min, -grad_min
+    return (alpha, grad, color.contiguous()) if return_color else (alpha, grad.contiguous())
 
 
 # ---- marching tetrahedra sharded by tet chunk (SURVEY 8(e); utils/tetmesh.py:55-95 is the single-GPU chunk loop) ---------
@@ -379,11 +425,14 @@ def marching_tetrahedra_sharded(vertices, tets, sdf, scales, group=None, chunk_t
 
 @torch.no_grad()
 def extract_level_set(points, points_scale, tets, views, integrate_fn, n_binary_steps=8, group=None, chunk_tets=None,
-                      return_color=False, timings=None):
+                      return_color=False, timings=None, return_normals=False):
     """marching_tetrahedra_with_binary_search (extract_mesh.py:37-120) up to the mesh arrays: opacity field on the tetrahedra
     vertices (view-sharded evaluate_alpha), marching tetrahedra on alpha - 0.5 (tet-chunk sharded), `n_binary_steps`
     bisection steps of every crossing edge, optional vertex colours and the reference's `distance <= scale` vertex mask.
-    Returns dict(vertices (E,3), faces (F,3) int64, mask (E,) bool, colors (E,3) or None)."""
+    Returns dict(vertices (E,3), faces (F,3) int64, mask (E,) bool, colors (E,3) or None).
+    return_normals=True (integrate_fn a CachedIntegrator) also returns "normals" (E,3): the field's outward unit normal at each
+    vertex, grad alpha / |grad alpha| = -grad o / |grad o| for the opacity o = 1 - alpha, (0, 0, 0) where the gradient is zero,
+    from one field_gradient pass that also gives the colours (DESIGN.md 4.14)."""
     import time as _time
 
     def tick(name, t0):
@@ -404,6 +453,15 @@ def extract_level_set(points, points_scale, tets, views, integrate_fn, n_binary_
     verts = binary_search(end_points, end_sdf, lambda p: evaluate_alpha(p, views, integrate_fn, group=group), n_steps=n_binary_steps)
     tick("binary_search_s", t0)
     colors = None
+    if return_normals:
+        t0 = _time.perf_counter()
+        _a, grad, *rest = field_gradient(verts, views, integrate_fn, return_color=return_color, group=group)
+        colors = rest[0] if return_color else None
+        norm = grad.norm(dim=1, keepdim=True)
+        # alpha = 1 - (the opacity min_v alpha_integrated) rises from ~0 inside the surface to ~1 outside it, so grad alpha points out
+        normals = torch.where(norm > 0, grad / torch.where(norm > 0, norm, torch.ones_like(norm)), torch.zeros_like(grad))
+        tick("field_gradient_s", t0)
+        return {"vertices": verts, "faces": faces, "mask": distance <= scale, "colors": colors, "normals": normals}
     if return_color:
         t0 = _time.perf_counter()
         _a, colors = evaluate_alpha(verts, views, integrate_fn, return_color=True, group=group)

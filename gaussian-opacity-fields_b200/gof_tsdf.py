@@ -242,21 +242,29 @@ def tsdf_fusion(views, render_fn, alpha_thres=0.5, voxel_size=0.002, depth_max=6
 
 
 def write_ply(path, mesh):
-    """Binary little-endian PLY: float x y z, uchar red green blue (colour * 255 clipped to [0, 255] and truncated), int32
-    vertex_indices lists -- what evaluate_dtu_mesh.py loads."""
+    """Binary little-endian PLY: float x y z, then float nx ny nz when the mesh has "normals" (not None), uchar red green blue
+    (colour * 255 clipped to [0, 255] and truncated), int32 vertex_indices lists -- what evaluate_dtu_mesh.py loads."""
     v = np.ascontiguousarray(torch.as_tensor(mesh["vertices"]).detach().cpu().numpy(), np.float32)
     f = np.ascontiguousarray(torch.as_tensor(mesh["faces"]).detach().cpu().numpy()).astype(np.int32)
     c = torch.as_tensor(mesh["colors"]).detach().cpu().numpy().astype(np.float32)
     rgb = np.clip(c * np.float32(255.0), 0, 255).astype(np.uint8)
-    vert = np.empty(v.shape[0], dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1")])
+    normals = mesh.get("normals")
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if normals is not None:
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+    vert = np.empty(v.shape[0], dtype=fields + [("red", "u1"), ("green", "u1"), ("blue", "u1")])
     vert["x"], vert["y"], vert["z"] = v[:, 0], v[:, 1], v[:, 2]
+    if normals is not None:
+        n = torch.as_tensor(normals).detach().cpu().numpy().astype(np.float32)
+        vert["nx"], vert["ny"], vert["nz"] = n[:, 0], n[:, 1], n[:, 2]
     vert["red"], vert["green"], vert["blue"] = rgb[:, 0], rgb[:, 1], rgb[:, 2]
     face = np.empty(f.shape[0], dtype=[("n", "u1"), ("i", "<i4", (3,))])
     face["n"] = 3
     face["i"] = f
     header = ("ply\nformat binary_little_endian 1.0\n"
               f"element vertex {v.shape[0]}\nproperty float x\nproperty float y\nproperty float z\n"
-              "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+              + ("property float nx\nproperty float ny\nproperty float nz\n" if normals is not None else "")
+              + "property uchar red\nproperty uchar green\nproperty uchar blue\n"
               f"element face {f.shape[0]}\nproperty list uchar int vertex_indices\nend_header\n")
     with open(path, "wb") as fh:
         fh.write(header.encode("ascii"))
@@ -265,19 +273,27 @@ def write_ply(path, mesh):
 
 
 def read_ply(path):
-    """Reads back what write_ply writes: dict(vertices [V,3] float32, colors_u8 [V,3] uint8, faces [F,3] int64)."""
+    """Reads back what write_ply writes: dict(vertices [V,3] float32, colors_u8 [V,3] uint8, faces [F,3] int64), and
+    normals [V,3] float32 when the header declares nx ny nz."""
     with open(path, "rb") as fh:
         data = fh.read()
     end = data.index(b"end_header\n") + len(b"end_header\n")
     lines = data[:end].decode("ascii").splitlines()
     nv = int(next(ln for ln in lines if ln.startswith("element vertex")).split()[-1])
     nf = int(next(ln for ln in lines if ln.startswith("element face")).split()[-1])
-    vdt = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1")])
+    has_normals = "property float nx" in lines
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if has_normals:
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+    vdt = np.dtype(fields + [("red", "u1"), ("green", "u1"), ("blue", "u1")])
     fdt = np.dtype([("n", "u1"), ("i", "<i4", (3,))])
     vert = np.frombuffer(data, vdt, nv, end)
     face = np.frombuffer(data, fdt, nf, end + nv * vdt.itemsize)
     if nf and not np.all(face["n"] == 3):
         raise ValueError("read_ply: only triangles are supported")
-    return {"vertices": np.stack([vert["x"], vert["y"], vert["z"]], 1),
-            "colors_u8": np.stack([vert["red"], vert["green"], vert["blue"]], 1),
-            "faces": face["i"].astype(np.int64).reshape(-1, 3)}
+    out = {"vertices": np.stack([vert["x"], vert["y"], vert["z"]], 1),
+           "colors_u8": np.stack([vert["red"], vert["green"], vert["blue"]], 1),
+           "faces": face["i"].astype(np.int64).reshape(-1, 3)}
+    if has_normals:
+        out["normals"] = np.stack([vert["nx"], vert["ny"], vert["nz"]], 1)
+    return out

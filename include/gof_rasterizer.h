@@ -246,7 +246,8 @@ GOF_API int gof_integrate_backward(const gof_scene_t* scene, int PN, const float
  * emission / tile sort of the Gaussians (rasterizer_impl.cu:566-660) are identical in every pass.
  *   gof_integrate_prepare: runs them once; `cache_alloc` is called once with gof_integrate_cache_bytes(P, W, H, *num_rendered)
  *                          and receives records, tile ranges and per-tile lists (64 B/Gaussian + 4 B/instance + 8 B/tile);
- *                          geom / binning / image buffers are scratch that may be released after the call; radii [P] out.
+ *                          geom / binning / image buffers are scratch that may be released after the call; radii [P] out
+ *                          (may be NULL when P == 0: a cache of no Gaussians).
  *   gof_integrate_cached:  the point side alone (rasterizer_impl.cu:662-792) against such a cache; of `scene` only P, width,
  *                          height, tan_fovx/y, viewmatrix, background and debug are read.  Outputs as gof_integrate. */
 GOF_API size_t gof_integrate_cache_bytes(int P, int width, int height, int num_rendered);
@@ -257,6 +258,19 @@ GOF_API int gof_integrate_cached(const gof_scene_t* scene, int PN, const float* 
                   gof_alloc_fn image_alloc, void* image_user, gof_alloc_fn point_alloc, void* point_user,
                   gof_alloc_fn point_binning_alloc, void* point_binning_user, float* out_color,
                   float* out_alpha_integrated, float* out_color_integrated, void* stream);
+
+/* gof_integrate_min against a gof_integrate_prepare cache (no reference counterpart; DESIGN section 4.14): the point side of
+ * `view` folded into alpha_min [PN] / argmin [PN] / color_min [PN,3] (NULL: alpha only) exactly as gof_integrate_min folds it,
+ * with the scene fields and the allocators of gof_integrate_cached.  grad_min [PN,3] (NULL: not formed) also keeps the winning
+ * view's gradient: whenever a view updates alpha_min[k], grad_min[k] takes d alpha_integrated / d point of that view in world
+ * space, with the point's contributor list, rejects and clamps held fixed -- formed per point in double in the same pass,
+ * rounded to float once, no atomics: the dL_dpoints3D of gof_integrate_backward for dL_dalpha = 1, bit for bit.  grad_min is
+ * initialised by the caller; points that no view updates keep that value.  A view outside [0, 2^30) fails with GOF_E_INVALID;
+ * with P == 0 or PN <= 0 nothing is written. */
+GOF_API int gof_integrate_cached_min(const gof_scene_t* scene, int PN, const float* points3D, int view, const void* cache,
+                  int num_rendered, gof_alloc_fn image_alloc, void* image_user, gof_alloc_fn point_alloc, void* point_user,
+                  gof_alloc_fn point_binning_alloc, void* point_binning_user, float* alpha_min, int* argmin, float* color_min,
+                  float* grad_min, void* stream);
 
 /* Rasterizer::markVisible (rasterizer_impl.cu:174-186) == _C.mark_visible.  present: [P] bytes (bool). */
 GOF_API int gof_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
