@@ -1,16 +1,27 @@
 """GPU: the focal-length gradient of the backward (gof_backward_out_t.dL_dtan_fov, DESIGN.md 4.10).
 
 (a) Every pixel's dL/drx, dL/dry (the [2,H,W] map the call leaves in its scratch) against the float64 oracle
-    (tests/focal_oracle/focal_oracle.c) run from this library's own forward state with the same dL_dpix:
+    (tests/focal_oracle/focal_oracle.c) run from this library's own forward state with the same dL_dpix, over every scene of
+    tests/_view_grad_scenes.py, from a call that also asks for the pose (the joint scratch layout):
 
-        |gpu - oracle|  <=  c * 2^-24 * (1 + L) * mag  +  marginal,      L = the view's longest walk, c = C_RAYS,
+        |gpu - oracle|  <=  (C_PAIR + C_RAYS (1 + L)) * 2^-24 * mag  +  marginal,      L = the view's longest walk,
 
     the model of tests/_grad_bounds.py: T is recovered pair by pair on the GPU, which drifts by about one ulp per pair, and a
-    pair near a blend threshold exempts every pair in front of it.  Both sums against the oracle's within the sum over the
-    pixels of |rx| (|ry|) times the pixel's allowance, over tan_fov, plus half an ulp of the float result.  Observed on an
-    H100 80GB HBM3 (700 W power limit): largest per-pixel ratio 0.0017 (c2_v3, L = 816) and 0.0055 (ragged_4097, L = 245);
-    largest summed error / allowance 1.7e-6 and 3.1e-4.  The per-pixel values go through no atomics, so these are the same
-    on every run.
+    pair near a blend threshold exempts every pair in front of it; at most SHARE_MARGINAL of the pixels may carry marginal
+    mass.  C_PAIR is the part that does not grow with the walk: each pair's dL/dr is a five-term float FMA chain of the float
+    dA, dB2 and dnrm, about one ulp of its magnitude.  At walks of hundreds of pairs C_RAYS (1 + L) covers it; at walks of
+    1-35 pairs (the scenes with P <= 129) it did not (need 0.92 at plain_33, L = 3).  Both sums against the oracle's within
+    the sum over the pixels of |rx| (|ry|) times the pixel's allowance, over tan_fov, plus half an ulp; and, because that
+    allowance is loose (a sum that missed half its tiles passed it at C2), against the float64 sum of the call's own ray map
+    within half an ulp + 2^-46 of the sum of |rx dL/drx|: the tile sums and k_focal_grad_sum add in double and round once.
+    Observed on an H100 80GB HBM3 (700 W power limit), largest |gpu - oracle - marginal| / (2^-24 (1 + L) mag), share of
+    pixels with marginal mass:
+      sh_deg0..3 (L 319-357) 0.003-0.005, 0;  c1 0.008, 1.5e-5;  precomp_bg_mip 0.005, 4.2e-5;  screen_filling 0.024, 0;
+      camera_inside / near_plane 0.003 / 0.004, 0;  stacked_* (L 888-1019) 0.001, 0;  c2_v3 0.0017, 1.3e-5;
+      c3_v5 0.0015, 2.7e-5;  plain_4097 0.010, 0;  saturation 0.009, 0;  threshold 0.010, 1.6e-4;  rows_8192..8321 <= 5e-4, 0;
+      image_* 0.0013-0.017, <= 1.5e-5;  ragged_4097 0.0055, 0;  and C_PAIR needed at the short walks: plain_1 / 33 0.52 /
+      0.92, rows_1 / 127 / 128 / 129 0.42 / 0.61 / <= 0.45.  Sums: largest error / oracle allowance 3e-4, largest error /
+      own-sum bound 0.996 (the float rounding itself).  The per-pixel values go through no atomics: the same on every run.
 (b) Two calls give identical bits; every other output, the pose gradient included, is bit-identical with and without the
     intrinsics outputs wherever the blend's outputs are identical (the blend backward sums with double atomics, see
     test_gpu_camera_grad (b)).
@@ -19,7 +30,9 @@
     markVisible accept tensor tan_fov values.
 (d) Descent: Adam on the field of view recovers a perturbed focal length against the unperturbed render, alone and together
     with a pose perturbation.  Reached on an H100 80GB HBM3 (700 W power limit): largest relative field-of-view error
-    0.040 -> 0.00003 alone, 0.040 -> 0.0071 together with the pose."""
+    0.040 -> 0.00003 alone, 0.040 -> 0.0071 together with the pose.
+(e) The caller's scratch, through gof_rasterize_backward_ex directly: a guard band after exactly the size the library asks
+    for stays intact, and outputs do not depend on the scratch's or the outputs' previous contents."""
 import math
 
 import numpy as np
@@ -29,24 +42,21 @@ import torch
 import _focal_oracle as fo
 import _grad_bounds as gb
 import _util
+import _view_grad_scenes as vs
 import gof_synth
 
 pytestmark = pytest.mark.gpu
 
 C_RAYS = 2.0 ** -5   # 4x the largest ratio observed (0.0055, ragged_4097), rounded up to a power of two
+C_PAIR = 4.0         # 4x the largest need observed at short walks (0.92, plain_33, L = 3), rounded up to a power of two
+SHARE_MARGINAL = 0.01   # at most this share of the pixels may carry marginal mass (as test_gpu_forward_edges)
 NAMES = ("dmeans2D", "dcolors", "dopacity", "dmeans3D", "dcov3D", "dsh", "dscales", "drot", "dv2g")
 BLEND = ("dmeans2D", "dcolors", "dopacity", "dv2g")
 
-SCENES = {
-    "c2_v3": (lambda: gof_synth.make_scene("C2", view=3), (0.0, 0.0, 0.0)),
-    # P not a multiple of the 128-Gaussian CTA, odd image size, a background
-    "ragged_4097": (lambda: gof_synth.make_scene(dict(P=4097, width=203, height=117, seed=17), view=4), (0.3, 0.6, 0.9)),
-}
 
-
-def _forward(cam, gs, bg=(0.0, 0.0, 0.0)):
+def _forward(cam, gs, **kw):
     from diff_gaussian_rasterization import _C
-    fa = _util.fwd_args(cam, gs, torch.device("cuda"), bg=bg)
+    fa = _util.fwd_args(cam, gs, torch.device("cuda"), **kw)
     R, _color, radii, geom, binning, img = _C.rasterize_gaussians(*fa)
     return fa, R, radii, geom, binning, img
 
@@ -64,35 +74,48 @@ def _ulp(x):
     return np.spacing(np.abs(np.float32(x))).astype(np.float64)
 
 
-@pytest.mark.parametrize("name", list(SCENES))
+@pytest.mark.parametrize("name", list(vs.SCENES))
 def test_ray_gradient_against_the_fp64_oracle(name):
     from diff_gaussian_rasterization import _C
-    make, bg = SCENES[name]
-    cam, gs = make()
+    cam, gs, kw = vs.inputs(name)
     P, W, H = gs["means3D"].shape[0], cam.image_width, cam.image_height
-    fwd = _forward(cam, gs, bg)
+    fwd = _forward(cam, gs, **kw)
     st = {k: v.cpu().numpy() for k, v in _C.export_state(P, W, H, fwd[1], fwd[3], fwd[4], fwd[5], fwd[2]).items()}
     dL = torch.randn(9, H, W, generator=torch.Generator().manual_seed(41))
-    g = _backward(fwd, dL.cuda(), intrinsics=True, ray_map=True)
-    gx, gy, rays = float(g[9]), float(g[10]), g[11].cpu().numpy()
-    d = fo.rays(W, H, cam.tanfovx, cam.tanfovy, st, np.asarray(bg, np.float32), dL.numpy(), float_geometry=True)
+    g = _backward(fwd, dL.cuda(), camera=True, intrinsics=True, ray_map=True)   # the pose outputs too: the joint scratch layout
+    gx, gy, rays = float(g[11]), float(g[12]), g[13].cpu().numpy()
+    d = fo.rays(W, H, cam.tanfovx, cam.tanfovy, st, np.asarray(kw["bg"], np.float32), dL.numpy(), float_geometry=True)
     L = int(st["n_contrib"][0].max())
-    allow = C_RAYS * gb.EPS * (1.0 + L) * d["mag"] + d["marginal"]
+    allow = (C_PAIR + C_RAYS * (1.0 + L)) * gb.EPS * d["mag"] + d["marginal"]
     err = np.abs(rays - d["drays"])
     with np.errstate(divide="ignore", invalid="ignore"):
         ratio = np.where(err > 0, np.maximum(err - d["marginal"], 0.0) / (gb.EPS * (1.0 + L) * d["mag"]), 0.0)
+        need = np.where(err > 0, np.maximum(err - d["marginal"] - C_RAYS * gb.EPS * (1.0 + L) * d["mag"], 0.0) / (gb.EPS * d["mag"]), 0.0)
+    share = float((d["marginal"].sum(axis=0) > 0).mean())
     print(f"{name}: L = {L}, largest per-pixel |gpu - oracle - marginal| / (2^-24 (1 + L) mag) = {float(ratio.max()):.3g}, "
-          f"pixels with marginal mass {float((d['marginal'].sum(axis=0) > 0).mean()):.2e}")
-    assert (err <= allow).all(), (float(ratio.max()), np.unravel_index(np.argmax(ratio), ratio.shape))
+          f"C_PAIR needed {float(need.max()):.3g}, pixels with marginal mass {share:.2e}")
+    assert (err <= allow).all(), (float(need.max()), np.unravel_index(np.argmax(need), need.shape))
+    assert share <= SHARE_MARGINAL, share
     assert np.abs(d["drays"]).max() > 0
     # the sums
     rx, ry = fo.pixel_rays(W, H, cam.tanfovx, cam.tanfovy)
     ox, oy = fo.tan_fov_grad(d["drays"], cam.tanfovx, cam.tanfovy)
     ax = float((np.abs(rx.astype(np.float64))[None, :] * allow[0]).sum()) / float(np.float32(cam.tanfovx))
     ay = float((np.abs(ry.astype(np.float64))[:, None] * allow[1]).sum()) / float(np.float32(cam.tanfovy))
-    for what, got, ora, a in (("tanfovx", gx, ox, ax), ("tanfovy", gy, oy, ay)):
+    # the reduction alone: the fp64 sums of this call's own ray map, which k_render_backward<true>'s tile sums and
+    # k_focal_grad_sum add in double (at most ~30 levels of double rounding) and round to float once
+    tx, ty = float(np.float32(cam.tanfovx)), float(np.float32(cam.tanfovy))
+    wx, wy = rx.astype(np.float64)[None, :] * rays[0], ry.astype(np.float64)[:, None] * rays[1]
+    for what, got, ora, a, n, w, tan in (("tanfovx", gx, ox, ax, W, wx, tx), ("tanfovy", gy, oy, ay, H, wy, ty)):
         bound = a + 0.5 * _ulp(ora)
-        print(f"{name} {what}: gpu {got:.9g} oracle {ora:.9g}, |gpu - oracle| / allowance = {abs(got - ora) / bound:.3g}")
+        own = float(w.sum()) / tan
+        tight = 0.5 * _ulp(max(abs(own), abs(got))) + 2.0 ** -46 * float(np.abs(w).sum()) / tan
+        print(f"{name} {what}: gpu {got:.9g} oracle {ora:.9g}, |gpu - oracle| / allowance = {abs(got - ora) / bound:.3g}, "
+              f"|gpu - sum of its ray map| / (half an ulp + 2^-46 sum|r dL/dr|) = {abs(got - own) / tight if tight else 0.0:.3g}")
+        if n == 1:   # the one pixel's ray is the optical axis: rx = 0 (ry = 0), and so is the sum
+            assert got == 0.0 and ora == 0.0, (what, got, ora)
+            continue
+        assert abs(got - own) <= tight, (what, got, own, tight)
         assert abs(got - ora) <= bound, (what, got, ora, bound)
         assert ora != 0.0
 
@@ -101,11 +124,19 @@ def _bits(a):
     return a.contiguous().view(torch.int32)
 
 
-@pytest.mark.parametrize("name", list(SCENES))
+def _same_blend(x, y, P):
+    """[P] bool: every blend-stage output of the Gaussian is bitwise equal in the gradient lists x and y."""
+    m = torch.ones(P, dtype=torch.bool, device=x[0].device)
+    for n in BLEND:
+        i = NAMES.index(n)
+        m &= (_bits(x[i]).view(P, -1) == _bits(y[i]).view(P, -1)).all(dim=1)
+    return m
+
+
+@pytest.mark.parametrize("name", list(vs.SCENES))
 def test_reproducible_and_other_outputs_unchanged(name):
-    make, bg = SCENES[name]
-    cam, gs = make()
-    fwd = _forward(cam, gs, bg)
+    cam, gs, kw = vs.inputs(name)
+    fwd = _forward(cam, gs, **kw)
     dL = torch.randn(9, cam.image_height, cam.image_width, generator=torch.Generator().manual_seed(5)).cuda()
     plain = _backward(fwd, dL, camera=True)
     both = _backward(fwd, dL, camera=True, intrinsics=True, ray_map=True)
@@ -118,16 +149,8 @@ def test_reproducible_and_other_outputs_unchanged(name):
         assert torch.equal(_bits(both[i]), _bits(again[i])) and torch.equal(_bits(both[i]), _bits(fov_only[9 + i - 11]))
     P = gs["means3D"].shape[0]
     vis = fwd[2] > 0
-
-    def same_blend(x, y):   # [P] bool: every blend-stage output of the Gaussian is bitwise equal in x and y
-        m = torch.ones(P, dtype=torch.bool, device=vis.device)
-        for n in BLEND:
-            i = NAMES.index(n)
-            m &= (_bits(x[i]).view(P, -1) == _bits(y[i]).view(P, -1)).all(dim=1)
-        return m
-
     for other in (both, fov_only):
-        same = same_blend(plain, other)
+        same = _same_blend(plain, other, P)
         assert float((~same & vis).sum()) <= 1e-3 * float(vis.sum())
         for i, n in enumerate(NAMES):
             a, b = plain[i], other[i]
@@ -135,11 +158,99 @@ def test_reproducible_and_other_outputs_unchanged(name):
                 assert _util.same_up_to_summation_order(b, a), n
             elif a.numel():
                 assert torch.equal(_bits(a).view(P, -1)[same], _bits(b).view(P, -1)[same]), n
-    if bool(same_blend(plain, both).all()):
+    if bool(_same_blend(plain, both, P).all()):
         assert torch.equal(_bits(plain[9]), _bits(both[9])) and torch.equal(_bits(plain[10]), _bits(both[10]))
     else:
         for i in (9, 10):
             assert _util.same_up_to_summation_order(both[i], plain[i])
+
+
+# ---- the caller's scratch ----------------------------------------------------------------------------------------------
+
+GUARD = 64 * 1024
+
+
+def _backward_ex(fwd, dL, camera, intrinsics, fill):
+    """gof_rasterize_backward_ex called directly, with every output and a scratch of exactly
+    gof_rasterize_backward_scratch_bytes(P, W, H, camera, intrinsics) bytes followed by a GUARD-byte band, all pre-filled with
+    the byte `fill`.  Returns (the nine gradients, the camera [19] or None, the focal sums [2] or None, the ray map [2,H,W] or
+    None, the scratch buffer, its size)."""
+    import ctypes
+    from diff_gaussian_rasterization import _C
+    fa, R, radii, geom, binning, img = fwd
+    (bg, means3D, colors, _opacity, scales, rotations, sm, cov3D, v2g, vm, pm, tfx, tfy, ks, subpix, H, W, sh, deg, campos,
+     _prefiltered, _debug) = fa
+    keep = []
+    s = _C._scene(keep, bg, means3D, colors, means3D, scales, rotations, sm, cov3D, v2g, vm, pm, tfx, tfy, ks, subpix, H, W, sh, deg,
+                  campos, False, False)
+    P, M, dev = means3D.shape[0], s.M, means3D.device
+    filled = lambda n, dt=torch.float32: torch.full((n,), fill, dtype=torch.uint8, device=dev).view(dt)   # noqa: E731
+    grads = [filled(4 * P * k) for k in (3, 3, 1, 3, 6, 3 * M, 3, 4, 10)]
+    cam, fov = filled(4 * 19), filled(4 * 2)
+    need = int(_C._lib.gof_rasterize_backward_scratch_bytes(P, W, H, int(camera), int(intrinsics)))
+    scratch = filled(need + GUARD, torch.uint8)
+    o = _C._BackwardOut(dL_dmean2D=grads[0].data_ptr(), dL_dcolor=grads[1].data_ptr(), dL_dopacity=grads[2].data_ptr(),
+                        dL_dmean3D=grads[3].data_ptr(), dL_dcov3D=grads[4].data_ptr(), dL_dsh=grads[5].data_ptr() if M else None,
+                        dL_dscale=grads[6].data_ptr(), dL_drot=grads[7].data_ptr(), dL_dview2gaussian=grads[8].data_ptr(),
+                        dL_dviewmatrix=cam.data_ptr() if camera else None, dL_dcampos=cam.data_ptr() + 64 if camera else None,
+                        dL_dtan_fov=fov.data_ptr() if intrinsics else None, scratch=scratch.data_ptr(), scratch_bytes=need)
+    g = dL.contiguous()
+    _C._check(_C._lib.gof_rasterize_backward_ex(ctypes.byref(s), int(R), radii.data_ptr(), geom.data_ptr(),
+                                                 binning.data_ptr() if binning.numel() else None, img.data_ptr(), g.data_ptr(),
+                                                 ctypes.byref(o), _C._stream()))
+    torch.cuda.synchronize()
+    rays = None
+    if intrinsics:
+        off = need - 16 * (W * H + ((W + 15) // 16) * ((H + 15) // 16))
+        rays = scratch[off:off + 16 * W * H].view(torch.float64).view(2, H, W).clone()
+    return grads, cam if camera else None, fov if intrinsics else None, rays, scratch, need
+
+
+def _camera_rows(P):
+    return (P + 127) // 128
+
+
+@pytest.mark.parametrize("P", [1, 128, 129, 64 * 128 + 1])
+@pytest.mark.parametrize("W,H", [(16, 16), (400, 656)])
+def test_scratch_bounds_and_initialisation(P, W, H):
+    """With the pose outputs, the focal-length outputs, both or neither: nothing is written past the scratch size the library
+    asks for (the guard band keeps its fill), and no output depends on what the scratch or the outputs held before the call
+    (pre-filled with 0x00 and with 0xFF, the pose, focal and ray outputs are bit-identical wherever the blend's outputs are;
+    the ray map and the focal sums always).  P = 1 and 128 have one camera row, which the joint layout pads from 128 to 256
+    bytes, and 8 193 has 65; W x H = 16 x 16 is one tile, 400 x 656 is 1 025.  The pose outputs are also the fp64
+    sum of the camera rows left in the scratch, rounded to float."""
+    cam, gs = gof_synth.make_scene(dict(P=P, width=W, height=H, seed=90 + P), view=3)
+    fwd = _forward(cam, gs)
+    assert int((fwd[2] > 0).sum()) > 0
+    dL = torch.randn(9, H, W, generator=torch.Generator().manual_seed(6)).cuda()
+    for camera in (False, True):
+        for intrinsics in (False, True):
+            runs = []
+            for fill in (0x00, 0xFF):
+                r = _backward_ex(fwd, dL, camera, intrinsics, fill)
+                scratch, need = r[4], r[5]
+                assert bool((scratch[need:] == fill).all()), (camera, intrinsics, fill, "write past the end of the scratch")
+                runs.append(r)
+            (g0, c0, f0, r0, _, _), (g1, c1, f1, r1, _, _) = runs
+            for t in g0 + g1:   # every gradient element was written
+                assert not bool(torch.isnan(t).any())
+            same = bool(_same_blend(g0, g1, P).all())
+            if camera:   # k_camera_grad_sum against the fp64 sum of the rows it read (at the front of the scratch)
+                rows = runs[0][4][:_camera_rows(P) * 128].view(torch.float64).view(-1, 16).cpu().numpy()
+                tot, mag = rows.sum(axis=0), np.abs(rows).sum(axis=0)
+                want = np.concatenate([np.stack([tot[3 * k:3 * k + 3] for k in range(4)], 0), np.zeros((4, 1))], 1).ravel()
+                want = np.concatenate([want, tot[12:15]])
+                wmag = np.concatenate([np.concatenate([np.stack([mag[3 * k:3 * k + 3] for k in range(4)], 0), np.zeros((4, 1))], 1).ravel(),
+                                       mag[12:15]])
+                got = c0.cpu().numpy().astype(np.float64)
+                assert (np.abs(got - want) <= 0.5 * _ulp(want) + 2.0 ** -46 * wmag).all(), (got, want)
+            if camera and same:
+                assert torch.equal(_bits(c0), _bits(c1)), (camera, intrinsics)
+            elif camera:   # the blend's double atomics rounded some Gaussian differently (test (b))
+                assert _util.same_up_to_summation_order(c0, c1), (camera, intrinsics)
+            if intrinsics:
+                assert torch.equal(_bits(f0), _bits(f1)) and torch.equal(r0.view(torch.int64), r1.view(torch.int64))
+                assert bool(torch.isfinite(r0).all())
 
 
 # ---- the public API ----------------------------------------------------------------------------------------------------
