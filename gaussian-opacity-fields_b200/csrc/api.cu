@@ -197,7 +197,7 @@ void gof_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* gof_last_error(void) { return g_err; }
-extern "C" int gof_version(void) { return 102; }
+extern "C" int gof_version(void) { return 103; }
 
 static int validate_scene(const gof_scene_t* s) {
   if (!s) { gof_set_error("scene is NULL"); return GOF_E_INVALID; }
@@ -273,13 +273,30 @@ static int gaussian_side(const gof_scene_t* s, const GofView& v, gof_alloc_fn ge
 // image scratch, NULL if its allocator failed).
 static int point_side(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
                       const uint32_t* point_list, const uint2* ranges, char* img, gof_alloc_fn point_alloc, void* point_user,
-                      gof_alloc_fn point_binning_alloc, void* point_binning_user, float* out_color, float* out_alpha_integrated,
-                      float* out_color_integrated, const GofIntMin* mn, cudaStream_t st) {
+                      gof_alloc_fn point_binning_alloc, void* point_binning_user, const gof_integrate_out_t& out, cudaStream_t st) {
   char* pts = (char*)point_alloc(point_user, gof_point_layout((size_t)PN).bytes);
   char* pbin = (char*)point_binning_alloc(point_binning_user, gof_point_bin_layout((size_t)PN, v.tiles, gof_sm_count()).bytes);
   if (!img || !pts || !pbin) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
-  return gof_launch_integrate(s, v, PN, points3D, splat, point_list, ranges, img, pts, pbin, out_color, out_alpha_integrated,
-                              out_color_integrated, mn, st);
+  return gof_launch_integrate(s, v, PN, points3D, splat, point_list, ranges, img, pts, pbin, out, st);
+}
+
+// The checks of both queries' outputs (gof_integrate_out_t) and allocators, in one order: out given, no field of the other mode,
+// the view, the allocators.  Then, with something to do, each query checks its buffers and integrate_outputs_given.
+static int check_integrate_out(const char* who, const gof_integrate_out_t* out, bool grad_min_offered, bool allocators) {
+  const char* err = nullptr;
+  const bool min = out && (out->alpha_min || out->argmin);
+  if (!out) err = "out is NULL";
+  else if (min && (out->out_color || out->out_alpha_integrated || out->out_color_integrated))
+    err = "out_color / out_alpha_integrated / out_color_integrated must be NULL with alpha_min / argmin";
+  else if (!min && (out->color_min || out->grad_min)) err = "color_min / grad_min need alpha_min and argmin";
+  else if (out->grad_min && !grad_min_offered) err = "grad_min is an output of gof_integrate_cached only";
+  else if (min && (out->view < 0 || out->view >= (1 << 30))) err = "view outside [0, 2^30)";   // 2^30 is argmin's "no view" value
+  else if (!allocators) err = "allocators must be non-NULL";
+  if (err) gof_set_error("%s: %s", who, err);
+  return err ? GOF_E_INVALID : GOF_OK;
+}
+static bool integrate_outputs_given(const gof_integrate_out_t& o) {
+  return o.alpha_min || o.argmin ? o.alpha_min && o.argmin : o.out_color && o.out_alpha_integrated && o.out_color_integrated;
 }
 
 extern "C" int gof_rasterize_forward(const gof_scene_t* s, gof_alloc_fn geom_alloc, void* geom_user,
@@ -488,17 +505,16 @@ extern "C" int gof_export_state(int P, int width, int height, int num_rendered, 
 extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D, gof_alloc_fn geom_alloc, void* geom_user,
                              gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc, void* image_user,
                              gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
-                             void* point_binning_user, float* out_color, int* radii, float* out_alpha_integrated,
-                             float* out_color_integrated, int* num_rendered, void* stream) {
+                             void* point_binning_user, int* radii, int* num_rendered, const gof_integrate_out_t* out, void* stream) {
   int rc = validate_scene(s);
   if (rc != GOF_OK) return rc;
-  if (!geom_alloc || !binning_alloc || !image_alloc || !point_alloc || !point_binning_alloc || !num_rendered) {
-    gof_set_error("integrate: allocators / num_rendered must be non-NULL");
-    return GOF_E_INVALID;
-  }
+  if ((rc = check_integrate_out("integrate", out, false, geom_alloc && binning_alloc && image_alloc && point_alloc &&
+                                point_binning_alloc)) != GOF_OK)
+    return rc;
+  if (!num_rendered) { gof_set_error("integrate: num_rendered is NULL"); return GOF_E_INVALID; }
   *num_rendered = 0;
   if (s->P == 0 || PN <= 0) return GOF_OK;   // rasterize_points.cu:305
-  if (!points3D || !out_color || !radii || !out_alpha_integrated || !out_color_integrated) {
+  if (!points3D || !radii || !integrate_outputs_given(*out)) {
     gof_set_error("integrate: NULL argument");
     return GOF_E_INVALID;
   }
@@ -510,43 +526,7 @@ extern "C" int gof_integrate(const gof_scene_t* s, int PN, const float* points3D
     return rc;
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
                     reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
-                    point_alloc, point_user, point_binning_alloc, point_binning_user, out_color, out_alpha_integrated,
-                    out_color_integrated, nullptr, st);
-}
-
-// One view of the multi-view opacity field (DESIGN.md 4.12): gof_integrate's Gaussian and point sides, then k_integrate<true>
-// folds each projecting point's alpha into alpha_min / argmin instead of writing the query's outputs.  With color_min,
-// k_integrate<true, true> also writes the winner's colour there (DESIGN.md 4.13).
-extern "C" int gof_integrate_min(const gof_scene_t* s, int PN, const float* points3D, int view, gof_alloc_fn geom_alloc,
-                                 void* geom_user, gof_alloc_fn binning_alloc, void* binning_user, gof_alloc_fn image_alloc,
-                                 void* image_user, gof_alloc_fn point_alloc, void* point_user, gof_alloc_fn point_binning_alloc,
-                                 void* point_binning_user, int* radii, float* alpha_min, int* argmin, float* color_min, void* stream) {
-  int rc = validate_scene(s);
-  if (rc != GOF_OK) return rc;
-  if (!geom_alloc || !binning_alloc || !image_alloc || !point_alloc || !point_binning_alloc) {
-    gof_set_error("integrate_min: allocators must be non-NULL");
-    return GOF_E_INVALID;
-  }
-  if (view < 0 || view >= (1 << 30)) {   // 2^30 is argmin's "no view" value
-    gof_set_error("integrate_min: view %d outside [0, 2^30)", view);
-    return GOF_E_INVALID;
-  }
-  if (s->P == 0 || PN <= 0) return GOF_OK;
-  if (!points3D || !radii || !alpha_min || !argmin) {
-    gof_set_error("integrate_min: NULL argument");
-    return GOF_E_INVALID;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  const GofView v = gof_make_view(s);
-  GaussianSide g;
-  int num_rendered = 0;
-  if ((rc = gaussian_side(s, v, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, radii, 0.5f, false,
-                          &num_rendered, st, g)) != GOF_OK)
-    return rc;
-  const GofIntMin mn{alpha_min, argmin, view, color_min};
-  return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(g.geom + g.GL.splat),
-                    reinterpret_cast<const uint32_t*>(g.bin + g.BL.point_list), reinterpret_cast<const uint2*>(g.img + g.IL.ranges), g.img,
-                    point_alloc, point_user, point_binning_alloc, point_binning_user, nullptr, nullptr, nullptr, &mn, st);
+                    point_alloc, point_user, point_binning_alloc, point_binning_user, *out, st);
 }
 
 extern "C" size_t gof_integrate_backward_scratch_bytes(int P) { return gof_integrate_backward_scratch(P); }
@@ -653,50 +633,17 @@ extern "C" int gof_integrate_prepare(const gof_scene_t* s, gof_alloc_fn geom_all
 
 extern "C" int gof_integrate_cached(const gof_scene_t* s, int PN, const float* points3D, const void* cache, int num_rendered,
                                     gof_alloc_fn image_alloc, void* image_user, gof_alloc_fn point_alloc, void* point_user,
-                                    gof_alloc_fn point_binning_alloc, void* point_binning_user, float* out_color,
-                                    float* out_alpha_integrated, float* out_color_integrated, void* stream) {
+                                    gof_alloc_fn point_binning_alloc, void* point_binning_user, const gof_integrate_out_t* out,
+                                    void* stream) {
   if (!s || s->P < 0 || s->width <= 0 || s->height <= 0 || !s->viewmatrix || !s->background) {
     gof_set_error("integrate_cached: scene needs P, width, height, tan_fov, viewmatrix, background");
     return GOF_E_INVALID;
   }
+  int rc = check_integrate_out("integrate_cached", out, true, image_alloc && point_alloc && point_binning_alloc);
+  if (rc != GOF_OK) return rc;
   if (s->P == 0 || PN <= 0) return GOF_OK;
-  if (!cache || !image_alloc || !point_alloc || !point_binning_alloc || !points3D || !out_color || !out_alpha_integrated ||
-      !out_color_integrated || num_rendered < 0) {
+  if (!cache || !points3D || num_rendered < 0 || !integrate_outputs_given(*out)) {
     gof_set_error("integrate_cached: NULL argument");
-    return GOF_E_INVALID;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  const GofView v = gof_make_view(s);
-  const GofIntCacheLayout CL = gof_int_cache_layout((size_t)s->P, s->width, s->height, (size_t)num_rendered);
-  const GofImageLayout IL = gof_image_layout(s->width, s->height);
-  char* img = (char*)image_alloc(image_user, IL.bytes);
-  const char* c = (const char*)cache;
-  return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(c + CL.splat), reinterpret_cast<const uint32_t*>(c + CL.point_list),
-                    reinterpret_cast<const uint2*>(c + CL.ranges), img, point_alloc, point_user, point_binning_alloc,
-                    point_binning_user, out_color, out_alpha_integrated, out_color_integrated, nullptr, st);
-}
-
-// The multi-view opacity field's running minimum (gof_integrate_min) against a gof_integrate_prepare cache, optionally with the
-// winning view's point gradient, formed in the same pass (k_integrate<true, *, true>, DESIGN.md 4.14).
-extern "C" int gof_integrate_cached_min(const gof_scene_t* s, int PN, const float* points3D, int view, const void* cache,
-                                        int num_rendered, gof_alloc_fn image_alloc, void* image_user, gof_alloc_fn point_alloc,
-                                        void* point_user, gof_alloc_fn point_binning_alloc, void* point_binning_user, float* alpha_min,
-                                        int* argmin, float* color_min, float* grad_min, void* stream) {
-  if (!s || s->P < 0 || s->width <= 0 || s->height <= 0 || !s->viewmatrix || !s->background) {
-    gof_set_error("integrate_cached_min: scene needs P, width, height, tan_fov, viewmatrix, background");
-    return GOF_E_INVALID;
-  }
-  if (!image_alloc || !point_alloc || !point_binning_alloc) {
-    gof_set_error("integrate_cached_min: allocators must be non-NULL");
-    return GOF_E_INVALID;
-  }
-  if (view < 0 || view >= (1 << 30)) {   // 2^30 is argmin's "no view" value
-    gof_set_error("integrate_cached_min: view %d outside [0, 2^30)", view);
-    return GOF_E_INVALID;
-  }
-  if (s->P == 0 || PN <= 0) return GOF_OK;
-  if (!cache || !points3D || !alpha_min || !argmin || num_rendered < 0) {
-    gof_set_error("integrate_cached_min: NULL argument");
     return GOF_E_INVALID;
   }
   cudaStream_t st = (cudaStream_t)stream;
@@ -704,8 +651,7 @@ extern "C" int gof_integrate_cached_min(const gof_scene_t* s, int PN, const floa
   const GofIntCacheLayout CL = gof_int_cache_layout((size_t)s->P, s->width, s->height, (size_t)num_rendered);
   char* img = (char*)image_alloc(image_user, gof_image_layout(s->width, s->height).bytes);
   const char* c = (const char*)cache;
-  const GofIntMin mn{alpha_min, argmin, view, color_min, grad_min};
   return point_side(s, v, PN, points3D, reinterpret_cast<const GofSplat*>(c + CL.splat), reinterpret_cast<const uint32_t*>(c + CL.point_list),
                     reinterpret_cast<const uint2*>(c + CL.ranges), img, point_alloc, point_user, point_binning_alloc,
-                    point_binning_user, nullptr, nullptr, nullptr, &mn, st);
+                    point_binning_user, *out, st);
 }

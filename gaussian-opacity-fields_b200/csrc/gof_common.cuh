@@ -407,17 +407,10 @@ static inline GofPointBinLayout gof_point_bin_layout(size_t PN, int tiles, int s
   L.ids = take((size_t)L.nblk * 256 * GOF_INT_MAX_CONTRIB * 2);
   L.bytes = o; return L;
 }
-// mn != NULL: the running minimum over views (gof_integrate_min, DESIGN.md 4.12) instead of the query's outputs, which are not read
-struct GofIntMin {
-  float* alpha_min;   // [PN]
-  int* argmin;        // [PN]
-  int view;
-  float* color_min;   // [PN][3] or NULL: also the winning view's colour (gof_integrate_min's color_min, DESIGN.md 4.13)
-  float* grad_min;    // [PN][3] or NULL: also the winning view's d alpha / d point (gof_integrate_cached_min, DESIGN.md 4.14)
-};
+// out: the query's outputs or, with out.alpha_min, the running minimum over views (gof_integrate_out_t; checked by the caller)
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
-                         const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin, float* out_color,
-                         float* out_alpha, float* out_color_int, const GofIntMin* mn, cudaStream_t st);
+                         const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin,
+                         const gof_integrate_out_t& out, cudaStream_t st);
 // The backward of the query (DESIGN.md 4.11) from the state gof_launch_integrate left in geom / pts / pbin: dL_dalpha [PN] ->
 // dL_dpoints3D [PN][3] (optional) and, through the accumulator rows and k_preprocess_backward, the Gaussian gradients.  The
 // contributor slab in pbin and the accumulator rows in geom are rewritten.  o.scratch: gof_integrate_backward_scratch(P) bytes.

@@ -717,8 +717,8 @@ IntQuery int_query(const GofView& v, const GofSplat* splat, const uint32_t* poin
 }  // namespace
 
 int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const float* points3D, const GofSplat* splat,
-                         const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin, float* out_color,
-                         float* out_alpha, float* out_color_int, const GofIntMin* mn, cudaStream_t st) {
+                         const uint32_t* point_list, const uint2* ranges, char* img, char* pts, char* pbin,
+                         const gof_integrate_out_t& out, cudaStream_t st) {
   const bool debug = s->debug != 0;
   const GofImageLayout IL = gof_image_layout(s->width, s->height);
   const GofPointLayout PL = gof_point_layout((size_t)PN);
@@ -744,17 +744,17 @@ int gof_launch_integrate(const gof_scene_t* s, const GofView& v, int PN, const f
   a.bg = s->background;
   a.final_T = reinterpret_cast<float*>(img + IL.accum);
   a.ncontrib = reinterpret_cast<uint32_t*>(img + IL.ncontrib);
-  a.out_color = out_color; a.out_alpha = out_alpha; a.out_color_int = out_color_int;
-  if (mn) {
-    a.alpha_min = mn->alpha_min; a.argmin = mn->argmin; a.view = mn->view; a.color_min = mn->color_min;
-    a.grad_min = mn->grad_min; a.points3D = points3D; a.vm = s->viewmatrix;
+  a.out_color = out.out_color; a.out_alpha = out.out_alpha_integrated; a.out_color_int = out.out_color_integrated;
+  if (out.alpha_min) {
+    a.alpha_min = out.alpha_min; a.argmin = out.argmin; a.view = out.view; a.color_min = out.color_min;
+    a.grad_min = out.grad_min; a.points3D = points3D; a.vm = s->viewmatrix;
     // persistent CTAs stride over the tiles, each with the slab of its blockIdx.x (PBL.nblk slabs exist)
     const int grad_grid = std::min(PBL.nblk, INT_GRAD_CTAS_PER_SM * gof_sm_count());
-    if (mn->grad_min && mn->color_min)
+    if (out.grad_min && out.color_min)
       GOF_LAUNCH("integrate_min_color_grad", st, k_integrate<true, true, true><<<grad_grid, GOF_BLOCK_SIZE, 0, st>>>(a));
-    else if (mn->grad_min)
+    else if (out.grad_min)
       GOF_LAUNCH("integrate_min_grad", st, k_integrate<true, false, true><<<grad_grid, GOF_BLOCK_SIZE, 0, st>>>(a));
-    else if (mn->color_min)
+    else if (out.color_min)
       GOF_LAUNCH("integrate_min_color", st, k_integrate<true, true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));
     else
       GOF_LAUNCH("integrate_min", st, k_integrate<true><<<PBL.nblk, GOF_BLOCK_SIZE, 0, st>>>(a));

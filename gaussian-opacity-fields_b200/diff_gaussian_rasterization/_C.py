@@ -48,6 +48,12 @@ class _BackwardOut(ctypes.Structure):
         [("scratch_bytes", ctypes.c_size_t)]
 
 
+class _IntegrateOut(ctypes.Structure):
+    """gof_integrate_out_t: the outputs of gof_integrate and gof_integrate_cached, the query's or the running minimum's."""
+    _fields_ = [(n, _fp) for n in ("out_color", "out_alpha_integrated", "out_color_integrated", "alpha_min", "argmin")] + \
+        [("view", ctypes.c_int), ("color_min", _fp), ("grad_min", _fp)]
+
+
 class _StateView(ctypes.Structure):
     _fields_ = [(n, _fp) for n in (
         "depths", "means2D", "conic_opacity", "rgb", "view2gaussian", "clamped", "tiles_touched",
@@ -70,7 +76,7 @@ _lib.gof_mark_visible.restype = ctypes.c_int
 _lib.gof_mark_visible.argtypes = [ctypes.c_int, _fp, _fp, _fp, _fp, ctypes.c_void_p]
 _lib.gof_integrate.restype = ctypes.c_int
 _lib.gof_integrate.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp] + [_ALLOC_FN, ctypes.c_void_p] * 5 + \
-    [_fp, _fp, _fp, _fp, ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
+    [_fp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(_IntegrateOut), ctypes.c_void_p]
 _lib.gof_export_state.restype = ctypes.c_int
 _lib.gof_export_state.argtypes = [ctypes.c_int] * 4 + [_fp] * 4 + [ctypes.POINTER(_StateView), ctypes.c_void_p]
 
@@ -416,21 +422,49 @@ def integrate_gaussians_to_points_state(*args):
     return _integrate(*args)
 
 
+def _running_min(PN, alpha_min, argmin, color_min=None, grad_min=None):
+    """Checks the running minimum's tensors: alpha_min float32 [PN], argmin int32 [PN], color_min and grad_min float32 [PN,3] or
+    None, all contiguous.  Returns those given, by name."""
+    given = {"alpha_min": (alpha_min, torch.float32, (PN,)), "argmin": (argmin, torch.int32, (PN,)),
+             "color_min": (color_min, torch.float32, (PN, 3)), "grad_min": (grad_min, torch.float32, (PN, 3))}
+    for name, (t, dt, shape) in given.items():
+        if t is not None and (t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous()):
+            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape {shape}")
+    return {name: t for name, (t, _, _) in given.items() if t is not None}
+
+
+def _query_outputs(PN, H, W, dev, minimum):
+    """The outputs of one query by gof_integrate_out_t's field names: the running minimum's tensors `minimum` (from _running_min)
+    or, with `minimum` None, the query's three, initialised as the library expects (it leaves the points that do not project,
+    and channels 3-5 of out_color, alone)."""
+    if minimum is not None:
+        return minimum
+    return {"out_color": torch.zeros((9, H, W), dtype=torch.float32, device=dev),
+            "out_alpha_integrated": torch.ones((PN,), dtype=torch.float32, device=dev),
+            "out_color_integrated": torch.zeros((PN, 3), dtype=torch.float32, device=dev)}
+
+
+def _integrate_out(outs, view, dev):
+    """The _IntegrateOut of _query_outputs' tensors."""
+    return _IntegrateOut(view=int(view), **{k: _ptr(t, t.dtype, device=dev) for k, t in outs.items()})
+
+
 def _integrate(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset, image_height,
-               image_width, sh, degree, campos, prefiltered, debug):
+               image_width, sh, degree, campos, prefiltered, debug, view=0, **running_min):
+    """gof_integrate, the query's outputs or, with `running_min` (the tensors of _running_min), a view's step of the running
+    minimum.  Returns integrate_gaussians_to_points_state's tuple; its three outputs are None with `running_min`."""
     if points3D.ndimension() != 2 or points3D.size(1) != 3:
         raise RuntimeError("points3D must have dimensions (num_points, 3)")
+    PN = points3D.size(0)
+    minimum = _running_min(PN, **running_min) if running_min else None
     keep = []
     s = _scene(keep, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset,
                image_height, image_width, sh, degree, campos, prefiltered, debug)
     dev = means3D.device
-    PN = points3D.size(0)
-    out_color = torch.zeros((9, int(image_height), int(image_width)), dtype=torch.float32, device=dev)
+    outs = _query_outputs(PN, int(image_height), int(image_width), dev, minimum)
     radii = torch.zeros((s.P,), dtype=torch.int32, device=dev)
-    alpha_int = torch.ones((PN,), dtype=torch.float32, device=dev)
-    color_int = torch.zeros((PN, 3), dtype=torch.float32, device=dev)
     sdev = dev if means3D.is_cuda else torch.device("cuda")
     geom, binning, img = _Scratch(sdev, "geom"), _Scratch(sdev, "binning", 1.25), _Scratch(sdev, "image")
     pts, pbin = _Scratch(sdev, "points"), _Scratch(sdev, "point_binning")
@@ -438,53 +472,26 @@ def _integrate(background, points3D, means3D, colors, opacity, scales, rotations
     if s.P != 0 and PN != 0:
         p3 = points3D.contiguous()
         with torch.cuda.device(dev):
-            _check(_lib.gof_integrate(ctypes.byref(s), PN, _ptr(p3), geom.cb, None, binning.cb, None, img.cb, None,
-                                      pts.cb, None, pbin.cb, None, out_color.data_ptr(), radii.data_ptr(),
-                                      alpha_int.data_ptr(), color_int.data_ptr(), ctypes.byref(rendered), _stream()))
-    return (rendered.value, out_color, alpha_int, color_int, radii, geom.tensor, binning.tensor, img.tensor, pts.tensor,
-            pbin.tensor)
-
-
-_lib.gof_integrate_min.restype = ctypes.c_int
-_lib.gof_integrate_min.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int] + [_ALLOC_FN, ctypes.c_void_p] * 5 + \
-    [_fp, _fp, _fp, _fp, ctypes.c_void_p]
+            _check(_lib.gof_integrate(ctypes.byref(s), PN, _ptr(p3, device=dev), geom.cb, None, binning.cb, None, img.cb, None,
+                                      pts.cb, None, pbin.cb, None, radii.data_ptr(), ctypes.byref(rendered),
+                                      ctypes.byref(_integrate_out(outs, view, dev)), _stream()))
+    return (rendered.value, outs.get("out_color"), outs.get("out_alpha_integrated"), outs.get("out_color_integrated"), radii,
+            geom.tensor, binning.tensor, img.tensor, pts.tensor, pbin.tensor)
 
 
 def integrate_gaussians_to_points_min(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier,
                                       cov3D_precomp, view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size,
                                       subpixel_offset, image_height, image_width, sh, degree, campos, prefiltered, debug, view,
                                       alpha_min, argmin, color_min=None):
-    """gof_integrate_min (extension, DESIGN.md 4.12): integrate_gaussians_to_points for view index `view`, folded into the running
-    minimum over views in place: where a point's alpha_integrated < alpha_min, alpha_min takes it and argmin takes `view`.
-    alpha_min (float32 [PN], start at 1) and argmin (int32 [PN], start at 2^30) must be contiguous.  With color_min (float32
-    [PN,3], contiguous; DESIGN.md 4.13) the same update also stores the point's color_integrated of
-    that view.  Returns radii [P]."""
-    if points3D.ndimension() != 2 or points3D.size(1) != 3:
-        raise RuntimeError("points3D must have dimensions (num_points, 3)")
-    PN = points3D.size(0)
-    checks = [("alpha_min", alpha_min, torch.float32, (PN,)), ("argmin", argmin, torch.int32, (PN,))]
-    if color_min is not None:
-        checks.append(("color_min", color_min, torch.float32, (PN, 3)))
-    for name, t, dt, shape in checks:
-        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
-            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape {shape}")
-    keep = []
-    s = _scene(keep, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-               view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset,
-               image_height, image_width, sh, degree, campos, prefiltered, debug)
-    dev = means3D.device
-    radii = torch.zeros((s.P,), dtype=torch.int32, device=dev)
-    if s.P != 0 and PN != 0:
-        sdev = dev if means3D.is_cuda else torch.device("cuda")
-        geom, binning, img = _Scratch(sdev, "geom"), _Scratch(sdev, "binning", 1.25), _Scratch(sdev, "image")
-        pts, pbin = _Scratch(sdev, "points"), _Scratch(sdev, "point_binning")
-        p3 = points3D.contiguous()
-        allocs = (geom.cb, None, binning.cb, None, img.cb, None, pts.cb, None, pbin.cb, None)
-        with torch.cuda.device(dev):
-            _check(_lib.gof_integrate_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), *allocs, radii.data_ptr(),
-                                          _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev),
-                                          _ptr(color_min, device=dev), _stream()))
-    return radii
+    """gof_integrate's running minimum (extension, DESIGN.md 4.12): integrate_gaussians_to_points for view index `view`, folded
+    into the running minimum over views in place: where a point's alpha_integrated < alpha_min, alpha_min takes it and argmin
+    takes `view`.  alpha_min (float32 [PN], start at 1) and argmin (int32 [PN], start at 2^30) must be contiguous.  With
+    color_min (float32 [PN,3], contiguous; DESIGN.md 4.13) the same update also stores the point's color_integrated of that
+    view.  Returns radii [P]."""
+    return _integrate(background, points3D, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                      view2gaussian_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, kernel_size, subpixel_offset, image_height,
+                      image_width, sh, degree, campos, prefiltered, debug, view, alpha_min=alpha_min, argmin=argmin,
+                      color_min=color_min)[4]
 
 
 _lib.gof_integrate_backward_scratch_bytes.restype = ctypes.c_size_t
@@ -556,7 +563,7 @@ _lib.gof_integrate_prepare.restype = ctypes.c_int
 _lib.gof_integrate_prepare.argtypes = [ctypes.POINTER(_Scene)] + [_ALLOC_FN, ctypes.c_void_p] * 4 + [_fp, ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
 _lib.gof_integrate_cached.restype = ctypes.c_int
 _lib.gof_integrate_cached.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, _fp, ctypes.c_int] + [_ALLOC_FN, ctypes.c_void_p] * 3 + \
-    [_fp, _fp, _fp, ctypes.c_void_p]
+    [ctypes.POINTER(_IntegrateOut), ctypes.c_void_p]
 
 
 class IntegrateCache:
@@ -590,64 +597,43 @@ def integrate_prepare(background, means3D, colors, opacity, scales, rotations, s
     return IntegrateCache(cache.tensor, rendered.value, radii, s.P, int(image_height), int(image_width))
 
 
-def integrate_points_cached(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, debug=False):
-    """Point side of integrate_gaussians_to_points against an IntegrateCache of the same view.
-    Returns (out_color[9,H,W], out_alpha_integrated[PN], out_color_integrated[PN,3])."""
+def _integrate_cached(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, debug, view=0, **running_min):
+    """gof_integrate_cached, the query's outputs or, with `running_min` (the tensors of _running_min), a view's step of the
+    running minimum.  Returns the three outputs, None with `running_min`."""
     if points3D.ndimension() != 2 or points3D.size(1) != 3:
         raise RuntimeError("points3D must have dimensions (num_points, 3)")
+    PN = points3D.size(0)
+    minimum = _running_min(PN, **running_min) if running_min else None
     dev = cache.buffer.device
     s = _Scene()
     s.P, s.width, s.height = cache.P, cache.W, cache.H
     s.tan_fovx, s.tan_fovy = _scalar(tan_fovx), _scalar(tan_fovy)
     bg, vm, p3 = _c(background), _c(viewmatrix), _c(points3D)
     s.background, s.viewmatrix, s.debug = _ptr(bg, device=dev), _ptr(vm, device=dev), int(bool(debug))
-    PN = p3.size(0)
-    out_color = torch.zeros((9, cache.H, cache.W), dtype=torch.float32, device=dev)
-    alpha_int = torch.ones((PN,), dtype=torch.float32, device=dev)
-    color_int = torch.zeros((PN, 3), dtype=torch.float32, device=dev)
+    outs = _query_outputs(PN, cache.H, cache.W, dev, minimum)
     img, pts, pbin = _Scratch(dev, "image"), _Scratch(dev, "points"), _Scratch(dev, "point_binning")
     if cache.P != 0 and PN != 0:
         with torch.cuda.device(dev):
-            _check(_lib.gof_integrate_cached(ctypes.byref(s), PN, _ptr(p3, device=dev), cache.buffer.data_ptr(), cache.num_rendered, img.cb,
-                                             None, pts.cb, None, pbin.cb, None, out_color.data_ptr(), alpha_int.data_ptr(),
-                                             color_int.data_ptr(), _stream()))
-    return out_color, alpha_int, color_int
+            _check(_lib.gof_integrate_cached(ctypes.byref(s), PN, _ptr(p3, device=dev), cache.buffer.data_ptr(), cache.num_rendered,
+                                             img.cb, None, pts.cb, None, pbin.cb, None, ctypes.byref(_integrate_out(outs, view, dev)),
+                                             _stream()))
+    return outs.get("out_color"), outs.get("out_alpha_integrated"), outs.get("out_color_integrated")
 
 
-_lib.gof_integrate_cached_min.restype = ctypes.c_int
-_lib.gof_integrate_cached_min.argtypes = [ctypes.POINTER(_Scene), ctypes.c_int, _fp, ctypes.c_int, _fp, ctypes.c_int] + \
-    [_ALLOC_FN, ctypes.c_void_p] * 3 + [_fp, _fp, _fp, _fp, ctypes.c_void_p]
+def integrate_points_cached(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, debug=False):
+    """Point side of integrate_gaussians_to_points against an IntegrateCache of the same view.
+    Returns (out_color[9,H,W], out_alpha_integrated[PN], out_color_integrated[PN,3])."""
+    return _integrate_cached(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, debug)
 
 
 def integrate_points_cached_min(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, view, alpha_min, argmin,
                                 color_min=None, grad_min=None, debug=False):
-    """gof_integrate_cached_min (extension, DESIGN.md 4.14): integrate_points_cached for view index `view`, folded into the
-    running minimum over views in place, as integrate_gaussians_to_points_min folds it (alpha_min float32 [PN] from 1, argmin
-    int32 [PN] from 2^30, color_min float32 [PN,3] or None).  With grad_min (float32 [PN,3]) the same update also stores the
-    winning view's d alpha_integrated / d point in world space; points that no view updates keep what the caller put there."""
-    if points3D.ndimension() != 2 or points3D.size(1) != 3:
-        raise RuntimeError("points3D must have dimensions (num_points, 3)")
-    PN = points3D.size(0)
-    checks = [("alpha_min", alpha_min, torch.float32, (PN,)), ("argmin", argmin, torch.int32, (PN,))]
-    for name, t in (("color_min", color_min), ("grad_min", grad_min)):
-        if t is not None:
-            checks.append((name, t, torch.float32, (PN, 3)))
-    for name, t, dt, shape in checks:
-        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
-            raise RuntimeError(f"gof_b200: {name} must be a contiguous {dt} tensor of shape {shape}")
-    dev = cache.buffer.device
-    s = _Scene()
-    s.P, s.width, s.height = cache.P, cache.W, cache.H
-    s.tan_fovx, s.tan_fovy = _scalar(tan_fovx), _scalar(tan_fovy)
-    bg, vm, p3 = _c(background), _c(viewmatrix), _c(points3D)
-    s.background, s.viewmatrix, s.debug = _ptr(bg, device=dev), _ptr(vm, device=dev), int(bool(debug))
-    if cache.P != 0 and PN != 0:
-        img, pts, pbin = _Scratch(dev, "image"), _Scratch(dev, "points"), _Scratch(dev, "point_binning")
-        with torch.cuda.device(dev):
-            _check(_lib.gof_integrate_cached_min(ctypes.byref(s), PN, _ptr(p3, device=dev), int(view), cache.buffer.data_ptr(),
-                                                 cache.num_rendered, img.cb, None, pts.cb, None, pbin.cb, None,
-                                                 _ptr(alpha_min, device=dev), _ptr(argmin, torch.int32, device=dev),
-                                                 _ptr(color_min, device=dev), _ptr(grad_min, device=dev), _stream()))
+    """gof_integrate_cached's running minimum (extension, DESIGN.md 4.14): integrate_points_cached for view index `view`, folded
+    into the running minimum over views in place, as integrate_gaussians_to_points_min folds it (alpha_min float32 [PN] from 1,
+    argmin int32 [PN] from 2^30, color_min float32 [PN,3] or None).  With grad_min (float32 [PN,3]) the same update also stores
+    the winning view's d alpha_integrated / d point in world space; points that no view updates keep what the caller put there."""
+    _integrate_cached(cache, background, points3D, viewmatrix, tan_fovx, tan_fovy, debug, view, alpha_min=alpha_min, argmin=argmin,
+                      color_min=color_min, grad_min=grad_min)
 
 
 def export_state(P, W, H, num_rendered, geomBuffer, binningBuffer, imgBuffer, radii, masks=False):

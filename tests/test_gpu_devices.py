@@ -63,6 +63,20 @@ def test_rasterizer_computes_the_same_on_every_device():
             assert _util.same_up_to_summation_order(a, b), (d, name)
 
 
+def test_queries_refuse_points_on_another_device():
+    """The binding refuses query points on another device than the Gaussians or the cache, before the library sees the pointer."""
+    _need_two()
+    from diff_gaussian_rasterization import _C
+    cam, gs = gof_synth.make_scene("C2", view=3)
+    fa = _util.fwd_args(cam, gs, torch.device("cuda", 0))
+    p = torch.rand(1000, 3, device="cuda:1")
+    with pytest.raises(RuntimeError, match="expected cuda:0"):
+        _C.integrate_gaussians_to_points(fa[0], p, *fa[1:])
+    cache = _C.integrate_prepare(*fa)
+    with pytest.raises(RuntimeError, match="expected cuda:0"):
+        _C.integrate_points_cached(cache, fa[0], p, fa[9], fa[11], fa[12])
+
+
 def test_conv_wgrad_on_every_device():
     """The 16 -> 16 instantiation needs its dynamic shared memory opt-in on each device; {-1, 0, 1} inputs make dW and db exact."""
     _need_two()

@@ -1,6 +1,6 @@
 """CPU: the float64 oracle of the query's colour backward (tests/integrate_grad_oracle/integrate_color_oracle.c, DESIGN.md 4.13) against central
 differences of a float64 restatement of one pixel's compositing with its blended set held fixed, and the argument checks of
-gof_integrate_backward and gof_integrate_min with the colour through the built library (decided before any device work)."""
+gof_integrate_backward with the colour through the built library (decided before any device work)."""
 import ctypes
 
 import numpy as np
@@ -120,7 +120,7 @@ def test_transmittance_skip_is_followed_by_accepted_pairs():
     assert np.all(o["dcol"][2] == 0) and np.all(o["dv2g"][2] == 0) and np.all(o["dcol"][3] != 0)
 
 
-# ---------------- argument checks of the two C entries with the colour ----------------
+# ---------------- argument checks of the colour backward and of the binding's color_min ----------------
 FAKE = 0x1000
 
 
@@ -177,28 +177,6 @@ def test_backward_color_refusals_with_out():
     assert _bwd(_C, bad) == -1
     o = _C._BackwardOut(dL_dopacity=FAKE, dL_dmean3D=FAKE, dL_dview2gaussian=FAKE, dL_dcolor=FAKE, scratch=FAKE, scratch_bytes=10 ** 6)
     assert _C._lib.gof_integrate_backward(None, 4, FAKE, 1, *[FAKE] * 9, ctypes.byref(o), None) == -1
-
-
-def test_min_color_refusals():
-    import test_integrate_min_abi as m
-    _C = _abi()
-    err = _C._lib.gof_last_error
-    s = _scene(_C)
-
-    def call(PN=4, view=0, allocs=None, points=FAKE, radii=FAKE, amin=FAKE, argmin=FAKE, cmin=FAKE):
-        allocs = allocs if allocs is not None else m._Allocs(_C)
-        return _C._lib.gof_integrate_min(ctypes.byref(s), PN, points, view, *allocs.args(), radii, amin, argmin, cmin, None)
-    for kw in (dict(points=None), dict(radii=None), dict(amin=None), dict(argmin=None)):
-        assert call(**kw) == -1 and b"NULL" in err(), kw
-    for view in (-1, 2 ** 30):
-        assert call(view=view) == -1 and b"view" in err()
-    a = m._Allocs(_C)
-    a.cbs[1] = _C._ALLOC_FN()
-    assert call(allocs=a) == -1 and b"allocators" in err()
-    a = m._Allocs(_C, fail=(0,))
-    assert call(allocs=a) == -3
-    a = m._Allocs(_C)
-    assert call(PN=0, allocs=a, points=None, radii=None, amin=None, argmin=None, cmin=None) == 0 and a.calls == []
 
 
 def test_binding_checks_color_min():

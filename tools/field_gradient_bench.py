@@ -3,7 +3,7 @@ from `--views` cached 1920x1080 cameras of the ring, queried at N points sampled
 
 Times, with CUDA events after a warm-up, alternating, `--reps` times each:
   * cached_alpha:   one evaluate_alpha pass over a CachedIntegrator (one gof_integrate_cached per view);
-  * field_gradient: one field_gradient pass over the same cache (one gof_integrate_cached_min with grad_min per view);
+  * field_gradient: one field_gradient pass over the same cache (one gof_integrate_cached with grad_min per view);
   * autograd_fwd / autograd_bwd: opacity_field(points, ...) and its .sum().backward() for the points alone (the uncached
     query per view, then the Gaussian side rebuilt for every winning view).
 Checks that field_gradient's alpha equals evaluate_alpha's and its gradient equals the autograd point gradient, bit for bit.

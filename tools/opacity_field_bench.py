@@ -2,8 +2,8 @@
 `--views` cameras of the ring, queried at N points sampled around the Gaussians' centres.
 
 Times, with CUDA events after warm-up, alternating: the plain multi-view query (`evaluate_alpha` over
-`GaussianRasterizer.integrate`, one call per view), the forward of `gof_extract.opacity_field` (one `gof_integrate_min` per
-view), the same forward with `return_color=True` (one `gof_integrate_min` with `color_min` per view, DESIGN.md 4.13) and the backward.  Reports ms per view for both forwards, the backward's ms in all and per winning view, and the
+`GaussianRasterizer.integrate`, one call per view), the forward of `gof_extract.opacity_field` (one running-minimum `gof_integrate` per
+view), the same forward with `return_color=True` (one with `color_min` per view, DESIGN.md 4.13) and the backward.  Reports ms per view for both forwards, the backward's ms in all and per winning view, and the
 per-kernel split of the library's event brackets.  Then the peak `torch.cuda.max_memory_allocated` growth over forward and
 backward of `opacity_field` against the naive composition (per-view `integrate_gaussians` kept by autograd, torch.min).  Checks
 that the field equals evaluate_alpha bit for bit and that the point gradients of two backward calls are bit-identical.
