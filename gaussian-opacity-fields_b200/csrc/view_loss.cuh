@@ -14,6 +14,12 @@
 //                       distortion mean and its constant gradient (ch 8); per-tile partial sums.
 //   kernel B (vl_b_*):  blurs the derivative maps back (the window is symmetric) and writes the rgb gradient (ch 0-2).
 //   kernel C:           fixed-order sum of the per-tile partials in double -> the four terms and the loss.
+//
+// Appearance mode (mapping != NULL; train.py:67-88, 157-159 with --use_decoupled_appearance): the L1 term becomes
+// mean over the crop (top, left, Hc, Wc) of |fl(m * rgb) - gt|, m = mapping[c][y-top][x-left] the appearance network's
+// output; SSIM, the normal and the distortion terms stay on the whole image.  Kernel A sums that L1 over the crop only,
+// kernel B adds its rgb gradient inside the crop and writes d loss / d mapping, kernel C divides by 3 Hc Wc.  With
+// mapping == NULL every phase does exactly what it did before the mode existed.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -43,6 +49,11 @@ struct VlParams {
   float* dmap;           // [9][H][W] scratch: d map/d mu1 [3], d map/d E11 [3], d map/d E12 [3]
   float* grad;           // [9][H][W] out (may be NULL: values only)
   float* partial;        // [tiles][4]: sum of SSIM map, sum |rgb-gt|, sum normal error, sum distortion
+  // appearance mode; the defaults are the plain L1
+  const float* mapping = nullptr;   // [3][Hc][Wc] appearance mapping, or NULL
+  float* grad_mapping = nullptr;    // [3][Hc][Wc] out: d loss / d mapping (NULL exactly when grad is)
+  int top = 0, left = 0, Hc = 0, Wc = 0;
+  float inv_Na3 = 0.f;              // 1/(3 Hc Wc)
 };
 
 struct VlShared {
@@ -58,6 +69,21 @@ struct VlShared {
 VL_HD float vl_load(const float* plane, int W, int H, int x, int y) {
   return (x >= 0 && x < W && y >= 0 && y < H) ? plane[(size_t)y * W + x] : 0.0f;
 }
+
+// m * v rounded to float before anything else touches it (torch's `mapping_image * crop_image`): no fused multiply-add
+VL_HD float vl_mul_rn(float m, float v) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(m, v);
+#else
+  return m * v;
+#endif
+}
+
+// appearance mode: is image pixel (x, y) inside the crop, and the offset of its mapping value in channel 0
+VL_HD bool vl_in_crop(const VlParams& p, int x, int y) {
+  return x >= p.left && x < p.left + p.Wc && y >= p.top && y < p.top + p.Hc;
+}
+VL_HD size_t vl_crop_offset(const VlParams& p, int x, int y) { return (size_t)(y - p.top) * p.Wc + (x - p.left); }
 
 VL_HD void vl_cross(const float* a, const float* b, float* o) {
   o[0] = a[1] * b[2] - a[2] * b[1];
@@ -128,7 +154,12 @@ VL_HD void vl_a_ssim(const VlParams& p, VlShared& s, int tile_x, int tile_y, int
   p.dmap[(6 + ch) * plane + o] = dm_de12;
   const float va = s.a[(ly + VL_R) * VL_HT + lx + VL_R], vb = s.b[(ly + VL_R) * VL_HT + lx + VL_R];
   s.red[0][tid] += map;
-  s.red[1][tid] += fabsf(va - vb);
+  if (p.mapping == nullptr) {
+    s.red[1][tid] += fabsf(va - vb);
+  } else if (vl_in_crop(p, x, y)) {
+    const float m = p.mapping[(size_t)ch * p.Hc * p.Wc + vl_crop_offset(p, x, y)];
+    s.red[1][tid] += fabsf(vl_mul_rn(m, va) - vb);
+  }
 }
 
 // phase N1: depth * ray direction on the 20x20 halo tile (outside the image: zero, never used)
@@ -274,7 +305,21 @@ VL_HD void vl_b_grad(const VlParams& p, VlShared& s, int tile_x, int tile_y, int
   }
   const size_t plane = (size_t)p.W * p.H, o = (size_t)y * p.W + x;
   const float va = p.render[ch * plane + o], vb = p.gt[ch * plane + o];
-  const float df = va - vb;
-  const float sgn = df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f);
-  p.grad[ch * plane + o] = (1.0f - p.lam) * sgn * p.inv_N3 - p.lam * p.inv_N3 * (v[0] + 2.f * va * v[1] + vb * v[2]);
+  if (p.mapping == nullptr) {
+    const float df = va - vb;
+    const float sgn = df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f);
+    p.grad[ch * plane + o] = (1.0f - p.lam) * sgn * p.inv_N3 - p.lam * p.inv_N3 * (v[0] + 2.f * va * v[1] + vb * v[2]);
+    return;
+  }
+  // appearance mode: the L1 term lives on the crop only; its sign is that of fl(m rgb) - gt (sgn(0) = 0, torch's abs)
+  float l1 = 0.f;
+  if (vl_in_crop(p, x, y)) {
+    const size_t oc = (size_t)ch * p.Hc * p.Wc + vl_crop_offset(p, x, y);
+    const float m = p.mapping[oc];
+    const float df = vl_mul_rn(m, va) - vb;
+    const float c = df > 0.f ? (1.0f - p.lam) * p.inv_Na3 : (df < 0.f ? -(1.0f - p.lam) * p.inv_Na3 : 0.f);
+    l1 = c * m;
+    p.grad_mapping[oc] = c * va;
+  }
+  p.grad[ch * plane + o] = l1 - p.lam * p.inv_N3 * (v[0] + 2.f * va * v[1] + vb * v[2]);
 }

@@ -104,6 +104,25 @@ def crop_window(origH, origW):
     return top, left, H, W
 
 
+def crop_window_checked(origH, origW):
+    """crop_window, refusing an image under 32 pixels in either dimension (its crop is empty; the reference fails there too)."""
+    if origH < 32 or origW < 32:
+        raise ValueError(f"decoupled appearance needs an image of at least 32 x 32 pixels, not {origH} x {origW}")
+    return crop_window(origH, origW)
+
+
+def appearance_mapping(image, network, appearance_embedding):
+    """The appearance network's output for this view, [3, Hc, Wc] on the crop_window of `image` [3, H, W] (train.py:67-84):
+    the network runs on a 1/32 bilinear downsample of the crop and the view's embedding row.  Differentiable with respect to
+    the image, the network and the embedding; gof_loss.view_loss(..., appearance=mapping) takes it."""
+    origH, origW = image.shape[1:]
+    top, left, H, W = crop_window_checked(origH, origW)
+    crop_image = image[:, top:top + H, left:left + W]
+    crop_image_down = F.interpolate(crop_image[None], size=(H // 32, W // 32), mode="bilinear", align_corners=True)[0]
+    emb = appearance_embedding.reshape(-1, 1, 1).expand(-1, H // 32, W // 32)      # the reference: repeat(H/32, W/32, 1).permute(2, 0, 1)
+    return network(torch.cat([crop_image_down, emb], dim=0)[None])[0]
+
+
 def l1_loss_appearance(image, gt_image, network, appearance_embedding, return_transformed_image=False):
     """L1_loss_appearance (train.py:67-88) with the model pieces passed explicitly: `appearance_embedding` is the view's row
     of GaussianModel._appearance_embeddings (64 floats), `network` the AppearanceNetwork."""
@@ -111,9 +130,7 @@ def l1_loss_appearance(image, gt_image, network, appearance_embedding, return_tr
     top, left, H, W = crop_window(origH, origW)
     crop_image = image[:, top:top + H, left:left + W]
     crop_gt_image = gt_image[:, top:top + H, left:left + W]
-    crop_image_down = F.interpolate(crop_image[None], size=(H // 32, W // 32), mode="bilinear", align_corners=True)[0]
-    emb = appearance_embedding.reshape(-1, 1, 1).expand(-1, H // 32, W // 32)      # the reference: repeat(H/32, W/32, 1).permute(2, 0, 1)
-    mapping_image = network(torch.cat([crop_image_down, emb], dim=0)[None])
+    mapping_image = appearance_mapping(image, network, appearance_embedding)[None]
     transformed_image = mapping_image * crop_image
     if not return_transformed_image:
         return torch.abs(transformed_image - crop_gt_image).mean()            # utils/loss_utils.py:17-18 l1_loss

@@ -406,6 +406,17 @@ GOF_API size_t gof_view_loss_scratch_bytes(int W, int H);
 GOF_API int gof_view_loss(int W, int H, const float* render, const float* gt, const float* c2w_R9, float fx, float fy,
                           float lambda_dssim, float lambda_depth_normal, float lambda_distortion, float* terms,
                           float* grad, void* scratch, void* stream);
+/* The same loss with the decoupled-appearance L1 in place of the plain one (train.py:67-88, 157-159): with m = mapping
+ * [3,Hc,Wc] (the appearance network's output, device pointer) on the crop of rows top..top+Hc-1 and columns left..left+Wc-1,
+ * terms[0] = L1_a = mean over the crop of |fl(m * rgb) - gt| (the product rounded to float, as torch's does) and
+ * total = (1-l)*L1_a + l*(1-SSIM) + l_dn*... + l_dist*...; SSIM and the other terms stay on the whole image.
+ * grad [9,H,W] = d total / d render, grad_mapping [3,Hc,Wc] = d total / d mapping; both NULL for values only.
+ * Scratch of gof_view_loss_scratch_bytes(W,H) bytes.  GOF_E_INVALID, before any device work, for gof_view_loss's bad
+ * arguments, a NULL mapping, Hc < 1 or Wc < 1, a crop not inside the image, or only one of grad and grad_mapping. */
+GOF_API int gof_view_loss_appearance(int W, int H, const float* render, const float* gt, const float* c2w_R9, float fx, float fy,
+                                     float lambda_dssim, float lambda_depth_normal, float lambda_distortion, const float* mapping,
+                                     int top, int left, int Hc, int Wc, float* terms, float* grad, float* grad_mapping,
+                                     void* scratch, void* stream);
 
 /* Parameter prologue / epilogue around the rasterizer (SURVEY.md 8(f) rank 2; callers of the rasterizer, staged):
  * activations with the 3D filter (scene/gaussian_model.py:152-194: scales = sqrt(exp(s)^2 + f^2), rotations = normalize(q),
