@@ -30,6 +30,8 @@ import ctypes
 import torch
 import torch.distributed as dist
 
+from diff_gaussian_rasterization import _C
+
 # per-Gaussian parameter gradients that must be reduced across views: 3 + 48 + 1 + 3 + 4 = 59 floats
 _FIELDS = (("dmeans3D", (3,)), ("dsh", None), ("dopacity", (1,)), ("dscales", (3,)), ("drot", (4,)))
 _STAT_FIELDS = (("dens_sum", (3,)), ("dens_max", (2,)))       # SUM region ends where dens_max starts
@@ -62,18 +64,13 @@ class GradBucket:
         if with_stats:
             for name, tail in _STAT_FIELDS:
                 shapes[name] = (self.P,) + tail
-        # Every field starts on a 256-byte boundary: k_preprocess_backward stores dL_drot as float4 and dL_dsh as
-        # 128-bit rows, so the views must be 16-byte aligned for ANY P (after densification P is arbitrary).
-        self._offsets, off = {}, 0
-        for name, shape in shapes.items():
-            self._offsets[name] = (off, shape)
-            off += (int(torch.Size(shape).numel()) + 63) // 64 * 64
+        self._offsets, off = _C._layout(shapes)
         self.n_reduce = off                                                    # floats [0, n_reduce) are reduced over the ranks:
         self.n_sum = self._offsets["dens_max"][0] if with_stats else off      #   [0, n_sum) SUM, [n_sum, n_reduce) MAX
         self._slot = 0
         self.dsh = None
         if self.factored:    # [n_reduce, numel): one record per view = SH_SLOT_HEADER floats (camera centre, degree) + rgb [P,3]
-            self._plane = (self.P + 63) // 64 * 64          # GOF_SH_PLANE(P): the record's three colour planes
+            self._plane = _C._sh_plane(self.P)              # the record's three colour planes
             self._slot = SH_SLOT_HEADER + 3 * self._plane
             off += self._n_views * self._slot
             self.dsh = torch.zeros(self.P, self.M, 3, dtype=dtype, device=device)
@@ -88,7 +85,7 @@ class GradBucket:
         self.exchange = "nccl"
 
     def _make_views(self):
-        views = {name: self.flat[off:off + int(torch.Size(shape).numel())].view(shape) for name, (off, shape) in self._offsets.items()}
+        views = _C._views(self.flat, self._offsets)
         if self.factored:
             rec = self._record(self._view)
             views["sh_hdr"] = rec[:SH_SLOT_HEADER]
@@ -109,7 +106,6 @@ class GradBucket:
     def _expand_sh(self, record_ptrs, means3D):
         """dsh = sum_v w(dir(means3D, camera_v)) (x) rgb_v from the records at `record_ptrs` (device addresses valid in this
         process: local or peer memory), by the library's kernel."""
-        from diff_gaussian_rasterization import _C
         if means3D is None:
             means3D = self.views.get("_means3D")
         if means3D is None:
@@ -145,7 +141,6 @@ class GradBucket:
         """Move the bucket into a CUDA-IPC shareable allocation, map every other rank's bucket into this process (one node,
         NVLink) and switch all_reduce() to the library's peer-memory kernel.  Collective: every rank of `group` must call
         it, before the views are handed to anyone (they are re-created).  Raises if mapping or the self-test fails."""
-        from diff_gaussian_rasterization import _C
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
             return self
         if not self.flat.is_cuda or self.flat.dtype != torch.float32:
@@ -273,7 +268,6 @@ class GradBucket:
         """Move the bucket into a torch symmetric-memory allocation -- every rank's copy bound to ONE NVSwitch multicast object
         -- and switch all_reduce() to the library's multimem kernel (csrc/exchange.cu: k_nvls_allreduce).  Collective; the views
         are re-created.  Raises (on every rank alike) when the fabric / driver offers no multicast or the self-test fails."""
-        from diff_gaussian_rasterization import _C
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
             return self
         if not self.flat.is_cuda or self.flat.dtype != torch.float32:
@@ -485,7 +479,7 @@ def sh_grad_from_views_torch(means3D, records, P, M):
     out = torch.zeros(P, M, 3, dtype=means3D.dtype, device=means3D.device)
     for rec in records:
         cam, degree = rec[:3], int(round(float(rec[3])))
-        plane = (P + 63) // 64 * 64
+        plane = _C._sh_plane(P)
         rgb = rec[SH_SLOT_HEADER:SH_SLOT_HEADER + 3 * plane].view(3, plane)[:, :P].t()
         d = means3D - cam[None, :]
         d = d / torch.linalg.vector_norm(d, dim=1, keepdim=True)

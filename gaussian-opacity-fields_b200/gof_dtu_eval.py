@@ -45,7 +45,7 @@ SORT_LIMIT = 2 ** 30   # points in any one sort (the library's radix passes)
 def _device(device):
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if dev.type != "cuda":
-        raise RuntimeError("gof_dtu_eval: a CUDA device is required (no CPU path)")
+        raise RuntimeError("gof_b200 evaluation: a CUDA device is required (no CPU path)")
     return dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
 
 

@@ -27,10 +27,33 @@ import torch
 import torch.distributed as dist
 
 
+_NO_VIEW = 2 ** 30   # argmin of a point no view lowered below 1
+
+
 def _world(group=None):
     if dist.is_available() and dist.is_initialized():
         return dist.get_rank(group), dist.get_world_size(group)
     return 0, 1
+
+
+def _merge_minimum(alpha_min, argmin, rows, group):
+    """The ranks' view-sharded running minima, merged into the minimum over all views.  alpha_min [N] becomes the global minimum
+    (all_reduce MIN).  With argmin [N] (int32, _NO_VIEW where no view lowered the point below 1), a point's winner is the lowest
+    view index that attains that minimum below 1, the view a serial strict `<` update in view order keeps; a second all_reduce
+    (MIN) agrees on it.  With rows [N,k] as well, a third all_reduce (SUM) gives every rank the winner's rows, and zeros where no
+    view won.  Returns (alpha_min, argmin, rows, won [N] bool), with None for what was not given (won needs argmin)."""
+    local = alpha_min.clone() if argmin is not None else None
+    dist.all_reduce(alpha_min, op=dist.ReduceOp.MIN, group=group)
+    if argmin is None:
+        return alpha_min, None, None, None
+    cand = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
+    argmin = cand.clone()
+    dist.all_reduce(argmin, op=dist.ReduceOp.MIN, group=group)
+    won = argmin < _NO_VIEW
+    if rows is not None:
+        rows = torch.where(((cand == argmin) & won).reshape(-1, 1), rows, torch.zeros_like(rows))
+        dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=group)
+    return alpha_min, argmin, rows, won
 
 
 @torch.no_grad()
@@ -40,7 +63,7 @@ def evaluate_alpha(points, views, integrate_fn, return_color=False, group=None):
     n, dev = points.shape[0], points.device
     final_alpha = torch.ones(n, dtype=torch.float32, device=dev)
     final_color = torch.ones(n, 3, dtype=torch.float32, device=dev) if return_color else None
-    best_view = torch.full((n,), 2 ** 30, dtype=torch.int32, device=dev) if return_color else None
+    best_view = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev) if return_color else None
     views = list(views)
     for vi in range(rank, len(views), world):
         alpha_integrated, color_integrated = integrate_fn(points, views[vi])
@@ -50,17 +73,9 @@ def evaluate_alpha(points, views, integrate_fn, return_color=False, group=None):
             best_view = torch.where(better, torch.full_like(best_view, vi), best_view)
         final_alpha = torch.min(final_alpha, alpha_integrated)
     if world > 1:
-        local_alpha = final_alpha.clone()
-        dist.all_reduce(final_alpha, op=dist.ReduceOp.MIN, group=group)
+        final_alpha, _argmin, contrib, won = _merge_minimum(final_alpha, best_view, final_color, group)
         if return_color:
-            # the winner is the lowest view index whose alpha equals the global minimum (and is < 1, the initial value)
-            cand = torch.where((local_alpha == final_alpha) & (local_alpha < 1.0), best_view, torch.full_like(best_view, 2 ** 30))
-            win = cand.clone()
-            dist.all_reduce(win, op=dist.ReduceOp.MIN, group=group)
-            mine = (cand == win) & (win < 2 ** 30)
-            contrib = torch.where(mine.reshape(-1, 1), final_color, torch.zeros_like(final_color))
-            dist.all_reduce(contrib, op=dist.ReduceOp.SUM, group=group)
-            final_color = torch.where((win < 2 ** 30).reshape(-1, 1), contrib, torch.ones_like(contrib))
+            final_color = torch.where(won.reshape(-1, 1), contrib, torch.ones_like(contrib))
     alpha = 1 - final_alpha
     return (alpha, final_color) if return_color else alpha
 
@@ -95,9 +110,6 @@ def make_integrate_fn(means3D, opacities, scales, rotations, shs, sh_degree, set
             rotations=rotations)
         return alpha_integrated, color_integrated
     return fn
-
-
-_NO_VIEW = 2 ** 30   # argmin of a point no view lowered below 1
 
 
 def _field_inputs(scales, rotations, shs):
@@ -138,16 +150,8 @@ class _OpacityField(torch.autograd.Function):
             dgr._call_native(_C.integrate_gaussians_to_points_min, args, rs.debug, "snapshot_fw.dump", "forward",
                              **({"color_min": color} if return_color else {}))
         if world > 1:
-            # evaluate_alpha's merge: the global minimum, won by the lowest view index that attains it (and is < 1)
-            local = alpha_min.clone()
-            dist.all_reduce(alpha_min, op=dist.ReduceOp.MIN, group=group)
-            cand = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
-            argmin = cand.clone()
-            dist.all_reduce(argmin, op=dist.ReduceOp.MIN, group=group)
-            if return_color:   # the winner's rank contributes its colour, as in evaluate_alpha
-                won = argmin < _NO_VIEW
-                contrib = torch.where(((cand == argmin) & won).reshape(-1, 1), color, torch.zeros_like(color))
-                dist.all_reduce(contrib, op=dist.ReduceOp.SUM, group=group)
+            alpha_min, argmin, contrib, won = _merge_minimum(alpha_min, argmin, color, group)
+            if return_color:
                 color = torch.where(won.reshape(-1, 1), contrib, torch.ones_like(contrib))
         ctx.save_for_backward(points, means3D, opacities, scales, rotations, shs, argmin)
         ctx.views, ctx.settings_for_view, ctx.group = views, settings_for_view, group
@@ -319,16 +323,9 @@ def field_gradient(points, views, integrate_fn, return_color=False, group=None):
     for vi in range(rank, len(views), world):
         integrate_fn.min_update(points, views[vi], vi, alpha_min, argmin, color_min=color, grad_min=grad_min)
     if world > 1:
-        local = alpha_min.clone()
-        dist.all_reduce(alpha_min, op=dist.ReduceOp.MIN, group=group)
-        cand = torch.where((local == alpha_min) & (local < 1.0), argmin, torch.full_like(argmin, _NO_VIEW))
-        argmin = cand.clone()
-        dist.all_reduce(argmin, op=dist.ReduceOp.MIN, group=group)
-        won = argmin < _NO_VIEW
         # the winner's gradient and colour rows in one [N,6] block, summed in a single all-reduce
         rows = torch.cat([grad_min, color], 1) if return_color else grad_min
-        rows = torch.where(((cand == argmin) & won).reshape(-1, 1), rows, torch.zeros_like(rows))
-        dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=group)
+        alpha_min, argmin, rows, won = _merge_minimum(alpha_min, argmin, rows, group)
         grad_min = rows[:, :3]
         if return_color:
             color = torch.where(won.reshape(-1, 1), rows[:, 3:], torch.ones_like(color))

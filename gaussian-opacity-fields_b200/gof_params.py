@@ -28,12 +28,7 @@ _lib.gof_adam_step.argtypes = [ctypes.c_size_t, _v, _v, _v, _v, ctypes.c_double,
 def _f32(t):
     if not t.is_cuda or t.dtype != torch.float32:
         raise RuntimeError("gof_b200 params: CUDA float32 tensors required (no CPU path)")
-    # the kernels move rotations as float4: a contiguous view at an odd storage offset (a parameter sliced out of a flat
-    # buffer) is copied to a fresh, aligned allocation, as the rasterizer binding does (_C._c)
-    t = t.contiguous()
-    if t.numel() and (t.data_ptr() & 15):
-        t = t.clone(memory_format=torch.contiguous_format)
-    return t
+    return _C._c(t)     # the kernels move rotations as float4
 
 
 class _Activate(torch.autograd.Function):

@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from diff_gaussian_rasterization import _C
-from gof_dtu_eval import read_ply, write_vis_ply
+from gof_dtu_eval import _device, _points, _scratch, _timer, read_ply, write_vis_ply
 
 _lib = _C._lib
 _fp = ctypes.c_void_p
@@ -45,7 +45,6 @@ for _name, _res, _args in (
     getattr(_lib, _name).restype = _res
     getattr(_lib, _name).argtypes = _args
 
-SORT_LIMIT = 2 ** 30   # points in any one sort (the library's radix passes)
 MAX_POINT_NUMBER = 4e6                       # registration.py:41
 MAX_POLYGON = 3072                           # polygon vertices the crop kernel stages in shared memory
 # config.py: scenes_tau_dict
@@ -54,28 +53,6 @@ SCENES_TAU = {"Barn": 0.01, "Caterpillar": 0.005, "Church": 0.025, "Courthouse":
 # ICPConvergenceCriteria(1e-6, max_itr) binds positionally in Open3D 0.10 to (relative_fitness, relative_rmse); max_iteration
 # keeps its default of 30 (DESIGN section 4.7)
 ICP_CRITERIA = {"relative_fitness": 1e-6, "relative_rmse": 20.0, "max_iteration": 30}
-
-
-def _device(device):
-    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-    if dev.type != "cuda":
-        raise RuntimeError("gof_tnt_eval: a CUDA device is required (no CPU path)")
-    return dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
-
-
-def _points(x, name, dev):
-    t = torch.as_tensor(x).to(dev, torch.float64)
-    if t.dim() != 2 or t.shape[1] != 3:
-        raise ValueError(f"{name}: expected [n, 3] coordinates, got shape {tuple(t.shape)}")
-    if t.shape[0] >= SORT_LIMIT:
-        raise ValueError(f"{name}: {t.shape[0]} points; at most 2^30 - 1 are supported (the limit of the library's radix sort)")
-    if t.numel() and not bool(torch.isfinite(t).all()):
-        raise ValueError(f"{name}: non-finite coordinates")
-    return t.contiguous()
-
-
-def _scratch(nbytes, dev):
-    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
 
 
 def _mat(T):
@@ -127,7 +104,7 @@ def crop(points, volume, transform=None, return_index=False):
     """SelectionPolygonVolume.crop_point_cloud, after `transform` (4x4) when given: the kept points in input order [k, 3]
     (and their input indices, int64)."""
     dev = points.device
-    P = _points(points, "crop points", dev)
+    P = _points(points, "crop points", dev, allow_empty=True)
     n = int(P.shape[0])
     poly = np.ascontiguousarray(volume["polygon_uv"], np.float64)
     out = torch.empty((n, 3), dtype=torch.float64, device=dev)
@@ -148,7 +125,7 @@ def voxel_down_sample(points, voxel):
     """PointCloud.voxel_down_sample: per occupied voxel the mean of its points (summed in input order), in ascending (x, y, z)
     voxel order."""
     dev = points.device
-    P = _points(points, "voxel_down_sample points", dev)
+    P = _points(points, "voxel_down_sample points", dev, allow_empty=True)
     n = int(P.shape[0])
     out = torch.empty((n, 3), dtype=torch.float64, device=dev)
     k = ctypes.c_int64(0)
@@ -173,7 +150,7 @@ class NNTree:
 
     def __init__(self, ref):
         self.dev = ref.device
-        self.ref = _points(ref, "nn reference", self.dev)
+        self.ref = _points(ref, "nn reference", self.dev, allow_empty=True)
         self.n = int(self.ref.shape[0])
         if self.n == 0:
             raise ValueError("nn reference: the cloud is empty")
@@ -183,7 +160,7 @@ class NNTree:
         self._qscratch, self._qn = None, -1
 
     def query(self, q, r2=math.inf, reuse_order=False):
-        Q = _points(q, "nn query", self.dev)
+        Q = _points(q, "nn query", self.dev, allow_empty=True)
         m = int(Q.shape[0])
         idx = torch.empty(m, dtype=torch.int32, device=self.dev)
         d2 = torch.empty(m, dtype=torch.float64, device=self.dev)
@@ -246,8 +223,8 @@ def registration_icp(source, target, threshold, relative_fitness=1e-6, relative_
     Returns dict(transformation, iterations, fitness, inlier_rmse).  trace (a list) gets (moving, idx, d2) of every
     evaluation, as device tensors."""
     dev = source.device
-    moving = _points(source, "icp source", dev).clone()
-    tgt = _points(target, "icp target", dev)
+    moving = _points(source, "icp source", dev, allow_empty=True).clone()
+    tgt = _points(target, "icp target", dev, allow_empty=True)
     n = int(moving.shape[0])
     r2 = float(np.float32(threshold * threshold))
     tree = NNTree(tgt) if tgt.shape[0] and n else None
@@ -394,17 +371,6 @@ def reconstruction_cloud(vertices, faces):
     return torch.cat([V, ((V[F[:, 0]] + V[F[:, 1]]) + V[F[:, 2]]) / three], 0)
 
 
-def _timer(enabled):
-    marks = []
-
-    def mark(name):
-        if enabled:
-            ev = torch.cuda.Event(enable_timing=True)
-            ev.record()
-            marks.append((name, ev))
-    return marks, mark
-
-
 def evaluate(vertices, faces, gt, traj, colmap_traj, gt_trans, volume, dTau, seed=0, max_points=MAX_POINT_NUMBER, device=None,
              timing=False):
     """run.py:58-184 on arrays.  vertices [V,3] / faces [F,3] of the mesh; gt [m,3]; traj and colmap_traj [k,4,4] poses; gt_trans
@@ -417,10 +383,10 @@ def evaluate(vertices, faces, gt, traj, colmap_traj, gt_trans, volume, dTau, see
     out = {}
     with torch.cuda.device(dev):
         mark("start")
-        V = _points(vertices, "mesh vertices", dev)
+        V = _points(vertices, "mesh vertices", dev, allow_empty=True)
         F = torch.as_tensor(np.asarray(faces, np.int64) if not torch.is_tensor(faces) else faces).to(dev).reshape(-1, 3)
         pcd = reconstruction_cloud(V, F)
-        gt_t = _points(gt, "gt", dev)
+        gt_t = _points(gt, "gt", dev, allow_empty=True)
         mark("upload")
         traj = np.asarray(traj, np.float64).reshape(-1, 4, 4)
         col = np.asarray(colmap_traj, np.float64).reshape(-1, 4, 4)
