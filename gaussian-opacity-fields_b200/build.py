@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "diff_gaussian_rasterization")
 LIB = os.path.join(OUT_DIR, "libgof_b200.so")
-SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "integrate.cu", "tetmesh.cu", "tsdf.cu", "knn.cu", "dtu_eval.cu", "tnt_eval.cu", "exchange.cu", "view_loss.cu", "param_ops.cu", "filter3d.cu", "tetra_points.cu", "densify.cu", "conv_wgrad.cu", "sh_views.cu"]
+SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "integrate.cu", "tetmesh.cu", "tsdf.cu", "knn.cu", "dtu_eval.cu", "tnt_eval.cu", "exchange.cu", "view_loss.cu", "param_ops.cu", "filter3d.cu", "tetra_points.cu", "field_grid.cu", "densify.cu", "conv_wgrad.cu", "sh_views.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",

@@ -13,37 +13,16 @@
 //             only updated voxels are written; the depth and colour images are gathers that stay in L2
 //   extract   one CTA per table block: its +1 neighbour blocks are found once by binary search; meshed cubes mark the
 //             edges they use at the edges' owner voxels; per-block vertex and face counts are scanned; the emit kernels
-//             re-derive each voxel's offset with a block scan and write vertices and faces in canonical order
+//             re-derive each voxel's offset with a block scan and write vertices and faces in canonical order; the same
+//             kernels, instantiated for one value plane without weights, mesh the opacity field's lattice (DESIGN 4.15)
 #include "gof_common.cuh"
 #include "mc_table.cuh"
+#include "voxel_blocks.cuh"
 
 namespace {
 
-constexpr int THREADS = 256;
 constexpr int TOUCH_STRIDE = 4;
-constexpr int KEY_BITS = 21;
-constexpr int64_t KEY_BIAS = (int64_t)1 << 20;
 constexpr int PLANES = 5;   // tsdf, weight, r, g, b
-
-__device__ __forceinline__ int64_t pack_key(int bx, int by, int bz) {
-  return (((int64_t)bz + KEY_BIAS) << (2 * KEY_BITS)) | (((int64_t)by + KEY_BIAS) << KEY_BITS) | ((int64_t)bx + KEY_BIAS);
-}
-__device__ __forceinline__ void unpack_key(int64_t k, int* b) {
-  const int64_t m = ((int64_t)1 << KEY_BITS) - 1;
-  b[0] = (int)((k & m) - KEY_BIAS);
-  b[1] = (int)(((k >> KEY_BITS) & m) - KEY_BIAS);
-  b[2] = (int)((k >> (2 * KEY_BITS)) - KEY_BIAS);
-}
-
-// position of the first key >= k in the sorted list
-__device__ __forceinline__ int64_t lower_bound(const int64_t* __restrict__ keys, int64_t n, int64_t k) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (keys[mid] < k) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
 
 struct Cam {
   int W, H;
@@ -169,16 +148,6 @@ __global__ void __launch_bounds__(THREADS) k_touch_emit(int npix, const float* _
       }
 }
 
-// ord: the instances in key order; head / uid: the runs of equal keys along it (gof_key_runs_u32)
-__global__ void __launch_bounds__(THREADS) k_key_emit(size_t n, const uint32_t* __restrict__ lo_w, const uint32_t* __restrict__ hi_w,
-                                                     const uint32_t* __restrict__ ord, const uint32_t* __restrict__ head,
-                                                     const uint32_t* __restrict__ uid, int64_t* __restrict__ keys) {
-  const size_t j = (size_t)blockIdx.x * THREADS + threadIdx.x;
-  if (j >= n || !head[j]) return;
-  const uint32_t i = ord[j];
-  keys[uid[j]] = (int64_t)(((uint64_t)hi_w[i] << 32) | lo_w[i]);
-}
-
 // ---- activate ----------------------------------------------------------------------------------------------------
 
 struct ActLayout { size_t header, pos, flag, off, scan_tmp, bytes; };
@@ -284,6 +253,14 @@ __global__ void __launch_bounds__(THREADS) k_integrate(const float* __restrict__
 }
 
 // ---- extract -----------------------------------------------------------------------------------------------------
+//
+// One set of kernels serves two value layouts, chosen at compile time:
+//   FIELD = false  the TSDF pool [slot][tsdf, weight, r, g, b][B^3] behind the table's slots; a cube is meshed iff its eight
+//                  corners exist with weight > theta; vertices are interpolated on their edge, with colours
+//   FIELD = true   the opacity field's lattice (field_grid.cu, DESIGN section 4.15): one value plane [n][B^3] in table order
+//                  (slot = table position), every voxel of a listed block present with weight 1 and theta 0, so a cube is
+//                  meshed iff its eight corners exist; each vertex is returned as its edge -- the two lattice points and
+//                  their values -- for the bisection
 
 struct MeshLayout { size_t header, nbr, marks, vid, bv, bf, bv_off, bf_off, scan_tmp, bytes; };
 // totals of the per-block counts in 64 bits (checked against the 32-bit ids) and as the scans report them
@@ -306,9 +283,10 @@ static MeshLayout mesh_layout(size_t n, int B) {
 struct MeshArgs {
   int64_t n;
   const int64_t* keys;
-  const int32_t* slots;
+  const int32_t* slots;  // FIELD: unused (slot = table position)
   const float* pool;
-  Par p;
+  int B;
+  float s;
   float theta;
   int32_t* nbr;          // [n][8] table position of the block at corner offset c (c = 0: itself), -1 if absent
   uint8_t* marks;        // [n][B^3] bit a: the voxel's edge along axis a carries a vertex
@@ -316,9 +294,15 @@ struct MeshArgs {
   uint32_t *bv, *bf;     // per block vertex / face counts
   uint32_t *bv_off, *bf_off;   // their exclusive scans: the block's first vertex / face
   unsigned long long* totals;  // [2] vertex and face totals
-  float *vertices, *colors;
+  float *vertices, *colors;    // !FIELD
+  float *edge_points, *edge_values;   // FIELD: [V][2][3] the owner's and the far end's lattice points, [V][2] their values
   int64_t* faces;
 };
+
+template <bool FIELD>
+__device__ __forceinline__ const float* block_values(const MeshArgs& a, int slot, size_t n3) {
+  return a.pool + (size_t)slot * (FIELD ? 1 : PLANES) * n3;
+}
 
 // voxel (x, y, z) in 0..B of this block (the +1 layer lies in a neighbour): returns which neighbour (its corner offset c,
 // 0 = this block) and its lin index there
@@ -328,6 +312,7 @@ __device__ __forceinline__ int locate(int B, int x, int y, int z, int* lin) {
   return c;
 }
 
+template <bool FIELD>
 __device__ __forceinline__ void load_neighbours(const MeshArgs& a, int* s_nbr, int* s_slot, bool find) {
   const int64_t p = blockIdx.x;
   if (threadIdx.x < 8) {
@@ -349,14 +334,16 @@ __device__ __forceinline__ void load_neighbours(const MeshArgs& a, int* s_nbr, i
       q = a.nbr[8 * p + c];
     }
     s_nbr[c] = q;
-    s_slot[c] = q >= 0 ? a.slots[q] : -1;
+    s_slot[c] = q >= 0 ? (FIELD ? q : a.slots[q]) : -1;
   }
   __syncthreads();
 }
 
-// cube at voxel (x, y, z) of this block: true if meshed (all 8 corners exist with weight > theta); *code: bit c = corner c negative
+// cube at voxel (x, y, z) of this block: true if meshed (all 8 corners exist, with weight > theta in the TSDF layout);
+// *code: bit c = corner c negative
+template <bool FIELD>
 __device__ __forceinline__ bool cube_code(const MeshArgs& a, const int* s_nbr, const int* s_slot, int x, int y, int z, uint32_t* code) {
-  const int B = a.p.B;
+  const int B = a.B;
   const size_t n3 = (size_t)B * B * B;
   uint32_t cd = 0;
 #pragma unroll
@@ -364,24 +351,25 @@ __device__ __forceinline__ bool cube_code(const MeshArgs& a, const int* s_nbr, c
     int lin;
     const int nb = locate(B, x + (c & 1), y + ((c >> 1) & 1), z + ((c >> 2) & 1), &lin);
     if (s_nbr[nb] < 0) return false;
-    const float* blk = a.pool + (size_t)s_slot[nb] * PLANES * n3;
-    if (!(__ldg(blk + n3 + lin) > a.theta)) return false;
+    const float* blk = block_values<FIELD>(a, s_slot[nb], n3);
+    if (!FIELD && !(__ldg(blk + n3 + lin) > a.theta)) return false;
     cd |= (__ldg(blk + lin) < 0.f ? 1u : 0u) << c;
   }
   *code = cd;
   return true;
 }
 
+template <bool FIELD>
 __global__ void __launch_bounds__(THREADS) k_mc_mark(const MeshArgs a) {
   __shared__ int s_nbr[8], s_slot[8];
-  load_neighbours(a, s_nbr, s_slot, true);
-  const int B = a.p.B;
+  load_neighbours<FIELD>(a, s_nbr, s_slot, true);
+  const int B = a.B;
   const int n3 = B * B * B;
   uint32_t nf = 0;
   for (int lin = threadIdx.x; lin < n3; lin += THREADS) {
     const int x = lin % B, y = (lin / B) % B, z = lin / (B * B);
     uint32_t code;
-    if (!cube_code(a, s_nbr, s_slot, x, y, z, &code)) continue;
+    if (!cube_code<FIELD>(a, s_nbr, s_slot, x, y, z, &code)) continue;
     nf += c_mc_ntri[code];
 #pragma unroll
     for (int e = 0; e < 12; ++e) {
@@ -402,7 +390,7 @@ __global__ void __launch_bounds__(THREADS) k_mc_mark(const MeshArgs a) {
 }
 
 __global__ void __launch_bounds__(THREADS) k_mc_vcount(const MeshArgs a) {
-  const int B = a.p.B;
+  const int B = a.B;
   const int n3 = B * B * B;
   const uint8_t* m = a.marks + (size_t)blockIdx.x * n3;
   uint32_t nv = 0;
@@ -422,10 +410,11 @@ __device__ __forceinline__ void thread_run(int n3, int* l0, int* l1) {
   *l1 = min(*l0 + per, n3);
 }
 
+template <bool FIELD>
 __global__ void __launch_bounds__(THREADS) k_mc_emit_vertices(const MeshArgs a) {
   __shared__ int s_nbr[8], s_slot[8];
-  load_neighbours(a, s_nbr, s_slot, false);
-  const int B = a.p.B;
+  load_neighbours<FIELD>(a, s_nbr, s_slot, false);
+  const int B = a.B;
   const int n3 = B * B * B;
   const size_t p = blockIdx.x;
   const uint8_t* m = a.marks + p * n3;
@@ -442,33 +431,46 @@ __global__ void __launch_bounds__(THREADS) k_mc_emit_vertices(const MeshArgs a) 
     a.vid[p * n3 + lin] = id;
     if (!mk) continue;
     const int li[3] = {lin % B, (lin / B) % B, lin / (B * B)};
-    const float* bo = a.pool + (size_t)s_slot[0] * PLANES * n3;
+    const float* bo = block_values<FIELD>(a, s_slot[0], n3);
     const float to = bo[lin];
     for (int ax = 0; ax < 3; ++ax) {
       if (!((mk >> ax) & 1u)) continue;
       int el;
       const int ec = locate(B, li[0] + (ax == 0), li[1] + (ax == 1), li[2] + (ax == 2), &el);
-      const float* be = a.pool + (size_t)s_slot[ec] * PLANES * n3;
+      const float* be = block_values<FIELD>(a, s_slot[ec], n3);
       const float te = be[el];
-      const float r = __fdiv_rn(__fsub_rn(0.f, to), __fsub_rn(te, to));
+      if (FIELD) {
+        // the two lattice points exactly as gof_field_grid_points computes them, and their values
 #pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const float g = __int2float_rn(b[k] * B + li[k]);
-        a.vertices[3 * (size_t)id + k] = __fmul_rn(k == ax ? __fadd_rn(g, r) : g, a.p.s);
+        for (int k = 0; k < 3; ++k) {
+          const int g = b[k] * B + li[k];
+          a.edge_points[6 * (size_t)id + k] = __fmul_rn(__int2float_rn(g), a.s);
+          a.edge_points[6 * (size_t)id + 3 + k] = __fmul_rn(__int2float_rn(k == ax ? g + 1 : g), a.s);
+        }
+        a.edge_values[2 * (size_t)id] = to;
+        a.edge_values[2 * (size_t)id + 1] = te;
+      } else {
+        const float r = __fdiv_rn(__fsub_rn(0.f, to), __fsub_rn(te, to));
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const float g = __int2float_rn(b[k] * B + li[k]);
+          a.vertices[3 * (size_t)id + k] = __fmul_rn(k == ax ? __fadd_rn(g, r) : g, a.s);
+        }
+        const float one_r = __fsub_rn(1.f, r);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch)
+          a.colors[3 * (size_t)id + ch] = __fadd_rn(__fmul_rn(one_r, bo[(size_t)(2 + ch) * n3 + lin]), __fmul_rn(r, be[(size_t)(2 + ch) * n3 + el]));
       }
-      const float one_r = __fsub_rn(1.f, r);
-#pragma unroll
-      for (int ch = 0; ch < 3; ++ch)
-        a.colors[3 * (size_t)id + ch] = __fadd_rn(__fmul_rn(one_r, bo[(size_t)(2 + ch) * n3 + lin]), __fmul_rn(r, be[(size_t)(2 + ch) * n3 + el]));
       ++id;
     }
   }
 }
 
+template <bool FIELD>
 __global__ void __launch_bounds__(THREADS) k_mc_emit_faces(const MeshArgs a) {
   __shared__ int s_nbr[8], s_slot[8];
-  load_neighbours(a, s_nbr, s_slot, false);
-  const int B = a.p.B;
+  load_neighbours<FIELD>(a, s_nbr, s_slot, false);
+  const int B = a.B;
   const int n3 = B * B * B;
   const size_t p = blockIdx.x;
   int l0, l1;
@@ -476,14 +478,14 @@ __global__ void __launch_bounds__(THREADS) k_mc_emit_faces(const MeshArgs a) {
   uint32_t cnt = 0;
   for (int lin = l0; lin < l1; ++lin) {
     uint32_t code;
-    if (cube_code(a, s_nbr, s_slot, lin % B, (lin / B) % B, lin / (B * B), &code)) cnt += c_mc_ntri[code];
+    if (cube_code<FIELD>(a, s_nbr, s_slot, lin % B, (lin / B) % B, lin / (B * B), &code)) cnt += c_mc_ntri[code];
   }
   uint32_t total;
   size_t f = a.bf_off[p] + block_excl_scan(cnt, &total);
   for (int lin = l0; lin < l1; ++lin) {
     const int x = lin % B, y = (lin / B) % B, z = lin / (B * B);
     uint32_t code;
-    if (!cube_code(a, s_nbr, s_slot, x, y, z, &code)) continue;
+    if (!cube_code<FIELD>(a, s_nbr, s_slot, x, y, z, &code)) continue;
     const int nt = c_mc_ntri[code];
     for (int k = 0; k < 3 * nt; ++k) {
       const int e = c_mc_tri[code][k];
@@ -498,15 +500,75 @@ __global__ void __launch_bounds__(THREADS) k_mc_emit_faces(const MeshArgs a) {
   }
 }
 
-static bool mesh_args(const gof_tsdf_params_t* params, int64_t n, const int64_t* keys, const int32_t* slots, const float* pool,
-                      float theta, char* S, const MeshLayout& L, MeshArgs* a) {
-  a->n = n; a->keys = keys; a->slots = slots; a->pool = pool; a->p = make_par(params); a->theta = theta;
+static void mesh_args(int64_t n, const int64_t* keys, const int32_t* slots, const float* pool, int B, float s, float theta, char* S,
+                      const MeshLayout& L, MeshArgs* a) {
+  a->n = n; a->keys = keys; a->slots = slots; a->pool = pool; a->B = B; a->s = s; a->theta = theta;
   a->nbr = (int32_t*)(S + L.nbr); a->marks = (uint8_t*)(S + L.marks); a->vid = (uint32_t*)(S + L.vid);
   a->bv = (uint32_t*)(S + L.bv); a->bf = (uint32_t*)(S + L.bf);
   a->bv_off = (uint32_t*)(S + L.bv_off); a->bf_off = (uint32_t*)(S + L.bf_off);
   a->totals = (unsigned long long*)(S + L.header);
-  a->vertices = nullptr; a->colors = nullptr; a->faces = nullptr;
-  return true;
+  a->vertices = nullptr; a->colors = nullptr; a->edge_points = nullptr; a->edge_values = nullptr; a->faces = nullptr;
+}
+
+// The count phase of either layout: marks, per-block counts and their scans; the totals, checked against the u32 ids.
+template <bool FIELD>
+static int mc_count(int64_t num_table, const int64_t* keys, const int32_t* slots, const float* pool, int B, float s, float theta,
+                    gof_alloc_fn scratch_alloc, void* scratch_user, int64_t* num_vertices_out, int64_t* num_faces_out, const char* who,
+                    cudaStream_t st) {
+  const size_t n3 = (size_t)B * B * B;
+  const MeshLayout L = mesh_layout((size_t)num_table, B);
+  char* S = (char*)scratch_alloc(scratch_user, L.bytes);
+  if (!S) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
+  MeshArgs a;
+  mesh_args(num_table, keys, slots, pool, B, s, theta, S, L, &a);
+  MeshHeader* hd = (MeshHeader*)(S + L.header);
+  GOF_CUDA_OK(cudaMemsetAsync(hd, 0, sizeof(MeshHeader), st));
+  GOF_CUDA_OK(cudaMemsetAsync(a.marks, 0, (size_t)num_table * n3, st));
+  const unsigned g = (unsigned)num_table;
+  GOF_LAUNCH(FIELD ? "field_mc_mark" : "tsdf_mc_mark", st, k_mc_mark<FIELD><<<g, THREADS, 0, st>>>(a));
+  GOF_LAUNCH_CHECK(false, st);
+  GOF_LAUNCH(FIELD ? "field_mc_vcount" : "tsdf_mc_vcount", st, k_mc_vcount<<<g, THREADS, 0, st>>>(a));
+  GOF_LAUNCH_CHECK(false, st);
+  uint32_t* tmp = (uint32_t*)(S + L.scan_tmp);
+  int rc;
+  if ((rc = gof_exclusive_scan_u32(a.bv, a.bv_off, tmp, &hd->nv, (size_t)num_table, false, st)) != GOF_OK) return rc;
+  if ((rc = gof_exclusive_scan_u32(a.bf, a.bf_off, tmp, &hd->nf, (size_t)num_table, false, st)) != GOF_OK) return rc;
+  MeshHeader h;
+  if ((rc = gof_read_back(&h, hd, sizeof(h), st)) != GOF_OK) return rc;
+  // vertex ids live in u32 (per-voxel first ids, scanned offsets): the mesh must have fewer than 2^32 vertices and faces
+  if (h.nv64 >= (1ull << 32) || h.nf64 >= (1ull << 32)) {
+    gof_set_error("%s: %llu vertices / %llu faces; at most 2^32 - 1 of each are supported", who, h.nv64, h.nf64);
+    return GOF_E_INVALID;
+  }
+  *num_vertices_out = (int64_t)h.nv64; *num_faces_out = (int64_t)h.nf64;
+  return GOF_OK;
+}
+
+// The emit phase: `out` carries the caller's output pointers (vertices / colors or edge_points / edge_values, and faces).
+template <bool FIELD>
+static int mc_emit(int64_t num_table, const int64_t* keys, const int32_t* slots, const float* pool, int B, float s, float theta,
+                   void* scratch, int64_t num_vertices, int64_t num_faces, const MeshArgs& out, const char* who, cudaStream_t st) {
+  const MeshLayout L = mesh_layout((size_t)num_table, B);
+  char* S = (char*)scratch;
+  MeshHeader h;
+  int rc;
+  if ((rc = gof_read_back(&h, S + L.header, sizeof(h), st)) != GOF_OK) return rc;
+  if ((int64_t)h.nv64 != num_vertices || (int64_t)h.nf64 != num_faces) {
+    gof_set_error("%s: sizes do not match the count phase", who);
+    return GOF_E_INVALID;
+  }
+  MeshArgs a;
+  mesh_args(num_table, keys, slots, pool, B, s, theta, S, L, &a);
+  a.vertices = out.vertices; a.colors = out.colors; a.edge_points = out.edge_points; a.edge_values = out.edge_values;
+  a.faces = out.faces;
+  const unsigned g = (unsigned)num_table;
+  GOF_LAUNCH(FIELD ? "field_mc_vertices" : "tsdf_mc_vertices", st, k_mc_emit_vertices<FIELD><<<g, THREADS, 0, st>>>(a));
+  GOF_LAUNCH_CHECK(false, st);
+  if (num_faces > 0) {
+    GOF_LAUNCH(FIELD ? "field_mc_faces" : "tsdf_mc_faces", st, k_mc_emit_faces<FIELD><<<g, THREADS, 0, st>>>(a));
+    GOF_LAUNCH_CHECK(false, st);
+  }
+  return GOF_OK;
 }
 
 }  // namespace
@@ -660,33 +722,9 @@ int gof_tsdf_extract_count(const gof_tsdf_params_t* params, int64_t num_table, c
   if ((rc = check_params(params, "tsdf_extract_count")) != GOF_OK) return rc;
   if (num_table <= 0) return GOF_OK;
   if (!table_keys || !table_slots || !pool) { gof_set_error("tsdf_extract_count: NULL input"); return GOF_E_INVALID; }
-  const size_t n3 = (size_t)params->block_resolution * params->block_resolution * params->block_resolution;
-  cudaStream_t st = (cudaStream_t)stream;
-  const MeshLayout L = mesh_layout((size_t)num_table, params->block_resolution);
-  char* S = (char*)scratch_alloc(scratch_user, L.bytes);
-  if (!S) { gof_set_error("scratch allocator returned NULL"); return GOF_E_ALLOC; }
-  MeshArgs a;
-  mesh_args(params, num_table, table_keys, table_slots, pool, weight_threshold, S, L, &a);
-  MeshHeader* hd = (MeshHeader*)(S + L.header);
-  GOF_CUDA_OK(cudaMemsetAsync(hd, 0, sizeof(MeshHeader), st));
-  GOF_CUDA_OK(cudaMemsetAsync(a.marks, 0, (size_t)num_table * n3, st));
-  const unsigned g = (unsigned)num_table;
-  GOF_LAUNCH("tsdf_mc_mark", st, k_mc_mark<<<g, THREADS, 0, st>>>(a));
-  GOF_LAUNCH_CHECK(false, st);
-  GOF_LAUNCH("tsdf_mc_vcount", st, k_mc_vcount<<<g, THREADS, 0, st>>>(a));
-  GOF_LAUNCH_CHECK(false, st);
-  uint32_t* tmp = (uint32_t*)(S + L.scan_tmp);
-  if ((rc = gof_exclusive_scan_u32(a.bv, a.bv_off, tmp, &hd->nv, (size_t)num_table, false, st)) != GOF_OK) return rc;
-  if ((rc = gof_exclusive_scan_u32(a.bf, a.bf_off, tmp, &hd->nf, (size_t)num_table, false, st)) != GOF_OK) return rc;
-  MeshHeader h;
-  if ((rc = gof_read_back(&h, hd, sizeof(h), st)) != GOF_OK) return rc;
-  // vertex ids live in u32 (per-voxel first ids, scanned offsets): the mesh must have fewer than 2^32 vertices and faces
-  if (h.nv64 >= (1ull << 32) || h.nf64 >= (1ull << 32)) {
-    gof_set_error("tsdf_extract_count: %llu vertices / %llu faces; at most 2^32 - 1 of each are supported", h.nv64, h.nf64);
-    return GOF_E_INVALID;
-  }
-  *num_vertices_out = (int64_t)h.nv64; *num_faces_out = (int64_t)h.nf64;
-  return GOF_OK;
+  const Par p = make_par(params);
+  return mc_count<false>(num_table, table_keys, table_slots, pool, p.B, p.s, weight_threshold, scratch_alloc, scratch_user,
+                         num_vertices_out, num_faces_out, "tsdf_extract_count", (cudaStream_t)stream);
 }
 
 extern "C" __attribute__((visibility("default")))
@@ -700,24 +738,44 @@ int gof_tsdf_extract_emit(const gof_tsdf_params_t* params, int64_t num_table, co
     gof_set_error("tsdf_extract_emit: NULL argument");
     return GOF_E_INVALID;
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  const MeshLayout L = mesh_layout((size_t)num_table, params->block_resolution);
-  char* S = (char*)scratch;
-  MeshHeader h;
-  if ((rc = gof_read_back(&h, S + L.header, sizeof(h), st)) != GOF_OK) return rc;
-  if ((int64_t)h.nv64 != num_vertices || (int64_t)h.nf64 != num_faces) {
-    gof_set_error("tsdf_extract_emit: sizes do not match the count phase");
+  const Par p = make_par(params);
+  MeshArgs out{};
+  out.vertices = vertices; out.colors = colors; out.faces = faces;
+  return mc_emit<false>(num_table, table_keys, table_slots, pool, p.B, p.s, weight_threshold, scratch, num_vertices, num_faces, out,
+                        "tsdf_extract_emit", (cudaStream_t)stream);
+}
+
+// ---- marching cubes of the opacity field's lattice (DESIGN section 4.15; the lattice itself is field_grid.cu's) ---------
+
+extern "C" __attribute__((visibility("default")))
+int gof_field_grid_extract_count(const gof_field_grid_params_t* params, int64_t num_blocks, const int64_t* keys, const float* values,
+                                 gof_alloc_fn scratch_alloc, void* scratch_user, int64_t* num_vertices_out, int64_t* num_faces_out,
+                                 void* stream) {
+  if (!num_vertices_out || !num_faces_out || !scratch_alloc) { gof_set_error("field_grid_extract_count: NULL argument"); return GOF_E_INVALID; }
+  *num_vertices_out = 0; *num_faces_out = 0;
+  int rc;
+  if ((rc = field_grid_check_params(params, "field_grid_extract_count")) != GOF_OK) return rc;
+  if ((rc = field_grid_check_points(params, num_blocks, "field_grid_extract_count")) != GOF_OK) return rc;
+  if (num_blocks == 0) return GOF_OK;
+  if (!keys || !values) { gof_set_error("field_grid_extract_count: NULL input"); return GOF_E_INVALID; }
+  return mc_count<true>(num_blocks, keys, nullptr, values, params->block_resolution, params->voxel_size, 0.f, scratch_alloc, scratch_user,
+                        num_vertices_out, num_faces_out, "field_grid_extract_count", (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default")))
+int gof_field_grid_extract_emit(const gof_field_grid_params_t* params, int64_t num_blocks, const int64_t* keys, const float* values,
+                                void* scratch, int64_t num_vertices, int64_t num_faces, float* edge_points, float* edge_values,
+                                int64_t* faces, void* stream) {
+  int rc;
+  if ((rc = field_grid_check_params(params, "field_grid_extract_emit")) != GOF_OK) return rc;
+  if ((rc = field_grid_check_points(params, num_blocks, "field_grid_extract_emit")) != GOF_OK) return rc;
+  if (num_blocks == 0 || (num_vertices == 0 && num_faces == 0)) return GOF_OK;
+  if (!scratch || !keys || !values || (num_vertices > 0 && (!edge_points || !edge_values)) || (num_faces > 0 && !faces)) {
+    gof_set_error("field_grid_extract_emit: NULL argument");
     return GOF_E_INVALID;
   }
-  MeshArgs a;
-  mesh_args(params, num_table, table_keys, table_slots, pool, weight_threshold, S, L, &a);
-  a.vertices = vertices; a.colors = colors; a.faces = faces;
-  const unsigned g = (unsigned)num_table;
-  GOF_LAUNCH("tsdf_mc_vertices", st, k_mc_emit_vertices<<<g, THREADS, 0, st>>>(a));
-  GOF_LAUNCH_CHECK(false, st);
-  if (num_faces > 0) {
-    GOF_LAUNCH("tsdf_mc_faces", st, k_mc_emit_faces<<<g, THREADS, 0, st>>>(a));
-    GOF_LAUNCH_CHECK(false, st);
-  }
-  return GOF_OK;
+  MeshArgs out{};
+  out.edge_points = edge_points; out.edge_values = edge_values; out.faces = faces;
+  return mc_emit<true>(num_blocks, keys, nullptr, values, params->block_resolution, params->voxel_size, 0.f, scratch, num_vertices,
+                       num_faces, out, "field_grid_extract_emit", (cudaStream_t)stream);
 }

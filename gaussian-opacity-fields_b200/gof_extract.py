@@ -20,6 +20,8 @@ reference's extract_mesh.py, restated with view sharding over the GPUs of one bo
 * get_tetra_points  == GaussianModel.get_tetra_points (scene/gaussian_model.py:433-463), get_frustum_mask == its module-level
                        get_frustum_mask (:31-72): one CUDA pass (csrc/tetra_points.cu, DESIGN §4.8) in memory linear in the
                        points, where the reference builds ~40 bytes per (view, point).
+* extract_level_set_grid -- the same level set without tetrahedra: the field sampled on a sparse voxel-block lattice around
+                       the Gaussians, marching cubes, the same bisection, colours and normals (csrc/field_grid.cu, DESIGN §4.15).
 """
 import ctypes
 
@@ -529,3 +531,206 @@ def get_frustum_mask(points, cameras, near=0.02, far=1e6):
         _C._check(lib.gof_frustum_mask(N, p.data_ptr(), int(table.shape[0]), table.data_ptr(), float(near), float(far), mask.data_ptr(),
                                        _C._stream()))
     return mask
+
+
+# ---- the level set on a sparse voxel-block lattice, without tetrahedra (csrc/field_grid.cu, DESIGN §4.15) -----------------
+_GOF_E_INVALID = -1
+_MAX_LATTICE_POINTS = 2 ** 31
+
+
+class _GridParams(ctypes.Structure):
+    _fields_ = [("voxel_size", ctypes.c_float), ("block_resolution", ctypes.c_int)]
+
+
+def _grid_lib():
+    from diff_gaussian_rasterization import _C
+    lib, v, i64, P = _C._lib, ctypes.c_void_p, ctypes.c_int64, ctypes.POINTER(_GridParams)
+    i64p, f, a = ctypes.POINTER(ctypes.c_int64), ctypes.c_float, _C._ALLOC_FN
+    for name, args in (
+            ("gof_field_grid_blocks_count", [P, ctypes.c_int, v, v, v, ctypes.c_int, v, f, f, a, v, a, v, i64p, v]),
+            ("gof_field_grid_blocks_emit", [P, ctypes.c_int, v, v, i64, v, v]),
+            ("gof_field_grid_points", [P, i64, v, v, v]),
+            ("gof_field_grid_extract_count", [P, i64, v, v, a, v, i64p, i64p, v]),
+            ("gof_field_grid_extract_emit", [P, i64, v, v, v, i64, i64, v, v, v, v])):
+        getattr(lib, name).restype = ctypes.c_int
+        getattr(lib, name).argtypes = args
+    return _C, lib
+
+
+def _grid_check(_C, rc):
+    """A refusal of the lattice's limits (GOF_E_INVALID) as ValueError with the library's message; other failures as _C._check."""
+    if rc == _GOF_E_INVALID:
+        _C._ALLOC_ERROR.exc = None
+        raise ValueError(f"field grid: {_C._lib.gof_last_error().decode()}")
+    _C._check(rc)
+
+
+def _grid_params(voxel_size, block_resolution):
+    import numpy as np
+    B = int(block_resolution)
+    s = float(np.float32(voxel_size))
+    if not 1 <= B <= 64:
+        raise ValueError(f"field grid: block_resolution must be in 1..64, got {block_resolution}")
+    if not s > 0 or s == float("inf"):
+        raise ValueError(f"field grid: voxel_size must be a finite float32 > 0, got {voxel_size}")
+    return _GridParams(s, B)
+
+
+@torch.no_grad()
+def field_grid_blocks(xyz, scales_with_filter, rotation, views, voxel_size, block_resolution=8, near=0.02, far=1e6):
+    """Sorted unique int64 keys [n] of the voxel blocks (B^3 voxels of size voxel_size) touched by the Gaussians whose centre some
+    view's frustum holds (get_tetra_points' test): on each axis the blocks from floor((lo - s) / (B s)) to floor((hi + s) / (B s)),
+    lo / hi the extent of the Gaussian's eight 3-sigma box corners.  Keys pack block coordinates as the TSDF volume's
+    (gof_tsdf, DESIGN §4.4).  Inputs as get_tetra_points'."""
+    from gof_params import _f32
+    _C, lib = _grid_lib()
+    par = _grid_params(voxel_size, block_resolution)
+    x, s, q = _f32(xyz), _f32(scales_with_filter), _f32(rotation)
+    P = int(x.shape[0])
+    if tuple(x.shape) != (P, 3) or tuple(s.shape) != (P, 3) or tuple(q.shape) != (P, 4):
+        raise ValueError(f"field_grid_blocks: expected xyz [P,3], scales [P,3], rotation [P,4]; got {tuple(x.shape)}, "
+                         f"{tuple(s.shape)}, {tuple(q.shape)}")
+    table = pack_views(views, x.device)
+    gs, inst = _C._Scratch(x.device, "field_grid_gauss"), _C._Scratch(x.device, "field_grid_inst")
+    n = ctypes.c_int64(0)
+    with torch.cuda.device(x.device):
+        _grid_check(_C, lib.gof_field_grid_blocks_count(ctypes.byref(par), P, x.data_ptr(), s.data_ptr(), q.data_ptr(),
+                                                         int(table.shape[0]), table.data_ptr(), float(near), float(far), gs.cb, None,
+                                                         inst.cb, None, ctypes.byref(n), _C._stream()))
+        keys = torch.empty(n.value, dtype=torch.int64, device=x.device)
+        if n.value:
+            _grid_check(_C, lib.gof_field_grid_blocks_emit(ctypes.byref(par), P, gs.tensor.data_ptr(), inst.tensor.data_ptr(), n.value,
+                                                            keys.data_ptr(), _C._stream()))
+    return keys
+
+
+def _grid_keys(keys, who):
+    """Block keys as the kernels read them: a 1-D int64 tensor (they are read 8 bytes a key)."""
+    if not isinstance(keys, torch.Tensor) or keys.dtype != torch.int64 or keys.dim() != 1:
+        raise ValueError(f"{who}: keys must be a 1-D int64 tensor, got "
+                         f"{keys.dtype if isinstance(keys, torch.Tensor) else type(keys).__name__} "
+                         f"{tuple(keys.shape) if isinstance(keys, torch.Tensor) else ''}")
+    return keys
+
+
+def _grid_on_cuda(t, name, who, device=None):
+    """Refuses, before any launch, a tensor the kernels cannot read: on the host, or on another device than `device`."""
+    if not t.is_cuda:
+        raise RuntimeError(f"gof_b200 {who}: {name} must be a CUDA tensor (no CPU path), got one on {t.device}")
+    if device is not None and t.device != device:
+        raise RuntimeError(f"gof_b200 {who}: {name} on {t.device}, keys on {device}")
+
+
+def _check_lattice_size(num_blocks, block_resolution):
+    n = int(num_blocks) * int(block_resolution) ** 3
+    if n >= _MAX_LATTICE_POINTS:
+        raise ValueError(f"field grid: {num_blocks} blocks of {int(block_resolution) ** 3} voxels make {n} lattice points; the "
+                         f"opacity-field query takes fewer than 2^31 points (raise voxel_size)")
+
+
+@torch.no_grad()
+def field_grid_points(keys, voxel_size, block_resolution=8):
+    """The lattice points [n B^3, 3] of the blocks `keys` (CUDA int64 [n], as field_grid_blocks returns them), in pool order
+    (block, then voxel i + B j + B^2 k): voxel (x, y, z) = key B + (i, j, k) at (float(x) s, float(y) s, float(z) s), as the TSDF
+    volume places it."""
+    _C, lib = _grid_lib()
+    par = _grid_params(voxel_size, block_resolution)
+    _grid_keys(keys, "field_grid_points")
+    _check_lattice_size(keys.numel(), par.block_resolution)
+    _grid_on_cuda(keys, "keys", "field_grid_points")
+    pts = torch.empty((keys.numel() * par.block_resolution ** 3, 3), dtype=torch.float32, device=keys.device)
+    if keys.numel():
+        k = keys.contiguous()
+        with torch.cuda.device(keys.device):
+            _grid_check(_C, lib.gof_field_grid_points(ctypes.byref(par), k.numel(), k.data_ptr(), pts.data_ptr(), _C._stream()))
+    return pts
+
+
+@torch.no_grad()
+def field_grid_marching_cubes(keys, values, voxel_size, block_resolution=8):
+    """Marching cubes of `values` (float32 [n B^3], pool order, the level already subtracted) on the lattice of `keys` (CUDA int64
+    [n], sorted, as field_grid_blocks returns them; values on the same device), with the TSDF extraction's table, winding
+    (normals towards increasing value) and canonical order; a cube is meshed iff its eight corners lie in listed blocks.  Returns (edge_points [V,2,3], edge_values [V,2], faces [F,3] int64): every vertex as its lattice edge, the
+    owner voxel's point and value first, then those of owner + axis."""
+    _C, lib = _grid_lib()
+    par = _grid_params(voxel_size, block_resolution)
+    who = "field_grid_marching_cubes"
+    _grid_keys(keys, who)
+    n, dev = int(keys.numel()), keys.device
+    _check_lattice_size(n, par.block_resolution)
+    if not isinstance(values, torch.Tensor) or tuple(values.shape) != (n * par.block_resolution ** 3,) or values.dtype != torch.float32:
+        raise ValueError(f"{who}: values must be a float32 tensor [{n * par.block_resolution ** 3}], got "
+                         f"{getattr(values, 'dtype', type(values).__name__)} {tuple(getattr(values, 'shape', ()))}")
+    _grid_on_cuda(keys, "keys", who)
+    _grid_on_cuda(values, "values", who, device=dev)
+    k, v = keys.contiguous(), values.contiguous()
+    scratch = _C._Scratch(dev)
+    nv, nf = ctypes.c_int64(0), ctypes.c_int64(0)
+    with torch.cuda.device(dev):
+        _grid_check(_C, lib.gof_field_grid_extract_count(ctypes.byref(par), n, k.data_ptr() if n else None, v.data_ptr() if n else None,
+                                                          scratch.cb, None, ctypes.byref(nv), ctypes.byref(nf), _C._stream()))
+        ep = torch.empty((nv.value, 2, 3), dtype=torch.float32, device=dev)
+        ev = torch.empty((nv.value, 2), dtype=torch.float32, device=dev)
+        faces = torch.empty((nf.value, 3), dtype=torch.int64, device=dev)
+        if nv.value or nf.value:
+            _grid_check(_C, lib.gof_field_grid_extract_emit(ctypes.byref(par), n, k.data_ptr(), v.data_ptr(), scratch.tensor.data_ptr(),
+                                                             nv.value, nf.value, ep.data_ptr(), ev.data_ptr(), faces.data_ptr(),
+                                                             _C._stream()))
+    return ep, ev, faces
+
+
+@torch.no_grad()
+def extract_level_set_grid(xyz, scales_with_filter, rotation, views, integrate_fn, voxel_size, block_resolution=8, n_binary_steps=8,
+                           near=0.02, far=1e6, group=None, return_color=False, return_normals=False, timings=None):
+    """The 0.5 level set of evaluate_alpha's field (1 - min over views of the integrated opacity) as a mesh, without Delaunay
+    tetrahedra: the field is sampled on the voxel lattice (size voxel_size, blocks of block_resolution^3 voxels) of the blocks the
+    Gaussians' 3-sigma boxes touch (field_grid_blocks), meshed by marching cubes on alpha - 0.5 (field_grid_marching_cubes), and
+    every vertex is bisected `n_binary_steps` times on its lattice edge (binary_search), as extract_level_set does on the
+    tetrahedra's edges.  Inputs: get_tetra_points' (get_xyz, get_scaling_with_3D_filter, the raw _rotation), the views, and the
+    integrate_fn (a CachedIntegrator for return_normals) that extract_level_set takes.
+
+    Returns dict(vertices (E,3), faces (F,3) int64, colors (E,3) or None); return_color: evaluate_alpha's colour at the vertices;
+    return_normals: also "normals" (E,3), grad alpha / |grad alpha| from field_gradient ((0, 0, 0) where the gradient is zero),
+    outward for GOF's field, with the colours from the same pass.  With torch.distributed initialised the field is view-sharded
+    over the ranks of `group` as evaluate_alpha shards it; the blocks and marching cubes are deterministic and run on every rank,
+    so every rank returns the same mesh.  ValueError for a bad voxel_size or block_resolution, a block outside [-2^20, 2^20) per
+    axis, 2^30 or more (Gaussian, block) pairs, or a lattice of 2^31 points or more.  `timings` (dict): seconds per stage."""
+    import time as _time
+
+    def tick(name, t0):
+        if timings is not None:
+            torch.cuda.synchronize()
+            timings[name] = timings.get(name, 0.0) + (_time.perf_counter() - t0)
+
+    t0 = _time.perf_counter()
+    keys = field_grid_blocks(xyz, scales_with_filter, rotation, views, voxel_size, block_resolution, near, far)
+    tick("blocks_s", t0)
+    t0 = _time.perf_counter()
+    points = field_grid_points(keys, voxel_size, block_resolution)
+    tick("lattice_s", t0)
+    t0 = _time.perf_counter()
+    sdf = evaluate_alpha(points, views, integrate_fn, group=group) - 0.5
+    del points
+    tick("evaluate_alpha_lattice_s", t0)
+    t0 = _time.perf_counter()
+    end_points, end_sdf, faces = field_grid_marching_cubes(keys, sdf, voxel_size, block_resolution)
+    del sdf
+    tick("marching_cubes_s", t0)
+    t0 = _time.perf_counter()
+    verts = binary_search(end_points, end_sdf.unsqueeze(-1), lambda p: evaluate_alpha(p, views, integrate_fn, group=group),
+                          n_steps=n_binary_steps)
+    tick("binary_search_s", t0)
+    colors = None
+    if return_normals:
+        t0 = _time.perf_counter()
+        _a, grad, *rest = field_gradient(verts, views, integrate_fn, return_color=return_color, group=group)
+        colors = rest[0] if return_color else None
+        norm = grad.norm(dim=1, keepdim=True)
+        normals = torch.where(norm > 0, grad / torch.where(norm > 0, norm, torch.ones_like(norm)), torch.zeros_like(grad))
+        tick("field_gradient_s", t0)
+        return {"vertices": verts, "faces": faces, "colors": colors, "normals": normals}
+    if return_color:
+        t0 = _time.perf_counter()
+        _a, colors = evaluate_alpha(verts, views, integrate_fn, return_color=True, group=group)
+        tick("evaluate_alpha_colors_s", t0)
+    return {"vertices": verts, "faces": faces, "colors": colors}

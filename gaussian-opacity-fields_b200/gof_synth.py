@@ -99,6 +99,11 @@ class SurfaceView(NamedTuple):
     focal_x: float
     gt_alpha_mask: object = None
 
+    @property
+    def focal_y(self):
+        """H / (2 tan(fovy / 2)), as the reference's Camera derives it: the frustum test of get_tetra_points reads it."""
+        return self.image_height / (2.0 * self.tanfovy)
+
 
 def make_surface_views(width, height, n_views, radius=4.0, fovx_deg=60.0, max_elevation=1.2, znear=0.01, zfar=100.0):
     """`n_views` cameras looking at the origin from rings of make_camera at elevations spread over

@@ -365,6 +365,41 @@ GOF_API int gof_tsdf_extract_emit(const gof_tsdf_params_t* params, int64_t num_t
                                   int64_t num_vertices, int64_t num_faces, float* vertices, float* colors, int64_t* faces,
                                   void* stream);
 
+/* The opacity field's level set on a sparse voxel-block lattice (csrc/field_grid.cu and csrc/tsdf.cu, DESIGN section 4.15):
+ * the blocks the Gaussians touch, their lattice points, and marching cubes of the field's values there.  Block keys pack as
+ * the TSDF's; a touched block outside [-2^20, 2^20) per axis fails with GOF_E_INVALID.  voxel_size > 0, block_resolution
+ * 1..64, or GOF_E_INVALID. */
+typedef struct {
+  float voxel_size;       /* s */
+  int block_resolution;   /* B, 1..64 */
+} gof_field_grid_params_t;
+/* Blocks: every Gaussian whose centre lies in some view's frustum (gof_tetra_points' test: views [n_views,20], near, far,
+ * width and height of views[0]) touches, on each axis, the blocks floor(fl(lo - s) / fl(B s)) .. floor(fl(hi + s) / fl(B s)),
+ * lo / hi the min / max of its eight 3-sigma box corners (gof_tetra_points' corners).  count returns the number of sorted
+ * unique keys, emit writes them.  Two scratch buffers: one per Gaussian (gauss_alloc), one per touched (Gaussian, block)
+ * instance (inst_alloc); emit takes both.  GOF_E_INVALID: P < 0, 9P > 2^32 - 1, n_views < 1, misaligned rotations, a block
+ * out of range, or 2^30 or more instances. */
+GOF_API int gof_field_grid_blocks_count(const gof_field_grid_params_t* params, int P, const float* xyz, const float* scales,
+                                        const float* rotations, int n_views, const float* views, float near, float far,
+                                        gof_alloc_fn gauss_alloc, void* gauss_user, gof_alloc_fn inst_alloc, void* inst_user,
+                                        int64_t* num_blocks_out, void* stream);
+GOF_API int gof_field_grid_blocks_emit(const gof_field_grid_params_t* params, int P, void* gauss_scratch, void* inst_scratch,
+                                       int64_t num_blocks, int64_t* keys_out, void* stream);
+/* Lattice points [num_blocks * B^3][3] in pool order (block, then voxel i + B j + B^2 k): voxel (x, y, z) = key * B + (i, j, k)
+ * at (fl(x) s, fl(y) s, fl(z) s), as the TSDF volume places it.  GOF_E_INVALID for 2^31 points or more. */
+GOF_API int gof_field_grid_points(const gof_field_grid_params_t* params, int64_t num_blocks, const int64_t* keys, float* points,
+                                  void* stream);
+/* Marching cubes of values [num_blocks][B^3] (pool order; the field minus the level) with the TSDF extraction's table, winding
+ * and canonical order; a cube is meshed iff its eight corners lie in listed blocks.  emit writes, per vertex, its edge:
+ * edge_points [V][2][3] (the owner voxel's lattice point, then the one at owner + axis) and edge_values [V][2] their values;
+ * and faces [F][3] int64. */
+GOF_API int gof_field_grid_extract_count(const gof_field_grid_params_t* params, int64_t num_blocks, const int64_t* keys,
+                                         const float* values, gof_alloc_fn scratch_alloc, void* scratch_user,
+                                         int64_t* num_vertices_out, int64_t* num_faces_out, void* stream);
+GOF_API int gof_field_grid_extract_emit(const gof_field_grid_params_t* params, int64_t num_blocks, const int64_t* keys,
+                                        const float* values, void* scratch, int64_t num_vertices, int64_t num_faces,
+                                        float* edge_points, float* edge_values, int64_t* faces, void* stream);
+
 /* Launch accounting and live per-kernel timing (CUDA events on the launching stream; not a profiler).
  * gof_launch_count(): kernels launched by this library so far.  gof_profile_report(): lines of
  * "<kernel> <launches> <total_ms>" accumulated while profiling was enabled. */
