@@ -197,7 +197,7 @@ void gof_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* gof_last_error(void) { return g_err; }
-extern "C" int gof_version(void) { return 103; }
+extern "C" int gof_version(void) { return 104; }
 
 static int validate_scene(const gof_scene_t* s) {
   if (!s) { gof_set_error("scene is NULL"); return GOF_E_INVALID; }

@@ -167,10 +167,8 @@ __global__ void __launch_bounds__(256) k_emit_faces(const EmitArgs a) {
 }  // namespace
 
 extern "C" __attribute__((visibility("default")))
-int gof_marching_tets_count(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, int64_t chunk_tets,
-                            gof_alloc_fn scratch_alloc, void* scratch_user, int64_t* num_edges_out, int64_t* num_faces_out,
-                            void* stream) {
-  (void)chunk_tets;
+int gof_marching_tets_count(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, gof_alloc_fn scratch_alloc,
+                            void* scratch_user, int64_t* num_edges_out, int64_t* num_faces_out, void* stream) {
   if (!num_edges_out || !num_faces_out || !scratch_alloc) { gof_set_error("marching_tets_count: NULL argument"); return GOF_E_INVALID; }
   *num_edges_out = 0; *num_faces_out = 0;
   if (num_tets <= 0) return GOF_OK;
@@ -218,11 +216,14 @@ int gof_marching_tets_count(int num_verts, const float* sdf, int64_t num_tets, c
 }
 
 extern "C" __attribute__((visibility("default")))
-int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, int64_t chunk_tets, void* scratch,
-                           int64_t num_edges, int64_t num_faces, int64_t* interp_v, int64_t* faces, const float* vertices,
-                           const float* scales, float* edge_pos, float* edge_sdf, float* edge_scales, void* stream) {
+int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, int64_t rows_per_chunk,
+                           void* scratch, int64_t num_edges, int64_t num_faces, int64_t* interp_v, int64_t* faces,
+                           const float* vertices, const float* scales, float* edge_pos, float* edge_sdf, float* edge_scales,
+                           void* stream) {
   (void)num_verts;
-  if (num_tets <= 0 || (num_edges == 0 && num_faces == 0)) return GOF_OK;
+  if (num_tets <= 0) return GOF_OK;
+  if (rows_per_chunk <= 0) { gof_set_error("marching_tets_emit: rows_per_chunk must be positive"); return GOF_E_INVALID; }
+  if (num_edges == 0 && num_faces == 0) return GOF_OK;
   if (!scratch || !tets || !sdf || (num_edges > 0 && !interp_v) || (num_faces > 0 && !faces)) {
     gof_set_error("marching_tets_emit: NULL argument");
     return GOF_E_INVALID;
@@ -239,12 +240,7 @@ int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, co
     return GOF_E_INVALID;
   }
   EmitArgs a{};
-  // rows per chunk: the reference splits with torch.chunk(tets, T // chunk_size + 1) (utils/tetmesh.py:56-58), i.e. ceil(T / n)
-  // rows; a NEGATIVE chunk_tets states the rows per chunk directly (tet-sharded extraction: every shard must cut where the
-  // unsharded call cuts)
-  a.T = num_tets;
-  if (chunk_tets < 0) a.chunk = -chunk_tets;
-  else a.chunk = (chunk_tets > 0 && num_tets > chunk_tets) ? (num_tets + (num_tets / chunk_tets + 1) - 1) / (num_tets / chunk_tets + 1) : num_tets;
+  a.T = num_tets; a.chunk = rows_per_chunk;
   a.tets = tets; a.code = (unsigned char*)(S + L.code);
   a.cross_off = (uint32_t*)(S + L.cross_off); a.f1_off = (uint32_t*)(S + L.f1_off); a.f2_off = (uint32_t*)(S + L.f2_off);
   a.inst_uid = (uint32_t*)(S + L.inst_uid); a.lo = (uint32_t*)(S + L.lo); a.hi = (uint32_t*)(S + L.hi);

@@ -23,7 +23,10 @@ reference's extract_mesh.py, restated with view sharding over the GPUs of one bo
 * extract_level_set_grid -- the same level set without tetrahedra: the field sampled on a sparse voxel-block lattice around
                        the Gaussians, marching cubes, the same bisection, colours and normals (csrc/field_grid.cu, DESIGN §4.15).
 """
+import contextlib
 import ctypes
+import functools
+import time
 
 import torch
 import torch.distributed as dist
@@ -36,6 +39,18 @@ def _world(group=None):
     if dist.is_available() and dist.is_initialized():
         return dist.get_rank(group), dist.get_world_size(group)
     return 0, 1
+
+
+def _views_of_rank(views, rank, world):
+    """The (index, view) pairs of `views` that `rank` of `world` processes in the view-sharded passes: views[rank::world]."""
+    views = list(views)
+    for vi in range(rank, len(views), world):
+        yield vi, views[vi]
+
+
+def _owns_view(vi, rank, world):
+    """Whether view index vi (an int or a tensor of them) is one that _views_of_rank gives `rank`."""
+    return vi % world == rank
 
 
 def _merge_minimum(alpha_min, argmin, rows, group):
@@ -66,9 +81,8 @@ def evaluate_alpha(points, views, integrate_fn, return_color=False, group=None):
     final_alpha = torch.ones(n, dtype=torch.float32, device=dev)
     final_color = torch.ones(n, 3, dtype=torch.float32, device=dev) if return_color else None
     best_view = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev) if return_color else None
-    views = list(views)
-    for vi in range(rank, len(views), world):
-        alpha_integrated, color_integrated = integrate_fn(points, views[vi])
+    for vi, view in _views_of_rank(views, rank, world):
+        alpha_integrated, color_integrated = integrate_fn(points, view)
         if return_color:
             better = alpha_integrated < final_alpha
             final_color = torch.where(better.reshape(-1, 1), color_integrated, final_color)
@@ -146,8 +160,8 @@ class _OpacityField(torch.autograd.Function):
         argmin = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev)
         color = torch.ones(n, 3, dtype=torch.float32, device=dev) if return_color else None
         views = list(views)
-        for vi in range(rank, len(views), world):
-            rs = settings_for_view(views[vi])
+        for vi, view in _views_of_rank(views, rank, world):
+            rs = settings_for_view(view)
             args = _field_args(rs, points, means3D, opacities, scales, rotations, shs) + (vi, alpha_min, argmin)
             dgr._call_native(_C.integrate_gaussians_to_points_min, args, rs.debug, "snapshot_fw.dump", "forward",
                              **({"color_min": color} if return_color else {}))
@@ -195,7 +209,7 @@ class _OpacityField(torch.autograd.Function):
         g_pts, g_means, g_scales, g_rot = g_pts.view(n, 3), g_means.view(P, 3), g_scales.view(P, 3), g_rot.view(P, 4)
         if n and P:
             colors, scales_, rotations_, cov3D, v2g, shs_ = _field_inputs(scales, rotations, shs)
-            mine = torch.nonzero((argmin != _NO_VIEW) & (argmin % world == rank)).flatten()
+            mine = torch.nonzero((argmin != _NO_VIEW) & _owns_view(argmin, rank, world)).flatten()
             order = mine[torch.argsort(argmin[mine], stable=True)]
             won, counts = torch.unique_consecutive(argmin[order], return_counts=True)
             start = 0
@@ -321,9 +335,8 @@ def field_gradient(points, views, integrate_fn, return_color=False, group=None):
     argmin = torch.full((n,), _NO_VIEW, dtype=torch.int32, device=dev)
     grad_min = torch.zeros(n, 3, dtype=torch.float32, device=dev)
     color = torch.ones(n, 3, dtype=torch.float32, device=dev) if return_color else None
-    views = list(views)
-    for vi in range(rank, len(views), world):
-        integrate_fn.min_update(points, views[vi], vi, alpha_min, argmin, color_min=color, grad_min=grad_min)
+    for vi, view in _views_of_rank(views, rank, world):
+        integrate_fn.min_update(points, view, vi, alpha_min, argmin, color_min=color, grad_min=grad_min)
     if world > 1:
         # the winner's gradient and colour rows in one [N,6] block, summed in a single all-reduce
         rows = torch.cat([grad_min, color], 1) if return_color else grad_min
@@ -369,28 +382,20 @@ def shard_tet_range(num_tets, rows, rank, world):
     return min(c0 * rows, num_tets), min(c1 * rows, num_tets)
 
 
-def _reference_chunk_rows(num_tets, chunk_tets):
-    if chunk_tets <= 0 or num_tets <= chunk_tets:
-        return max(int(num_tets), 1)
-    n = num_tets // chunk_tets + 1
-    return -(-num_tets // n)
-
-
 @torch.no_grad()
 def marching_tetrahedra_sharded(vertices, tets, sdf, scales, group=None, chunk_tets=None, extract_fn=None):
     """`gof_tetmesh.marching_tetrahedra` for ONE batch element with the tets sharded by chunk over the ranks of `group`:
-    each rank extracts its chunks, ONE all-gather exchanges the crossing-edge keys and the faces (as edge keys), every rank
-    ends with the complete mesh -- bit-identical to the unsharded call (faces are ordered per chunk, so shards are whole
-    chunks of the unsharded split; with fewer chunks than ranks some ranks idle).  vertices (N,3), tets (T,4), sdf (N,),
+    each rank extracts its chunks, ONE all-gather exchanges the crossing-edge keys and the faces, merge_tet_shards merges them,
+    and every rank ends with the complete mesh -- bit-identical to the unsharded call (faces are ordered per chunk, so shards
+    are whole chunks of the unsharded split; with fewer chunks than ranks some ranks idle).  vertices (N,3), tets (T,4), sdf (N,),
     scales (N,1).  World size 1: the plain call.  `extract_fn(vertices, tets, sdf, scales, rows=...)` defaults to the CUDA
     implementation (tests pass the oracle)."""
+    import gof_tetmesh
     if extract_fn is None:
-        import gof_tetmesh
         extract_fn = lambda v, t, s, sc, rows: gof_tetmesh._unbatched_marching_tetrahedra(v, t, s, sc, rows=rows)   # noqa: E731
-    chunk = int(chunk_tets or 32 * 1024 * 1024)    # utils/tetmesh.py:55
     rank, world = _world(group)
     T = int(tets.shape[0])
-    rows = _reference_chunk_rows(T, chunk)
+    rows = gof_tetmesh.chunk_rows(T, int(chunk_tets or gof_tetmesh.CHUNK_TETS))
     if world == 1:
         return extract_fn(vertices, tets, sdf, scales, rows)
     b, e = shard_tet_range(T, rows, rank, world)
@@ -404,22 +409,49 @@ def marching_tetrahedra_sharded(vertices, tets, sdf, scales, group=None, chunk_t
     all_sizes = [torch.zeros_like(sizes) for _ in range(world)]
     dist.all_gather(all_sizes, sizes, group=group)
     nk, nf = max(int(s[0]) for s in all_sizes), max(int(s[1]) for s in all_sizes)
-    # one padded all-gather carries both the keys and the faces (as global keys: renumbering then needs no second exchange)
-    face_keys = keys[faces.reshape(-1)] if faces.numel() else torch.zeros(0, dtype=torch.int64, device=dev)
+    # one padded all-gather carries both the keys and the faces: a shard's faces index its own keys, which travel with them
     payload = torch.full((nk + 3 * nf,), -1, dtype=torch.int64, device=dev)
     payload[:keys.numel()] = keys
-    payload[nk:nk + face_keys.numel()] = face_keys
+    payload[nk:nk + faces.numel()] = faces.reshape(-1)
     gathered = [torch.empty_like(payload) for _ in range(world)]
     dist.all_gather(gathered, payload, group=group)
     shard_keys = [g[:int(s[0])] for g, s in zip(gathered, all_sizes)]
-    union = torch.unique(torch.cat(shard_keys))
-    faces_all = torch.cat([torch.searchsorted(union, g[nk:nk + 3 * int(s[1])]).reshape(-1, 3) for g, s in zip(gathered, all_sizes)])
-    interp = torch.stack([union >> 32, union & 0xFFFFFFFF], dim=1)
-    v = vertices.reshape(-1, 3)
-    edge_pos = v[interp.reshape(-1)].reshape(-1, 2, 3)
-    edge_sdf = sdf.reshape(-1)[interp.reshape(-1)].reshape(-1, 2, 1)
-    edge_scales = scales.reshape(-1)[interp.reshape(-1)].reshape(-1, 2, 1)
-    return (edge_pos, edge_sdf), edge_scales, faces_all, interp
+    shard_faces = [g[nk:nk + 3 * int(s[1])].reshape(-1, 3) for g, s in zip(gathered, all_sizes)]
+    return merge_tet_shards(vertices, sdf, scales, shard_keys, shard_faces)
+
+
+def _stopwatch(timings, cuda):
+    """stage(name): a context that adds its seconds to timings[name], after a device synchronise when `cuda`; nothing without
+    `timings`."""
+    @contextlib.contextmanager
+    def stage(name):
+        t0 = time.perf_counter()
+        yield
+        if timings is not None:
+            if cuda:
+                torch.cuda.synchronize()
+            timings[name] = timings.get(name, 0.0) + (time.perf_counter() - t0)
+    return stage
+
+
+def _refine(end_points, end_sdf, views, integrate_fn, n_steps, group, return_color, return_normals, stage):
+    """The vertices of both extractions: `n_steps` bisection steps of every edge (end_points (E,2,3), end_sdf (E,2,1)) onto the
+    0.5 level set, then, with return_normals, the unit normals and the colours from one field_gradient pass, or with
+    return_color alone evaluate_alpha's colours.  Returns (vertices (E,3), colours (E,3) or None, normals (E,3) or None)."""
+    with stage("binary_search_s"):
+        verts = binary_search(end_points, end_sdf, lambda p: evaluate_alpha(p, views, integrate_fn, group=group), n_steps=n_steps)
+    colors = normals = None
+    if return_normals:
+        with stage("field_gradient_s"):
+            _a, grad, *rest = field_gradient(verts, views, integrate_fn, return_color=return_color, group=group)
+            colors = rest[0] if return_color else None
+            norm = grad.norm(dim=1, keepdim=True)
+            # alpha = 1 - (the opacity min_v alpha_integrated) rises from ~0 inside the surface to ~1 outside it, so grad alpha points out
+            normals = torch.where(norm > 0, grad / torch.where(norm > 0, norm, torch.ones_like(norm)), torch.zeros_like(grad))
+    elif return_color:
+        with stage("evaluate_alpha_colors_s"):
+            _a, colors = evaluate_alpha(verts, views, integrate_fn, return_color=True, group=group)
+    return verts, colors, normals
 
 
 @torch.no_grad()
@@ -432,53 +464,59 @@ def extract_level_set(points, points_scale, tets, views, integrate_fn, n_binary_
     return_normals=True (integrate_fn a CachedIntegrator) also returns "normals" (E,3): the field's outward unit normal at each
     vertex, grad alpha / |grad alpha| = -grad o / |grad o| for the opacity o = 1 - alpha, (0, 0, 0) where the gradient is zero,
     from one field_gradient pass that also gives the colours (DESIGN.md 4.14)."""
-    import time as _time
-
-    def tick(name, t0):
-        if timings is not None:
-            torch.cuda.synchronize() if points.is_cuda else None
-            timings[name] = timings.get(name, 0.0) + (_time.perf_counter() - t0)
-
-    t0 = _time.perf_counter()
-    alpha = evaluate_alpha(points, views, integrate_fn, group=group)
-    tick("evaluate_alpha_vertices_s", t0)
-    t0 = _time.perf_counter()
-    (end_points, end_sdf), end_scales, faces, _iv = marching_tetrahedra_sharded(points, tets, alpha - 0.5, points_scale, group=group,
-                                                                             chunk_tets=chunk_tets)
-    tick("marching_tetrahedra_s", t0)
+    stage = _stopwatch(timings, points.is_cuda)
+    with stage("evaluate_alpha_vertices_s"):
+        alpha = evaluate_alpha(points, views, integrate_fn, group=group)
+    with stage("marching_tetrahedra_s"):
+        (end_points, end_sdf), end_scales, faces, _iv = marching_tetrahedra_sharded(points, tets, alpha - 0.5, points_scale, group=group,
+                                                                                 chunk_tets=chunk_tets)
     distance = torch.norm(end_points[:, 0, :] - end_points[:, 1, :], dim=-1)
     scale = end_scales[:, 0, 0] + end_scales[:, 1, 0]
-    t0 = _time.perf_counter()
-    verts = binary_search(end_points, end_sdf, lambda p: evaluate_alpha(p, views, integrate_fn, group=group), n_steps=n_binary_steps)
-    tick("binary_search_s", t0)
-    colors = None
+    verts, colors, normals = _refine(end_points, end_sdf, views, integrate_fn, n_binary_steps, group, return_color, return_normals,
+                                     stage)
+    out = {"vertices": verts, "faces": faces, "mask": distance <= scale, "colors": colors}
     if return_normals:
-        t0 = _time.perf_counter()
-        _a, grad, *rest = field_gradient(verts, views, integrate_fn, return_color=return_color, group=group)
-        colors = rest[0] if return_color else None
-        norm = grad.norm(dim=1, keepdim=True)
-        # alpha = 1 - (the opacity min_v alpha_integrated) rises from ~0 inside the surface to ~1 outside it, so grad alpha points out
-        normals = torch.where(norm > 0, grad / torch.where(norm > 0, norm, torch.ones_like(norm)), torch.zeros_like(grad))
-        tick("field_gradient_s", t0)
-        return {"vertices": verts, "faces": faces, "mask": distance <= scale, "colors": colors, "normals": normals}
-    if return_color:
-        t0 = _time.perf_counter()
-        _a, colors = evaluate_alpha(verts, views, integrate_fn, return_color=True, group=group)
-        tick("evaluate_alpha_colors_s", t0)
-    return {"vertices": verts, "faces": faces, "mask": distance <= scale, "colors": colors}
+        out["normals"] = normals
+    return out
 
 
-# ---- the tetrahedra points and their multi-view frustum mask (csrc/tetra_points.cu) ---------------------------------------
+# ---- the entry points of the tetrahedra points and the field grid (csrc/tetra_points.cu, csrc/field_grid.cu) -------------
+class _GridParams(ctypes.Structure):
+    _fields_ = [("voxel_size", ctypes.c_float), ("block_resolution", ctypes.c_int)]
+
+
+@functools.cache
 def _tetra_lib():
+    """(_C, its library) with the signatures of the tetra-point and field-grid entry points declared, on first use: gof_extract
+    itself imports without the library."""
     from diff_gaussian_rasterization import _C
-    lib, v = _C._lib, ctypes.c_void_p
-    lib.gof_tetra_points.restype = ctypes.c_int
-    lib.gof_tetra_points.argtypes = [ctypes.c_int, v, v, v, ctypes.c_int, v, ctypes.c_float, ctypes.c_float, v, v, v, v]
-    lib.gof_frustum_mask.restype = ctypes.c_int
-    lib.gof_frustum_mask.argtypes = [ctypes.c_int64, v, ctypes.c_int, v, ctypes.c_float, ctypes.c_float, v, v]
+    lib, v, i32, i64, f, a = _C._lib, ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, _C._ALLOC_FN
+    P, i64p = ctypes.POINTER(_GridParams), ctypes.POINTER(ctypes.c_int64)
+    for name, args in (
+            ("gof_tetra_points", [i32, v, v, v, i32, v, f, f, v, v, v, v]),
+            ("gof_frustum_mask", [i64, v, i32, v, f, f, v, v]),
+            ("gof_field_grid_blocks_count", [P, i32, v, v, v, i32, v, f, f, a, v, a, v, i64p, v]),
+            ("gof_field_grid_blocks_emit", [P, i32, v, v, i64, v, v]),
+            ("gof_field_grid_points", [P, i64, v, v, v]),
+            ("gof_field_grid_extract_count", [P, i64, v, v, a, v, i64p, i64p, v]),
+            ("gof_field_grid_extract_emit", [P, i64, v, v, v, i64, i64, v, v, v, v])):
+        getattr(lib, name).restype = ctypes.c_int
+        getattr(lib, name).argtypes = args
     return _C, lib
 
 
+def _gaussian_inputs(xyz, scales_with_filter, rotation, who):
+    """get_tetra_points' inputs as the kernels read them: contiguous CUDA float32 xyz [P,3], scales [P,3], rotation [P,4]."""
+    from gof_params import _f32
+    x, s, q = _f32(xyz), _f32(scales_with_filter), _f32(rotation)
+    P = int(x.shape[0])
+    if tuple(x.shape) != (P, 3) or tuple(s.shape) != (P, 3) or tuple(q.shape) != (P, 4):
+        raise ValueError(f"{who}: expected xyz [P,3], scales [P,3], rotation [P,4]; got {tuple(x.shape)}, "
+                         f"{tuple(s.shape)}, {tuple(q.shape)}")
+    return x, s, q
+
+
+# ---- the tetrahedra points and their multi-view frustum mask (csrc/tetra_points.cu) ---------------------------------------
 def pack_views(views, device):
     """[n,20] float32 table of gof_tetra_points / gof_frustum_mask from objects with the reference Camera's attributes
     (world_view_transform, focal_x, focal_y, image_width, image_height; scene/cameras.py).  The scalars are rounded to float32
@@ -498,13 +536,9 @@ def get_tetra_points(xyz, scales_with_filter, rotation, views, near=0.02, far=1e
     they are normalised here as build_rotation does).  Returns (points [M,3], points_scale [M,1]): the 8 corners of every
     Gaussian's 3-sigma box, then the centres, kept where some view's frustum holds them.  Width and height come from views[0]
     for every view, as in the reference."""
-    from gof_params import _f32
     _C, lib = _tetra_lib()
-    x, s, q = _f32(xyz), _f32(scales_with_filter), _f32(rotation)
+    x, s, q = _gaussian_inputs(xyz, scales_with_filter, rotation, "get_tetra_points")
     P = int(x.shape[0])
-    if tuple(x.shape) != (P, 3) or tuple(s.shape) != (P, 3) or tuple(q.shape) != (P, 4):
-        raise ValueError(f"get_tetra_points: expected xyz [P,3], scales [P,3], rotation [P,4]; got {tuple(x.shape)}, "
-                         f"{tuple(s.shape)}, {tuple(q.shape)}")
     table = pack_views(views, x.device)
     pts = torch.empty((9 * P, 3), dtype=torch.float32, device=x.device)
     sc = torch.empty((9 * P, 1), dtype=torch.float32, device=x.device)
@@ -538,25 +572,6 @@ _GOF_E_INVALID = -1
 _MAX_LATTICE_POINTS = 2 ** 31
 
 
-class _GridParams(ctypes.Structure):
-    _fields_ = [("voxel_size", ctypes.c_float), ("block_resolution", ctypes.c_int)]
-
-
-def _grid_lib():
-    from diff_gaussian_rasterization import _C
-    lib, v, i64, P = _C._lib, ctypes.c_void_p, ctypes.c_int64, ctypes.POINTER(_GridParams)
-    i64p, f, a = ctypes.POINTER(ctypes.c_int64), ctypes.c_float, _C._ALLOC_FN
-    for name, args in (
-            ("gof_field_grid_blocks_count", [P, ctypes.c_int, v, v, v, ctypes.c_int, v, f, f, a, v, a, v, i64p, v]),
-            ("gof_field_grid_blocks_emit", [P, ctypes.c_int, v, v, i64, v, v]),
-            ("gof_field_grid_points", [P, i64, v, v, v]),
-            ("gof_field_grid_extract_count", [P, i64, v, v, a, v, i64p, i64p, v]),
-            ("gof_field_grid_extract_emit", [P, i64, v, v, v, i64, i64, v, v, v, v])):
-        getattr(lib, name).restype = ctypes.c_int
-        getattr(lib, name).argtypes = args
-    return _C, lib
-
-
 def _grid_check(_C, rc):
     """A refusal of the lattice's limits (GOF_E_INVALID) as ValueError with the library's message; other failures as _C._check."""
     if rc == _GOF_E_INVALID:
@@ -582,14 +597,10 @@ def field_grid_blocks(xyz, scales_with_filter, rotation, views, voxel_size, bloc
     view's frustum holds (get_tetra_points' test): on each axis the blocks from floor((lo - s) / (B s)) to floor((hi + s) / (B s)),
     lo / hi the extent of the Gaussian's eight 3-sigma box corners.  Keys pack block coordinates as the TSDF volume's
     (gof_tsdf, DESIGN §4.4).  Inputs as get_tetra_points'."""
-    from gof_params import _f32
-    _C, lib = _grid_lib()
+    _C, lib = _tetra_lib()
     par = _grid_params(voxel_size, block_resolution)
-    x, s, q = _f32(xyz), _f32(scales_with_filter), _f32(rotation)
+    x, s, q = _gaussian_inputs(xyz, scales_with_filter, rotation, "field_grid_blocks")
     P = int(x.shape[0])
-    if tuple(x.shape) != (P, 3) or tuple(s.shape) != (P, 3) or tuple(q.shape) != (P, 4):
-        raise ValueError(f"field_grid_blocks: expected xyz [P,3], scales [P,3], rotation [P,4]; got {tuple(x.shape)}, "
-                         f"{tuple(s.shape)}, {tuple(q.shape)}")
     table = pack_views(views, x.device)
     gs, inst = _C._Scratch(x.device, "field_grid_gauss"), _C._Scratch(x.device, "field_grid_inst")
     n = ctypes.c_int64(0)
@@ -633,7 +644,7 @@ def field_grid_points(keys, voxel_size, block_resolution=8):
     """The lattice points [n B^3, 3] of the blocks `keys` (CUDA int64 [n], as field_grid_blocks returns them), in pool order
     (block, then voxel i + B j + B^2 k): voxel (x, y, z) = key B + (i, j, k) at (float(x) s, float(y) s, float(z) s), as the TSDF
     volume places it."""
-    _C, lib = _grid_lib()
+    _C, lib = _tetra_lib()
     par = _grid_params(voxel_size, block_resolution)
     _grid_keys(keys, "field_grid_points")
     _check_lattice_size(keys.numel(), par.block_resolution)
@@ -652,7 +663,7 @@ def field_grid_marching_cubes(keys, values, voxel_size, block_resolution=8):
     [n], sorted, as field_grid_blocks returns them; values on the same device), with the TSDF extraction's table, winding
     (normals towards increasing value) and canonical order; a cube is meshed iff its eight corners lie in listed blocks.  Returns (edge_points [V,2,3], edge_values [V,2], faces [F,3] int64): every vertex as its lattice edge, the
     owner voxel's point and value first, then those of owner + axis."""
-    _C, lib = _grid_lib()
+    _C, lib = _tetra_lib()
     par = _grid_params(voxel_size, block_resolution)
     who = "field_grid_marching_cubes"
     _grid_keys(keys, who)
@@ -695,42 +706,20 @@ def extract_level_set_grid(xyz, scales_with_filter, rotation, views, integrate_f
     over the ranks of `group` as evaluate_alpha shards it; the blocks and marching cubes are deterministic and run on every rank,
     so every rank returns the same mesh.  ValueError for a bad voxel_size or block_resolution, a block outside [-2^20, 2^20) per
     axis, 2^30 or more (Gaussian, block) pairs, or a lattice of 2^31 points or more.  `timings` (dict): seconds per stage."""
-    import time as _time
-
-    def tick(name, t0):
-        if timings is not None:
-            torch.cuda.synchronize()
-            timings[name] = timings.get(name, 0.0) + (_time.perf_counter() - t0)
-
-    t0 = _time.perf_counter()
-    keys = field_grid_blocks(xyz, scales_with_filter, rotation, views, voxel_size, block_resolution, near, far)
-    tick("blocks_s", t0)
-    t0 = _time.perf_counter()
-    points = field_grid_points(keys, voxel_size, block_resolution)
-    tick("lattice_s", t0)
-    t0 = _time.perf_counter()
-    sdf = evaluate_alpha(points, views, integrate_fn, group=group) - 0.5
-    del points
-    tick("evaluate_alpha_lattice_s", t0)
-    t0 = _time.perf_counter()
-    end_points, end_sdf, faces = field_grid_marching_cubes(keys, sdf, voxel_size, block_resolution)
-    del sdf
-    tick("marching_cubes_s", t0)
-    t0 = _time.perf_counter()
-    verts = binary_search(end_points, end_sdf.unsqueeze(-1), lambda p: evaluate_alpha(p, views, integrate_fn, group=group),
-                          n_steps=n_binary_steps)
-    tick("binary_search_s", t0)
-    colors = None
+    stage = _stopwatch(timings, xyz.is_cuda)
+    with stage("blocks_s"):
+        keys = field_grid_blocks(xyz, scales_with_filter, rotation, views, voxel_size, block_resolution, near, far)
+    with stage("lattice_s"):
+        points = field_grid_points(keys, voxel_size, block_resolution)
+    with stage("evaluate_alpha_lattice_s"):
+        sdf = evaluate_alpha(points, views, integrate_fn, group=group) - 0.5
+        del points
+    with stage("marching_cubes_s"):
+        end_points, end_sdf, faces = field_grid_marching_cubes(keys, sdf, voxel_size, block_resolution)
+        del sdf
+    verts, colors, normals = _refine(end_points, end_sdf.unsqueeze(-1), views, integrate_fn, n_binary_steps, group, return_color,
+                                     return_normals, stage)
+    out = {"vertices": verts, "faces": faces, "colors": colors}
     if return_normals:
-        t0 = _time.perf_counter()
-        _a, grad, *rest = field_gradient(verts, views, integrate_fn, return_color=return_color, group=group)
-        colors = rest[0] if return_color else None
-        norm = grad.norm(dim=1, keepdim=True)
-        normals = torch.where(norm > 0, grad / torch.where(norm > 0, norm, torch.ones_like(norm)), torch.zeros_like(grad))
-        tick("field_gradient_s", t0)
-        return {"vertices": verts, "faces": faces, "colors": colors, "normals": normals}
-    if return_color:
-        t0 = _time.perf_counter()
-        _a, colors = evaluate_alpha(verts, views, integrate_fn, return_color=True, group=group)
-        tick("evaluate_alpha_colors_s", t0)
-    return {"vertices": verts, "faces": faces, "colors": colors}
+        out["normals"] = normals
+    return out

@@ -17,8 +17,8 @@ from diff_gaussian_rasterization import _C
 
 _lib = _C._lib
 _lib.gof_marching_tets_count.restype = ctypes.c_int
-_lib.gof_marching_tets_count.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, _C._ALLOC_FN,
-                                         ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p]
+_lib.gof_marching_tets_count.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, _C._ALLOC_FN, ctypes.c_void_p,
+                                         ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p]
 _lib.gof_marching_tets_emit.restype = ctypes.c_int
 _lib.gof_marching_tets_emit.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
                                         ctypes.c_int64, ctypes.c_int64] + [ctypes.c_void_p] * 7 + [ctypes.c_void_p]
@@ -27,7 +27,8 @@ CHUNK_TETS = 32 * 1024 * 1024   # utils/tetmesh.py:55
 
 
 def chunk_rows(num_tets, chunk_tets=CHUNK_TETS):
-    """Rows per chunk of the reference's split: torch.chunk(tets, T // chunk_size + 1) (utils/tetmesh.py:56-58)."""
+    """Rows per chunk of the reference's split: torch.chunk(tets, T // chunk_size + 1) when T > chunk_size (utils/tetmesh.py:55-58),
+    else one chunk; chunk_tets <= 0 also means one chunk.  The CUDA face order takes these rows (gof_marching_tets_emit)."""
     if chunk_tets <= 0 or num_tets <= chunk_tets:
         return max(int(num_tets), 1)
     n = num_tets // chunk_tets + 1
@@ -35,9 +36,8 @@ def chunk_rows(num_tets, chunk_tets=CHUNK_TETS):
 
 
 def _unbatched_marching_tetrahedra(vertices, tets, sdf, scales, chunk_tets=CHUNK_TETS, rows=None):
-    """`rows`: rows per chunk stated directly (overrides the reference's rule applied to chunk_tets; see gof_extract)."""
-    if rows is not None:
-        chunk_tets = -int(rows)
+    """`rows`: rows per chunk stated directly, in place of chunk_rows(T, chunk_tets) (gof_extract's tet shards cut where the
+    unsharded call cuts)."""
     if not (vertices.is_cuda and tets.is_cuda and sdf.is_cuda and scales.is_cuda):
         raise RuntimeError("gof_b200 marching_tetrahedra: CUDA tensors required (no CPU path)")
     dev = vertices.device
@@ -46,11 +46,12 @@ def _unbatched_marching_tetrahedra(vertices, tets, sdf, scales, chunk_tets=CHUNK
     s = sdf.contiguous().float().reshape(-1)
     sc = scales.contiguous().float().reshape(-1)
     V, T = int(v.shape[0]), int(t.shape[0])
+    rows = int(rows) if rows is not None else chunk_rows(T, chunk_tets)
     scratch = _C._Scratch(dev, "tets")
     nE, nF = ctypes.c_int64(0), ctypes.c_int64(0)
     with torch.cuda.device(dev):
-        _C._check(_lib.gof_marching_tets_count(V, s.data_ptr(), T, t.data_ptr() if T else None, chunk_tets, scratch.cb, None,
-                                               ctypes.byref(nE), ctypes.byref(nF), _C._stream()))
+        _C._check(_lib.gof_marching_tets_count(V, s.data_ptr(), T, t.data_ptr() if T else None, scratch.cb, None, ctypes.byref(nE),
+                                               ctypes.byref(nF), _C._stream()))
         E, F = nE.value, nF.value
         interp_v = torch.empty((E, 2), dtype=torch.long, device=dev)
         faces = torch.empty((F, 3), dtype=torch.long, device=dev)
@@ -58,7 +59,7 @@ def _unbatched_marching_tetrahedra(vertices, tets, sdf, scales, chunk_tets=CHUNK
         edge_sdf = torch.empty((E, 2, 1), dtype=torch.float32, device=dev)
         edge_scales = torch.empty((E, 2, 1), dtype=torch.float32, device=dev)
         if T and (E or F):
-            _C._check(_lib.gof_marching_tets_emit(V, s.data_ptr(), T, t.data_ptr(), chunk_tets, scratch.tensor.data_ptr(), E, F,
+            _C._check(_lib.gof_marching_tets_emit(V, s.data_ptr(), T, t.data_ptr(), rows, scratch.tensor.data_ptr(), E, F,
                                                   interp_v.data_ptr() if E else None, faces.data_ptr() if F else None, v.data_ptr(),
                                                   sc.data_ptr(), edge_pos.data_ptr() if E else None, edge_sdf.data_ptr() if E else None,
                                                   edge_scales.data_ptr() if E else None, _C._stream()))

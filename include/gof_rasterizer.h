@@ -303,16 +303,16 @@ GOF_API int gof_export_state(int P, int width, int height, int num_rendered,
 /* Marching tetrahedra, utils/tetmesh.py:47-138 (_unbatched_marching_tetrahedra), as CUDA.
  * Two phases because the output sizes are data dependent: `count` classifies the tets, emits and sorts the crossing
  * edges and returns the number of unique crossing edges E and of faces F on the host; `emit` then fills
- * caller-allocated outputs.  `chunk_tets` reproduces the reference's chunked face order (its chunk_size of
- * 32*1024*1024, tetmesh.py:55: the tets are cut into T / chunk_tets + 1 pieces of ceil(T / pieces) rows); pass 0 for "one
- * chunk", or a NEGATIVE value -r to state r rows per chunk directly (used when the tets are sharded over ranks: every shard
- * must cut where the unsharded call cuts).  tets: [T,4] int64 vertex ids < 2^32.  Outputs:
- * interp_v [E,2] int64 (sorted unique crossing edges), faces [F,3] int64; optional gathers of the edge endpoints:
+ * caller-allocated outputs.  `rows_per_chunk` (> 0 when num_tets > 0, else GOF_E_INVALID) sets the face order: the faces
+ * come chunk by chunk of that many tets, as in the reference's chunk loop (tetmesh.py:55-58 cuts the T tets into
+ * T / (32*1024*1024) + 1 pieces of ceil(T / pieces) rows; gof_tetmesh.chunk_rows states that rule).  A caller that shards the
+ * tets passes the rows of the unsharded call, so that every shard cuts where it cuts.  tets: [T,4] int64 vertex ids < 2^32.
+ * Outputs: interp_v [E,2] int64 (sorted unique crossing edges), faces [F,3] int64; optional gathers of the edge endpoints:
  * edge_pos [E,2,3] from vertices [V,3], edge_sdf [E,2], edge_scales [E,2] from scales [V] (any may be NULL). */
-GOF_API int gof_marching_tets_count(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, int64_t chunk_tets,
+GOF_API int gof_marching_tets_count(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets,
                                     gof_alloc_fn scratch_alloc, void* scratch_user,
                                     int64_t* num_edges_out, int64_t* num_faces_out, void* stream);
-GOF_API int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, int64_t chunk_tets,
+GOF_API int gof_marching_tets_emit(int num_verts, const float* sdf, int64_t num_tets, const int64_t* tets, int64_t rows_per_chunk,
                                    void* scratch, int64_t num_edges, int64_t num_faces,
                                    int64_t* interp_v /* [E,2] */, int64_t* faces /* [F,3] */,
                                    const float* vertices, const float* scales,

@@ -111,9 +111,10 @@ def _golden_chunked():
 def test_merge_of_tet_shards_equals_reference_chunked_output():
     """Shards cut at the chunk boundaries of the unsharded call, extracted independently and merged by
     gof_extract.merge_tet_shards, reproduce the reference's own chunked output (golden from utils/tetmesh.py) bit for bit."""
+    import gof_tetmesh
     g, chunk = _golden_chunked()
     T = g["tets"].shape[0]
-    rows = gof_extract._reference_chunk_rows(T, chunk)
+    rows = gof_tetmesh.chunk_rows(T, chunk)
     assert rows == -(-T // (T // chunk + 1))
     for world in (1, 2, 3, 4, 7):
         keys, faces = [], []

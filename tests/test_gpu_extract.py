@@ -156,7 +156,6 @@ def test_tet_sharded_marching_tetrahedra_equals_unsharded():
     v, tets, sdf, sc = v.to(dev), tets.to(dev), sdf.to(dev), sc.to(dev)
     (pos0, sdf0), sc0, f0, iv0 = gof_tetmesh._unbatched_marching_tetrahedra(v, tets, sdf, sc, chunk_tets=chunk)
     rows = gof_tetmesh.chunk_rows(T, chunk)
-    assert rows == gof_extract._reference_chunk_rows(T, chunk)
     for world in (2, 3, 8):
         keys, faces = [], []
         for r in range(world):

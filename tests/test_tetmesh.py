@@ -31,6 +31,21 @@ def test_oracle_matches_reference(path):
     np.testing.assert_array_equal(esc, z["edge_scales"])
 
 
+def test_chunk_rows_is_the_reference_split():
+    """gof_tetmesh.chunk_rows, the rows per chunk that set the face order of the CUDA implementation, cuts the tets as
+    utils/tetmesh.py:55-58 does: torch.chunk(tets, T // chunk_size + 1) when T > chunk_size, else one chunk.  chunk_tets = 0:
+    one chunk."""
+    import gof_tetmesh
+    for chunk in (1, 7, 1000, gof_tetmesh.CHUNK_TETS):
+        for T in sorted({k * chunk + d for k in (1, 2, 3, 10) for d in (-1, 0, 1)} - {0}):
+            tets = torch.empty((T, 0))        # the split depends on the row count alone
+            want = torch.chunk(tets, T // chunk + 1) if T > chunk else (tets,)
+            got = torch.split(tets, gof_tetmesh.chunk_rows(T, chunk))
+            assert [t.shape[0] for t in got] == [t.shape[0] for t in want], (T, chunk)
+    for T in (1, 7, 1000, 3 * gof_tetmesh.CHUNK_TETS + 1):
+        assert gof_tetmesh.chunk_rows(T, 0) == T
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("path", FIX, ids=[os.path.basename(p) for p in FIX])
 def test_cuda_matches_reference_golden(path):
