@@ -5,8 +5,9 @@
 // rank holds all means and can learn every rank's camera centre, so the ranks only need each other's dL_dRGB: 3 floats per
 // Gaussian and view instead of an all-reduce over 48.  This kernel forms sum_v w(dir_v) (x) rgb_v for all views v, in rank
 // order and with the products rounded before the additions -- bit-identical to adding the per-view dL_dsh tensors that
-// k_preprocess_backward would have written (it evaluates the same gof_sh_grad_weights).  The view records are read through
-// a pointer per view: local memory after an NCCL all-gather, or the peers' buckets themselves over NVLink.
+// k_preprocess_backward would have written (it evaluates the same gof_sh_grad_weights), except that a zero sum is always +0
+// (the accumulator starts at +0; an all-zero record row cannot say whether the view wrote +0 or -0).  The view records are
+// read through a pointer per view: local memory after an NCCL all-gather, or the peers' buckets themselves over NVLink.
 #include "gof_common.cuh"
 #include "gof_math.cuh"
 
