@@ -29,6 +29,10 @@ struct PlanArgs {
   uint32_t* flags;          // [4][P]: kept original | clone | split child 1 | split child 2
 };
 
+// A split child's raw scaling, scaling_inverse_activation(get_scaling / (0.8 * N)) with N = 2 (gaussian_model.py:649): torch
+// divides a CUDA tensor by a Python scalar as a product with the scalar's float reciprocal, and 1 / 1.6f rounds to 0.625f.
+__device__ __forceinline__ float child_raw_scaling(float s) { return logf(s * 0.625f); }
+
 __global__ void __launch_bounds__(256) k_densify_plan(const PlanArgs a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.P) return;
@@ -36,13 +40,16 @@ __global__ void __launch_bounds__(256) k_densify_plan(const PlanArgs a) {
   if (g != g) g = 0.f;                                   // grads[grads.isnan()] = 0.0
   if (ga != ga) ga = 0.f;
   const bool sel = (g >= a.max_grad) || (ga >= a.abs_threshold);
-  const float smax = fmaxf(fmaxf(expf(a.scaling[3 * i]), expf(a.scaling[3 * i + 1])), expf(a.scaling[3 * i + 2]));
+  const float s0 = expf(a.scaling[3 * i]), s1 = expf(a.scaling[3 * i + 1]), s2 = expf(a.scaling[3 * i + 2]);
+  const float smax = fmaxf(fmaxf(s0, s1), s2);
   const bool clone = sel && smax <= a.dense_extent;
   const bool split = sel && smax > a.dense_extent;
   const float op = 1.0f / (1.0f + expf(-a.opacity[i]));
   const bool low = op < a.min_opacity;
   const bool prune_self = low || (a.prune_scale > 0.f && smax > a.prune_scale);
-  const bool prune_child = low || (a.prune_scale > 0.f && smax / 1.6f > a.prune_scale);   // children carry scaling / (0.8 * 2)
+  // a child is pruned on the scale it is stored with, read back: exp(log(s * 0.625f)), which can differ from s / 1.6f
+  const bool prune_child = low || (split && a.prune_scale > 0.f &&
+                                   fmaxf(fmaxf(expf(child_raw_scaling(s0)), expf(child_raw_scaling(s1))), expf(child_raw_scaling(s2))) > a.prune_scale);
   a.flags[i] = (!split && !prune_self) ? 1u : 0u;
   a.flags[(size_t)a.P + i] = (clone && !prune_self) ? 1u : 0u;
   const uint32_t c = (split && !prune_child) ? 1u : 0u;
@@ -126,8 +133,8 @@ __global__ void __launch_bounds__(256) k_densify_emit(const EmitArgs a) {
       nx = px + R[0] * v0 + R[1] * v1 + R[2] * v2;
       ny = py + R[3] * v0 + R[4] * v1 + R[5] * v2;
       nz = pz + R[6] * v0 + R[7] * v1 + R[8] * v2;
-      if (k >= 2) {   // scaling_inverse_activation(get_scaling / (0.8 * N)), N = 2
-        ns0 = logf(s0 / 1.6f); ns1 = logf(s1 / 1.6f); ns2 = logf(s2 / 1.6f);
+      if (k >= 2) {
+        ns0 = child_raw_scaling(s0); ns1 = child_raw_scaling(s1); ns2 = child_raw_scaling(s2);
       }
     }
     a.new_xyz[3 * (size_t)o] = nx; a.new_xyz[3 * (size_t)o + 1] = ny; a.new_xyz[3 * (size_t)o + 2] = nz;
